@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- BASELINE.json metric: audio frames/sec (22.05 kHz) of the generator forward.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one generator forward over one synthetic batch of config 2 (B=64 mel segments of
 80 x 32 frames -> 64 x 8192 audio frames) per GPU.  1 audio frame = 1 PCM sample; 1 mel frame = 256
@@ -17,7 +17,10 @@ audio frames (SURVEY 8d).  Weights are seeded random-init (melgan_multi_b200.syn
              per-forward weight-norm included, all host threads) on the FULL config-2 batch, a bounded
              number of iterations, median; rank 0 at N=1 only.
   --impl reference   times that same CPU port as the reference arm at the same config (the reference is pure
-             Python and /root/reference does not exist on the GPU box); value from the MEDIAN step.
+             Python); value from the MEDIAN step.
+  --dump-outputs DIR  after the timed steps, writes the audio the timed path returned in its LAST step (rank r of N > 1:
+             audio_rank<r>.npy) as DIR/audio.npy, float32 [B, 1, 256 T]; the inputs are seeded, so two builds run with the
+             same arguments can be compared output for output.
 """
 import argparse
 import ctypes
@@ -61,7 +64,8 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained"), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA's H100 SXM data sheet: HBM3 bandwidth and dense BF16 tensor rate of a 700 W card (not reached figures)
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": None, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -192,7 +196,7 @@ def cpu_port_steps(n_steps, warmup, budget_s=None):
 
 def run_reference(args):
     """Reference arm: the reference's CPU implementation of the path (PyTorch-CPU restatement of models.py:61-71 with the
-    per-forward weight-norm hooks), same config as the B200 arm: the full B=64 batch per step."""
+    per-forward weight-norm hooks), same config as the GPU arm: the full B=64 batch per step."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -302,7 +306,8 @@ def multi_gpu_blocks(dev, rank, world, barrier, max_over_ranks, steps=10, warmup
     gbytes, dbytes = fg_.flat.numel() * 4, fd_.flat.numel() * 4
     exposed = max(0.0, ddp_ms - dry_ms)
     out["ddp_train_step"] = {
-        "config": "configs[3]: DDP train step batch=16/gpu, 8192-sample segments, %d x B200, NCCL all-reduce" % world,
+        "config": "configs[3]: DDP train step batch=16/gpu, 8192-sample segments, %d x %s, NCCL all-reduce" % (
+            world, torch.cuda.get_device_name(dev)),
         "ms": ddp_ms, "ms_same_step_unwrapped_single_gpu": nocomm_ms, "ms_wrapped_without_the_collectives": dry_ms,
         "exposed_communication_ms": exposed,
         "allreduce_ms": bare_ms,
@@ -321,7 +326,7 @@ def multi_gpu_blocks(dev, rank, world, barrier, max_over_ranks, steps=10, warmup
                                "the generator's 18.1 MB bucket is launched when its (single-node) backward returns",
         "dedup": "discriminator gradients of the generator step (67.7 MB) are not reduced: learned at run time from the "
                  "optimizer/forward order, no train.py edit",
-        "steps": steps, "warmup": warmup, "dtype": "f32 (forwards: 3-pass split-bf16 tcgen05; backward: see DESIGN.md)",
+        "steps": steps, "warmup": warmup, "dtype": "f32 (forwards: 3-pass split-bf16 wgmma; backward: see DESIGN.md)",
     }
     del gen1, msd1, g1, d1
     # -- config 5 sharded along time
@@ -367,9 +372,10 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="h100", choices=["h100", "reference"])
     ap.add_argument("--cpu-budget", type=float, default=15.0, help="seconds of CPU-baseline timing")
     ap.add_argument("--no-multi", action="store_true", help="skip the DDP train-step / utterance-shard blocks at N > 1")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's audio to DIR/audio.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
@@ -415,7 +421,7 @@ def main():
             [to(state[n + ".bias"]) for n in order])
     mels = [to(synth.mel_input(B, T, 10 * rank + i)) for i in range(4)]
     out = torch.empty((B, 1, 256 * T), dtype=torch.float32, device=dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     sampler = ClockSampler(local_rank)
     for i in range(W):
@@ -430,6 +436,10 @@ def main():
         gd.forward(mels[k % 4], out)
         ev[k][1].record()
     barrier()
+    if args.dump_outputs:  # before the per-kernel pass below overwrites `out`
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "audio.npy" if world == 1 else "audio_rank%d.npy" % rank),
+                out.cpu().numpy().astype(np.float32))
     step_ms = [a.elapsed_time(b) for a, b in ev]
     total_ms = max_over_ranks(sum(step_ms))
     frames_per_step = B * T * 256 * world
@@ -479,36 +489,21 @@ def main():
     alg_bytes = ALG_BYTES_PER_FRAME * frames + ALG_WEIGHT_BYTES
     moved_bytes = (ALG_BYTES_PER_FRAME + extra) * frames + packed_bytes
     fwd_ms = total_ms / K
-    # dram bytes per launch of the dominant kernel from the committed `ncu --set full` capture -- quoted only if that capture
-    # was taken with the kernel configuration this build runs (profiles/r02_ncu_traffic.json records mg_gen_kernel_config)
-    traffic, traffic_note = None, None
+    # the configuration of the dominant kernel (what a kernel-level measurement of it must record)
     L_ = engine.lib()
     L_.mg_gen_kernel_config.restype = ctypes.c_char_p
     L_.mg_gen_kernel_config.argtypes = [ctypes.c_int, ctypes.c_int]
     cfg_now = L_.mg_gen_kernel_config(dom, T).decode()
-    tpath = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-    if os.path.exists(tpath):
-        t = json.load(open(tpath)).get(dom_name)
-        if t and t.get("kernel_config") == cfg_now:
-            traffic = t["dram_read_bytes"] + t["dram_write_bytes"]
-            traffic_note = ("dram__bytes_read.sum + dram__bytes_write.sum of one launch, ncu --set full of this kernel configuration "
-                            "(profiles/r02_ncu_traffic.json, %.1f us under ncu); algorithmic HBM bytes of this kernel: 2 * 64*128*2048*4 "
-                            "= 134.2 MB (the 126 MB L2 keeps part of the output)" % t["gpu_time_us"])
-        else:
-            traffic_note = ("STALE CAPTURE IGNORED: profiles/r02_ncu_traffic.json holds %r for %s, this build runs %r -- re-run "
-                            "scripts/gpu_profile_r02.sh" % (t.get("kernel_config") if t else None, dom_name, cfg_now))
-            print("bench.py: " + traffic_note, file=sys.stderr)
-    else:
-        traffic_note = "no ncu capture committed for this build"
+    traffic, traffic_note = None, "not measured (no DRAM counters in this run)"
     roofline = {
         "kernel": ("resblock_tc_kernel<C=128> (%s: stage-1 ResBlock, 6 k3 convs%s; %.0f%% of generator FLOPs)" % (
             dom_name, " + stage-2 ConvTranspose at its tail" if "+" in dom_name else "", 100.0 * k_flops[dom] / sum(k_flops))),
         "bound": "tensor", "achieved": dom_tflops, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
         "frac": dom_tflops / peaks["bf16_tflops"], "traffic": traffic,
         "traffic_note": traffic_note, "kernel_config": cfg_now,
-        "peak_source": "%s bf16 dense burst (MEASURED_PEAKS.json)" % peaks["source"],
+        "peak_source": "bf16 dense, %s" % peaks["source"],
         "algorithmic_flops_per_launch": k_flops[dom], "avg_launch_ms": float(kms[dom]),
-        "math": ("split-bf16 tcgen05: 3 MMA passes per product, so tensor-pipe work is 3x the algorithmic FLOPs "
+        "math": ("split-bf16 wgmma: 3 MMA passes per product, so tensor-pipe work is 3x the algorithmic FLOPs "
                  "(pipe-level fraction = 3 * frac)"),
         "kernel_ms": {n: float(v) for n, v in zip(names, kms)},
         "kernel_tflops": {n: k_flops[i] / (kms[i] * 1e-3) / 1e12 for i, n in enumerate(names)},
@@ -517,7 +512,8 @@ def main():
                 "algorithmic_bytes_per_forward": alg_bytes, "moved_bytes_per_forward_by_design": moved_bytes,
                 "wasted_traffic_ratio": moved_bytes / alg_bytes,
                 "note": "whole forward, SURVEY 8(d) bytes (152 896 B/frame + 18.08 MB weights); the fused generator is "
-                        "683 FLOP/B, i.e. math-bound: 60 % of HBM peak would need 2.5 PFLOP/s (SURVEY 8d)"},
+                        "683 FLOP/B, i.e. math-bound: 60 %% of HBM peak would need %.2f PFLOP/s" % (
+                            0.6 * peaks["hbm_gbs"] * 1e9 * 683 / 1e15)},
         "forward_tflops": fwd_flops / (fwd_ms * 1e-3) / 1e12,
     }
 
@@ -554,7 +550,7 @@ def main():
         emit(({
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W,
             "ms_per_step": total_ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "f32 in/out; products as 3 split-bf16 tcgen05 passes with fp32 accumulation (fp32-equivalent, ~1e-5)",
+            "dtype": "f32 in/out; products as 3 split-bf16 wgmma passes with fp32 accumulation (fp32-equivalent, ~1e-5)",
             "data": "synthetic",
             "config": {"workload": WORKLOAD, "batch_per_gpu": B, "mel_frames": T, "global_batch": B * world,
                        "parallelism": "dp%d (independent batches, no collective)" % world,

@@ -1,5 +1,5 @@
 /*
- * melgan_b200.h -- C ABI of the B200-native MelGAN engine (libmelgan_b200.so).
+ * melgan_b200.h -- C ABI of the native (sm_90a, H100) MelGAN engine (libmelgan_b200.so).
  *
  * The reference (diver-j/melgan-multi) has no FFI or operator registry: its boundary for the
  * hot path is the torch.nn.Module protocol of models.py, imported by name at train.py:13
@@ -43,7 +43,7 @@ int mg_abi_version(void);
 /* Message describing the last failure on the calling thread ("" if none). */
 const char *mg_last_error_string(void);
 
-/* 0 if the current CUDA device can run the sm_100a kernels, MG_ERR_UNSUPPORTED_DEVICE /
+/* 0 if the current CUDA device can run the sm_90a kernels (an H100), MG_ERR_UNSUPPORTED_DEVICE /
  * MG_ERR_CUDA otherwise.  There is no CPU fallback anywhere in this library. */
 int mg_device_check(void);
 
@@ -91,11 +91,11 @@ int mg_gen_check_status(const void *workspace, int B, int T, void *stream);
 
 /* LeakyReLU -> ConvTranspose1d (models.py:64-65, ups[stage], models.py:48-51) on the tensor-core path:
  * x [B, 512>>stage, Lin] -> y [B, 256>>stage, S*Lin] (S = 8, 8, 2, 2), device fp32, x != y.  Synchronous;
- * parity-test entry point for the tcgen05 ConvT kernel. */
+ * parity-test entry point for the tensor-core ConvT kernel. */
 int mg_gen_convt(const void *packed, int stage, const float *x, float *y, int B, int Lin, void *stream);
 
 /* One ResBlock (models.py:32-40) of stage `stage` (C = 256 >> stage channels) on the tensor-core path:
- * x, y [B, C, L] device fp32, x != y.  Synchronous; parity-test entry point for the tcgen05 kernel. */
+ * x, y [B, C, L] device fp32, x != y.  Synchronous; parity-test entry point for the tensor-core kernel. */
 int mg_gen_resblock(const void *packed, int stage, const float *x, float *y, int B, int L, void *stream);
 /* Stage 2 or 3 as the pipeline runs it: LeakyReLU -> ConvTranspose1d(k4, s2) -> ResBlock in ONE kernel
  * (models.py:64-66); x [B][2C][Lin] is the previous stage's output, y [B][C][2 Lin] (C = 64 / 32).  Synchronous, like
@@ -115,7 +115,7 @@ int mg_gen_conv_pre(const void *packed, const float *mel, float *y, int B, int T
 int mg_gen_resblock_post(const void *packed, const float *x, float *audio, int B, int L, void *stream);
 
 /* Diagnostic twin of mg_gen_resblock: also returns 128 clock64 stamps (host buffer) of one interior CTA's
- * epilogue and MMA roles (slot meaning documented at the definition in csrc/mg_api.cu). */
+ * hand-off and MMA phases (slot meaning documented at the definition in csrc/mg_api.cu). */
 int mg_gen_resblock_trace(const void *packed, int stage, const float *x, float *y, int B, int L, long long *trace_host);
 
 /* Debug/parity tap: copies the activation after stage `which` (0 = conv_pre output [B,512,T],
@@ -217,11 +217,11 @@ int mg_msd_grouped_backward(const void *packed, int scale, int layer, const floa
                             float *db, void *workspace, size_t workspace_bytes, int Bt, int Lin, int Lout, void *stream);
 
 /* Data gradient of conv_post1 (Conv1d 1024 -> 1024, k5, pad 2; models.py:84,96) of discriminator `scale`: dz [Bt][1024][L]
- * -> dx [Bt][1024][L], on the same tcgen05 kernel as the forward, streaming the transposed, tap-flipped copy of the weights
+ * -> dx [Bt][1024][L], on the same tensor-core kernel as the forward, streaming the transposed, tap-flipped copy of the weights
  * that mg_msd_pack / mg_disc_pack keep for it. */
 int mg_msd_post1_dgrad(const void *packed, int scale, const float *dz, float *dx, int Bt, int L, void *status_word, void *stream);
 /* Weight and bias gradient of conv_post1 (no weights needed): x [Bt][1024][L], dz [Bt][1024][L] -> dw [1024][1024][5],
- * db [1024]; one tcgen05 launch, split-bf16 (fp32-grade) with fp32 accumulation over all Bt * L positions. */
+ * db [1024]; one tensor-core launch, split-bf16 (fp32-grade) with fp32 accumulation over all Bt * L positions. */
 int mg_msd_post1_wgrad(const float *x, const float *dz, float *dw, float *db, int Bt, int L, void *status_word, void *stream);
 
 /* Backward of conv_pre (layer 0: Conv1d 1 -> 16, k15; x [Bt][1][L], dz [Bt][16][L], dw [16][1][15]) or conv_post2 (layer 6:

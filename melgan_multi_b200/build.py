@@ -1,4 +1,4 @@
-"""In-tree build of libmelgan_b200.so (sm_100a only) with nvcc.  No JIT, no torch extension:
+"""In-tree build of libmelgan_b200.so (sm_90a only) with nvcc.  No JIT, no torch extension:
 the library is a plain C-ABI shared object loaded through ctypes (melgan_multi_b200/engine.py)."""
 import os
 import shutil
@@ -14,7 +14,7 @@ LIB = os.path.join(LIBDIR, "libmelgan_b200.so")
 TEST_LIB = os.path.join(LIBDIR, "libmelgan_b200_simt_test.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "-shared",
     "-cudart", "static",
 ]

@@ -61,8 +61,8 @@ int mg_device_check(void) {
     MG_CUDA_TRY(cudaGetDevice(&dev));
     cudaDeviceProp p;
     MG_CUDA_TRY(cudaGetDeviceProperties(&p, dev));
-    if (p.major != 10)
-        return set_error(MG_ERR_UNSUPPORTED_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a (B200) only",
+    if (p.major != 9 || p.minor != 0)
+        return set_error(MG_ERR_UNSUPPORTED_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a (H100) only",
                          dev, p.major, p.minor);
     return MG_OK;
 }
@@ -279,10 +279,10 @@ int mg_gen_resblock_post(const void *packed, const float *x, float *audio, int B
     });
 }
 
-/* Diagnostic: runs one tensor-core ResBlock and returns clock64 stamps of one interior CTA in trace[0..127]
- * (host buffer): [0] start, [1] input loaded, per conv c: [2+3c] X handed to MMA warp, [3+3c] accumulator ready,
- * [4+3c] next X written, [20] output stored; MMA thread: [64+3c] X received, [65+3c] first weights landed,
- * [66+3c] last MMA issued. */
+/* Diagnostic: runs one tensor-core ResBlock and returns clock64 stamps of thread 0 of one interior CTA in trace[0..127]
+ * (host buffer): [0] start, [1] input loaded, per conv c: [2+3c] X handed to the MMAs, [3+3c] accumulator ready,
+ * [4+3c] next X written, [20] output stored; the same thread's MMA issue: [64+3c] X received, [65+3c] first weights
+ * landed, [66+3c] last MMA issued. */
 int mg_gen_resblock_trace(const void *packed, int stage, const float *x, float *y, int B, int L, long long *trace_host) {
     if (!packed || !x || !y || x == y || !trace_host || stage < 0 || stage > 3)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_resblock_trace: bad argument");

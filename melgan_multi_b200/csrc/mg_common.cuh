@@ -10,6 +10,9 @@
 
 namespace mg {
 
+// streaming multiprocessors of the H100 SXM: grid sizes of the persistent-style kernels are multiples of it
+constexpr int kNumSMs = 132;
+
 // thread-local error string (the only mutable global state of the library)
 char *error_buffer();
 int set_error(int code, const char *fmt, ...);
@@ -34,26 +37,18 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
 
-// Launch helper of the tensor-core kernels: optional thread-block cluster (x dimension) and programmatic dependent launch
+// Launch helper of the tensor-core kernels: optional programmatic dependent launch
 // (mg_tc.cuh pdl_*; MG_PDL=0 in the environment turns the attribute off for A/B runs).
 bool pdl_enabled();
 template <class... KArgs, class... Args>
-inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, int cluster, bool pdl,
-                             Args... args) {
+inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl, Args... args) {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
-    cudaLaunchAttribute attr[2];
+    cudaLaunchAttribute attr[1];
     int n = 0;
-    if (cluster > 1) {
-        attr[n].id = cudaLaunchAttributeClusterDimension;
-        attr[n].val.clusterDim.x = cluster;
-        attr[n].val.clusterDim.y = 1;
-        attr[n].val.clusterDim.z = 1;
-        ++n;
-    }
     if (pdl && pdl_enabled()) {
         attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[n].val.programmaticStreamSerializationAllowed = 1;

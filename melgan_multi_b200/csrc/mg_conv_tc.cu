@@ -1,144 +1,153 @@
-// Stride-1 "same" Conv1d with a dense channel contraction on the tensor cores (tcgen05 + TMEM, split-bf16).
+// Stride-1 "same" Conv1d with a dense channel contraction on the tensor cores (wgmma, split-bf16).
 //
 // Used for   Generator.conv_pre      Conv1d(80 -> 512, k7, pad 3)                       models.py:46,62
 //            Discriminator.conv_post1 Conv1d(1024 -> 1024, k5, pad 2) + LeakyReLU       models.py:84,96-97
 //
 // GEMM view: D[v, co] = sum_tap sum_pass X_pass[v + tap - PAD, :] * W_pass[tap][co, :]^T with M = 128 virtual positions
-// (TMEM lane), N = 256 or 128 output channels, K = 16 per instruction.  Rows are VIRTUAL positions: the batch items are
-// concatenated with PAD zero rows after each item (v = item*(L+PAD) + s), so every tap -- the same A buffer read
-// `tap - PAD` rows further (row-linear operand layout, mg_tc.cuh) -- sees exactly the zero padding of the reference and
-// short sequences (L = 17..128 in the discriminators, 32 in the generator) still fill the 128-row MMA.
+// (two warpgroups of 64 rows), N = 128 output channels, K = 16 per instruction.  Rows are VIRTUAL positions: the
+// batch items are concatenated with PAD zero rows after each item (v = item*(L+PAD) + s), so every tap -- the same A
+// buffer read `tap - PAD` rows further (row-linear operand layout, mg_tc.cuh) -- sees exactly the zero padding of the
+// reference and short sequences (L = 17..128 in the discriminators, 32 in the generator) still fill the 128-row tile.
 // One CTA = 128 virtual positions x one group of N output channels; K = Cin is streamed: A slots (KCA channels, hi/lo
-// split of x, optional LeakyReLU on the way in) are produced by the converter warps straight from the fp32 NCL input,
-// B slots (one tap of 16 input channels: [hi, lo][k-panel][N][8] bf16 = 64 N bytes) arrive by 1-D bulk TMA.
+// split of x) are produced by the converter warps straight from the fp32 NCL input, B slots (one tap of 16 input
+// channels: [hi, lo][k-panel][N][8] bf16 = 64 N bytes) arrive by 1-D bulk TMA.
+// Warp roles: converter warpgroup (A slots), two MMA warpgroups (rows 0..63 / 64..127; accumulators in registers, they
+// also run the epilogue), one TMA producer warp.
 #include "mg_common.cuh"
 #include "mg_tc.cuh"
 
 namespace mg {
 using namespace tc;
 
-template <int CIN_, int COUT_, int NTAP_, int KCA_, bool LRELU_OUT_, int MINB_ = 1, int N_ = 256, int CL_ = 1>
+template <int CIN_, int COUT_, int NTAP_, int KCA_, bool LRELU_OUT_, int N_>
 struct ConvCfg {
-    // CL consecutive row tiles form a thread-block cluster: they stream the SAME weight slots (same output-channel group), so
-    // the leader's bulk copies are multicast into every CTA's ring and L2 is read once per cluster instead of once per tile
-    static constexpr int CL = CL_;
-    static constexpr int MINB = MINB_;                      // CTAs per SM the shared-memory footprint is sized for
     static constexpr int CIN = CIN_, COUT = COUT_, NTAP = NTAP_, PAD = NTAP_ / 2, KCA = KCA_;
     static constexpr bool LRELU_OUT = LRELU_OUT_;
-    static constexpr int N = N_;                            // output channels per CTA (= TMEM columns: 128 or 256)
+    static constexpr int N = N_;                            // output channels per CTA (MMA N)
     static constexpr int NCG = COUT / N;
     static constexpr int ROWS = 128;
     static constexpr int AROWS = ROWS + 2 * PAD + 2;        // row index i <-> virtual position r0 - PAD + i
     static constexpr int APITCH = AROWS * 16;
     static constexpr int ASLOT = 2 * (KCA / 8) * APITCH;    // [half][k-panel][AROWS][16 B]
     static constexpr int BSLOT = 2 * 2 * N * 16;            // [half][k-panel: 2][N][16 B]
-    // B ring: a CTA streams CIN/16 * NTAP slots and each is consumed in 3 MMAs (192-381 cycles), far less than a bulk copy's
+    // B ring: a CTA streams CIN/16 * NTAP slots and each is consumed in 3 MMAs per warpgroup, far less than a bulk copy's
     // latency, so the ring depth (bytes in flight) sets the pace: 8 x 8 KB for the N = 128 tiles, 4 x 16 KB for N = 256
     static constexpr int NSA = (CIN == KCA) ? 1 : 2, NSB = (N_ == 128) ? 8 : 4;
-    static constexpr int NCONV = 128;
-    static constexpr int NT = NCONV + 64;
-    static constexpr int SMEM_BYTES = NSA * ASLOT + NSB * BSLOT + (2 * NSA + 2 * NSB + 1) * 8 + 16;
+    static constexpr int NCONV = 128, NMW = 2;              // converter threads, MMA warpgroups
+    static constexpr int NT = NCONV + 128 * NMW + 32;
+    static constexpr int SMEM_BYTES = NSA * ASLOT + NSB * BSLOT + (2 * NSA + 2 * NSB) * 8;
     static_assert(CIN % KCA == 0 && KCA % 16 == 0 && COUT % N == 0, "shape");
-    static_assert(MINB * (SMEM_BYTES + 1024) <= 228 * 1024 && MINB * N <= 512, "shared memory / TMEM budget");
+    static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "shared memory budget");
 };
 
 // packed weights for this kernel: conv_tc_weight_index() in mg_layout.h
 
 template <class Cfg>
-__global__ void __launch_bounds__(Cfg::NT, Cfg::MINB)
+__global__ void __launch_bounds__(Cfg::NT, 1)
 conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const uint8_t *__restrict__ wtc,
                     const float *__restrict__ bias, int L, int B, int *__restrict__ status) {
     constexpr int CIN = Cfg::CIN, COUT = Cfg::COUT, NTAP = Cfg::NTAP, PAD = Cfg::PAD, KCA = Cfg::KCA, N = Cfg::N;
     constexpr int ROWS = Cfg::ROWS, APITCH = Cfg::APITCH, ASLOT = Cfg::ASLOT, BSLOT = Cfg::BSLOT;
-    constexpr int NSA = Cfg::NSA, NSB = Cfg::NSB, NCONV = Cfg::NCONV;
+    constexpr int NSA = Cfg::NSA, NSB = Cfg::NSB, NCONV = Cfg::NCONV, NMW = Cfg::NMW;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *aring = smem, *bring = smem + NSA * ASLOT;
     uint64_t *fullA = reinterpret_cast<uint64_t *>(bring + NSB * BSLOT);
-    uint64_t *emptyA = fullA + NSA, *fullB = emptyA + NSA, *emptyB = fullB + NSB, *done = emptyB + NSB;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(done + 1);
+    uint64_t *emptyA = fullA + NSA, *fullB = emptyA + NSA, *emptyB = fullB + NSB;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * ROWS, cg = blockIdx.y;
     const int Lv = L + PAD;  // virtual rows per item: L positions + PAD zero rows
 
-    if (warp == 0) tmem_alloc(tmem_slot, N);
-    if (tid == 32) {
-        for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], 1); }
-        for (int s = 0; s < NSB; ++s) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], Cfg::CL); }  // every CTA of the cluster frees a slot
-        mbar_init(done, 1);
+    if (tid == 0) {
+        for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NMW); }
+        for (int s = 0; s < NSB; ++s) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], NMW); }  // one arrival per MMA warpgroup
         fence_mbar_init();
     }
-    tc_fence_before();
     __syncthreads();
-    if constexpr (Cfg::CL > 1) cluster_sync();  // every CTA's barriers exist before a peer's copy or commit can land on them
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    constexpr uint16_t kClusterMask = (uint16_t)((1u << Cfg::CL) - 1);
 
-    if (warp == NCONV / 32) {
+    if (warp == (NCONV + 128 * NMW) / 32) {
         // ================= TMA producer: B slot = (16-channel chunk, tap) =================
-        // (cluster: every CTA arms its own full barrier; only the leader copies, into all the CTAs' rings at once)
         if (lane == 0) {
             const uint8_t *src = wtc + (size_t)cg * (CIN / 16) * NTAP * BSLOT;
-            const bool leader = Cfg::CL == 1 || cluster_ctarank() == 0;
             int s = 0, ph = 0;
             bool ok = true;
             for (int i = 0; i < (CIN / 16) * NTAP && ok; ++i) {
                 if (!mbar_wait(&emptyB[s], ph ^ 1)) { ok = false; break; }
                 mbar_arrive_expect_tx(&fullB[s], BSLOT);
-                if constexpr (Cfg::CL > 1) {
-                    if (leader) bulk_g2s_multicast(bring + s * BSLOT, src + (size_t)i * BSLOT, BSLOT, &fullB[s], kClusterMask);
-                } else {
-                    bulk_g2s(bring + s * BSLOT, src + (size_t)i * BSLOT, BSLOT, &fullB[s]);
-                }
+                bulk_g2s(bring + s * BSLOT, src + (size_t)i * BSLOT, BSLOT, &fullB[s]);
                 if (++s == NSB) { s = 0; ph ^= 1; }
             }
             if (!ok) atomicExch(status, 22);
         }
-    } else if (warp == NCONV / 32 + 1) {
-        // ================= MMA issuer (warp-uniform loop, one elected lane issues) =================
-        const uint32_t idesc = make_idesc_bf16(128, N);
+    } else if (warp >= NCONV / 32) {
+        // ================= MMA warpgroups: rows [64 mw, 64 mw + 64) of the tile, all N columns =================
+        const int mw = warp / 4 - NCONV / 128, t = tid & 127;
         const uint64_t adesc_t = desc_template(APITCH, 128), bdesc_t = desc_template(N * 16, 128);
-        const uint32_t aring_addr = smem_u32(aring), bring_addr = smem_u32(bring);
+        const uint32_t aring_addr = smem_u32(aring) + mw * 64 * 16, bring_addr = smem_u32(bring);
+        float acc[N / 2];
         int sa = 0, pha = 0, sb = 0, phb = 0;
+        int psb = -1, psa = -1;  // ring slots read by the MMA group still in flight (freed once it completes)
         bool ok = true;
 #pragma unroll 1
         for (int ca = 0; ca < CIN / KCA; ++ca) {
             ok &= mbar_wait(&fullA[sa], pha);
-            tc_fence_after();
             const uint64_t abase = desc_at(adesc_t, aring_addr + sa * ASLOT);
 #pragma unroll 1
             for (int j = 0; j < KCA / 16; ++j) {
 #pragma unroll 1
                 for (int tap = 0; tap < NTAP; ++tap) {
                     ok &= mbar_wait(&fullB[sb], phb);
-                    tc_fence_after();
                     const uint64_t bbase = desc_at(bdesc_t, bring_addr + sb * BSLOT);
                     // A rows for this tap start at index `tap` (row i <-> v = r0 - PAD + i; the tap reads v + tap - PAD)
                     const uint64_t arow = abase + (uint64_t)tap + (uint64_t)(2 * j * (APITCH >> 4));
+                    wgmma_fence();
 #pragma unroll
                     for (int pass = 0; pass < 3; ++pass) {
                         const uint64_t adesc = arow + (uint64_t)(((pass == 1) * (KCA / 8) * APITCH) >> 4);
                         const uint64_t bdesc = bbase + (uint64_t)(((pass == 2) * 2 * N * 16) >> 4);
-                        const bool acc = !(ca == 0 && j == 0 && tap == 0 && pass == 0);
-                        if (elect_one()) mma_bf16(tmem, adesc, bdesc, idesc, acc);
+                        wgmma_bf16<N>(acc, adesc, bdesc, (ca | j | tap | pass) != 0);
                     }
-                    if (elect_one()) {
-                        if constexpr (Cfg::CL > 1) mma_commit_multicast(&emptyB[sb], kClusterMask);
-                        else mma_commit(&emptyB[sb]);
+                    wgmma_commit();
+                    wgmma_wait<1>();  // the previous slot's MMAs are complete: free its ring slots
+                    if (t == 0 && psb >= 0) {
+                        mbar_arrive(&emptyB[psb]);
+                        if (psa >= 0) mbar_arrive(&emptyA[psa]);
                     }
+                    psb = sb;
+                    psa = (j == KCA / 16 - 1 && tap == NTAP - 1) ? sa : -1;
                     if (++sb == NSB) { sb = 0; phb ^= 1; }
                 }
             }
-            if (elect_one()) mma_commit(&emptyA[sa]);
             if (++sa == NSA) { sa = 0; pha ^= 1; }
         }
-        if (elect_one()) mma_commit(done);
-        if (!ok && lane == 0) atomicExch(status, 23);
+        wgmma_wait<0>();
+        acc_fence<N / 2>(acc);
+        if (!ok && t == 0) atomicExch(status, 23);
+        pdl_trigger();  // MMAs done, only the output store is left: the next kernel of the chain may be scheduled
+        pdl_wait();     // (y may still be read by the previous kernel of the chain)
+        // ================= epilogue: D[v, co] + bias (-> LeakyReLU) -> y[item][co][s] =================
+        const float *bp = bias + cg * N;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int v = r0 + 64 * mw + frag_row(t, h);
+            const int item = v / Lv, s = v - item * Lv;
+            if (item < B && s < L) {
+                float *yp = y + ((size_t)item * COUT + cg * N) * L + s;
+#pragma unroll
+                for (int k = 0; k < N / 8; ++k)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = frag_col(lane & 3, 4 * k + e);
+                        float o = acc[4 * k + 2 * h + e] + __ldg(bp + col);
+                        if (Cfg::LRELU_OUT) o = lrelu(o);
+                        yp[(size_t)col * L] = o;
+                    }
+            }
+        }
     } else {
         // ================= converter warps: A slots = split(x), KCA channels of every row =================
         // Thread tid owns row tid of every slot and keeps the NEXT chunk's KCA loads in flight while it converts the
-        // current one (the chain of dependent memory round trips, not the MMAs, bounds a CTA: 32 chunks at K = 1024);
+        // current one (the chain of dependent memory round trips bounds a CTA: 32 chunks at K = 1024);
         // the 2 PAD rows beyond the first NCONV are picked up by the first threads without prefetch.
         pdl_wait();  // x: the previous kernel's output
         int sa = 0, pha = 0;
@@ -195,36 +204,7 @@ conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const ui
                 }
             }
         }
-        // ================= epilogue: D[v, co] + bias (-> LeakyReLU) -> y[item][co][s] =================
-        if (ok && !mbar_wait(done, 0)) { ok = false; if (lane == 0) atomicExch(status, 25); }
-        tc_fence_after();
-        pdl_trigger();  // MMAs done, only the output store is left: the next kernel of the chain may be scheduled
-        const int q = warp & 3;
-        const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-        const int v = r0 + q * 32 + lane;
-        const int item = v / Lv, s = v - item * Lv;
-        const bool row_ok = item < B && s < L;
-        float *yp = y + ((size_t)(row_ok ? item : 0) * COUT + cg * N) * L + (row_ok ? s : 0);
-        const float *bp = bias + cg * N;
-#pragma unroll 1
-        for (int c0 = 0; c0 < N; c0 += 32) {
-            uint32_t w[32];
-            tmem_ld32(lane_addr + c0, w);
-            tmem_ld_wait();
-            if (row_ok) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    float o = __uint_as_float(w[j]) + __ldg(bp + c0 + j);
-                    if (Cfg::LRELU_OUT) o = lrelu(o);
-                    yp[(size_t)(c0 + j) * L] = o;
-                }
-            }
-        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, N);
-    if constexpr (Cfg::CL > 1) cluster_sync();  // no CTA leaves while a peer may still multicast into its ring or barriers
 }
 
 template <class Cfg>
@@ -236,23 +216,17 @@ static int launch_conv_rows(const float *x, float *y, const uint8_t *wtc, const 
         configured = true;
     }
     const long long vrows = (long long)B * (L + Cfg::PAD);
-    unsigned tiles = (unsigned)((vrows + Cfg::ROWS - 1) / Cfg::ROWS);
-    tiles = (tiles + Cfg::CL - 1) / Cfg::CL * Cfg::CL;  // whole clusters (a tile past the last row converts zeros and stores nothing)
-    MG_CUDA_TRY(launch_ex(conv_rows_tc_kernel<Cfg>, dim3(tiles, Cfg::NCG), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, Cfg::CL, true, x, y, wtc,
-                          bias, L, B, status));
+    const unsigned tiles = (unsigned)((vrows + Cfg::ROWS - 1) / Cfg::ROWS);
+    MG_CUDA_TRY(launch_ex(conv_rows_tc_kernel<Cfg>, dim3(tiles, Cfg::NCG), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, x, y, wtc, bias,
+                          L, B, status));
     return MG_OK;
 }
 
-using PreCfg = ConvCfg<80, 512, 7, 80, false>;          // generator conv_pre
-// discriminator conv_post1 (+ LeakyReLU): N = 128 per CTA (an N = 128 MMA is as efficient as an N = 256 one: 64 cycles of
-// math = 64 cycles of operand reads), two CTAs per SM (the prefetching converter wants > 96 registers): the tiles of all three scales
-// (264 + 136 + 40 CTAs at 8192 samples) are resident together and hide each other's conversion and ring stalls
-// (CL = 2 -- the pair's weight slots multicast from one L2 read, frees by multicast commits -- is correct (the parity tests
-//  pass) and measured neutral: 105 vs 102 us on scale 0.  The kernel is bound by SHARED-memory traffic, not L2: an N = 128 MMA
-//  reads 8 KB of operands per 64 cycles = the whole 128 B/cycle, and the ring's bulk-copy writes (42 B/cycle) and the
-//  converter's stores come on top.  The lever is cta_group::2, where each CTA of a pair holds half of B.)
-using Post1Cfg = ConvCfg<1024, 1024, 5, 32, true, 2, kPost1NG, 1>;
-using Post1DgradCfg = ConvCfg<1024, 1024, 5, 32, false, 2, kPost1NG, 1>;  // the same contraction on the transposed blob, no activation
+using PreCfg = ConvCfg<80, 512, 7, 80, false, kPreNG>;  // generator conv_pre
+// discriminator conv_post1 (+ LeakyReLU): N = 128 per CTA, 8 channel groups -> 8x the row tiles' CTAs (264 + 136 + 40 per
+// group at 8192 samples over the three scales), so the grid spans several waves of the 132 SMs
+using Post1Cfg = ConvCfg<1024, 1024, 5, 32, true, kPost1NG>;
+using Post1DgradCfg = ConvCfg<1024, 1024, 5, 32, false, kPost1NG>;  // the same contraction on the transposed blob, no activation
 
 // mel [B][80][T] -> y [B][512][T]   (Generator.conv_pre)
 int launch_gen_pre_tc(const float *mel, float *y, const float *packed, int B, int T, int *status, cudaStream_t s) {

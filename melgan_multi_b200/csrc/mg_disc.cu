@@ -5,9 +5,9 @@
 //   conv_pre   1 -> 16, k15  (+ LeakyReLU), with the AvgPool1d chain of the scale fused into the input read
 //              (models.py:114-117,125-127: scale 1 sees AvgPool1d(4,2,pad 2)(y), scale 2 AvgPool1d(4,4,pad 2) of that;
 //              count_include_pad=True, so every window divides by 4)                                   fp32 SIMT
-//   grouped    k41, 4 input channels per group, stride 4/4/4/1 (+ LeakyReLU)                           tcgen05 (mg_disc_tc.cu;
+//   grouped    k41, 4 input channels per group, stride 4/4/4/1 (+ LeakyReLU)                           wgmma   (mg_disc_tc.cu;
 //              the fp32 SIMT kernels below are the second implementation, MG_DISC_GROUP=simt)
-//   conv_post1 1024 -> 1024, k5 (+ LeakyReLU): 88% of the FLOPs                                        tcgen05 (mg_conv_tc.cu)
+//   conv_post1 1024 -> 1024, k5 (+ LeakyReLU): 88% of the FLOPs                                        wgmma   (mg_conv_tc.cu)
 //   conv_post2 1024 -> 1, k3                                                                           fp32 SIMT
 // Every layer writes its feature map (fp32 NCL) because Discriminator.forward returns all seven (models.py:87-103).
 #include "mg_common.cuh"
@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(128) disc_pack_kernel(DiscPackArgs a, uint8_t 
         const int cog = sh.cout / sh.groups, grp = row / cog, col = row % cog;
         for (int j = threadIdx.x; j < inner; j += blockDim.x)  // j = ci*41 + tap -> [grp][ci][tap][col]
             fw[((size_t)grp * inner + j) * cog + col] = scale * vr[j];
-        if (l <= 3) {  // split-bf16 Toeplitz copy for the tcgen05 kernel (layout: mg_layout.h d_gtc_index), zeros included
+        if (l <= 3) {  // split-bf16 Toeplitz copy for the tensor-core kernel (layout: mg_layout.h d_gtc_index), zeros included
             __nv_bfloat16 *gt = reinterpret_cast<__nv_bfloat16 *>(blob + d_gtc_start() + d_gtc_offset(l) + (size_t)grp * d_gtc_group_bytes());
             for (int s = threadIdx.x; s < kDgPanels * 64; s += blockDim.x) {
                 const int ci = s & 3, pos = (s >> 2) & 1, e = (s >> 3) & 1, r = (s >> 4) & 3, kp = s >> 6;
@@ -325,7 +325,7 @@ static int disc_chain(const uint8_t *blob, const float *y, int sc, int Bt, int L
     else if (sc == 1) disc_pre_kernel<1><<<gpre, 256, 0, q>>>(y, f[0], fw, L, L1, L2);
     else disc_pre_kernel<2><<<gpre, 256, 0, q>>>(y, f[0], fw, L, L1, L2);
     MG_CUDA_TRY(cudaGetLastError());
-    for (int l = 1; l <= 3; ++l) {  // stride-4 grouped convs: tcgen05 (MG_DISC_GROUP=simt: the fp32 SIMT second implementation)
+    for (int l = 1; l <= 3; ++l) {  // stride-4 grouped convs: tensor cores (MG_DISC_GROUP=simt: the fp32 SIMT second implementation)
         const DLayer d = d_layer(l);
         if (group_tc)
             rc = launch_disc_group_tc(f[l - 1], f[l], blob + d_gtc_start() + d_gtc_offset(l), fw + d_bias_offset(l), Bt, d.cin,

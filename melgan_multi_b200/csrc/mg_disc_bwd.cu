@@ -1,6 +1,6 @@
 // Backward of the discriminators' grouped convs (layers 1..4 of models.py:78-82: k41, pad 20, 4 input channels per group,
 // stride 4/4/4/1) and of weight-norm for all 21 discriminator layers.  cuDNN runs a grouped conv's backward as one small
-// kernel per group (thousands of launches per step: 29 ms of a 32 ms training step at BASELINE config 3); here each
+// kernel per group (thousands of launches per step at BASELINE config 3); here each
 // gradient is one launch.  fp32 SIMT: the FLOPs are small (1.4 GF per layer), the dense layers' backward stays on
 // cuDNN (aten::convolution_backward) for now.
 //
@@ -448,18 +448,19 @@ __global__ void __launch_bounds__(256) lrelu_grad_kernel(const float *__restrict
 int launch_lrelu_grad(const float *g1, const float *g2, const float *out, float *dz, long long n, cudaStream_t s) {
     if (!g1 || !out || !dz || n < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_lrelu_backward: bad argument");
     long long blocks = (n / 4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
     if (blocks < 1) blocks = 1;
     lrelu_grad_kernel<<<(unsigned)blocks, 256, 0, s>>>(g1, g2, out, dz, n);
     MG_CUDA_TRY(cudaGetLastError());
     return MG_OK;
 }
 
-constexpr int kDw4Ctas = 1184;  // grouped_dw4_kernel: 64 threads and 17 KB of shared memory per CTA -> 8 per SM
+constexpr int kDw4Ctas = 8 * kNumSMs;  // grouped_dw4_kernel: 64 threads and 17 KB of shared memory per CTA -> 8 per SM
+constexpr int kDwCtas = 4 * kNumSMs;   // the 192-thread weight-gradient kernels: 4 per SM
 struct GroupedBwdPlan {
     int tiles_per_item, tiles_per_chunk, chunks;
 };
-static GroupedBwdPlan grouped_plan(int groups, int Bt, int Lout, int ctas = 592) {
+static GroupedBwdPlan grouped_plan(int groups, int Bt, int Lout, int ctas = kDwCtas) {
     GroupedBwdPlan p;
     p.tiles_per_item = (Lout + 127) / 128;
     const int total = Bt * p.tiles_per_item;
@@ -477,7 +478,7 @@ static int group_blocks(int groups, int cog, int stride) { return (stride == 1 &
 size_t grouped_bwd_workspace_bytes(int l, int Bt, int Lout) {
     const DLayer d = d_layer(l);
     const int cog = d.cout / d.groups;
-    return (size_t)grouped_plan(group_blocks(d.groups, cog, d.stride), Bt, Lout, d.stride == 4 ? kDw4Ctas : 592).chunks * d.groups * 165 * cog *
+    return (size_t)grouped_plan(group_blocks(d.groups, cog, d.stride), Bt, Lout, d.stride == 4 ? kDw4Ctas : kDwCtas).chunks * d.groups * 165 * cog *
            sizeof(float);
 }
 
@@ -499,7 +500,7 @@ static int grouped_backward(const float *w, const float *dz, const float *x, flo
         MG_CUDA_TRY(cudaGetLastError());
     }
     if (dw) {
-        const GroupedBwdPlan p = grouped_plan(group_blocks(groups, COG, S), Bt, Lout, S == 4 ? kDw4Ctas : 592);
+        const GroupedBwdPlan p = grouped_plan(group_blocks(groups, COG, S), Bt, Lout, S == 4 ? kDw4Ctas : kDwCtas);
         if (S == 4 && COG == 16) {
             dim3 grid(p.chunks, groups);
             grouped_dw4_kernel<<<grid, 64, 0, s>>>(dz, x, ws, Bt, Cin, Cout, Lin, Lout, p.tiles_per_item, p.tiles_per_chunk);

@@ -1,7 +1,7 @@
 // The whole backward of ONE Discriminator (autograd of models.py:87-103 of the reference) behind a single call: the host walks
 // the seven layers from the logits down and enqueues every kernel itself -- LeakyReLU', grouped-conv dx / dw / db, conv_post1
-// dgrad + wgrad (tcgen05), conv_pre / conv_post2 -- so a training step pays one host call per discriminator instead of ~25
-// Python-level launches (the step was bound by that host work, not by the GPU: 11.9 ms of kernels in a 13.5 ms step).
+// dgrad + wgrad (wgmma), conv_pre / conv_post2 -- so a training step pays one host call per discriminator instead of ~25
+// Python-level launches (host work that would otherwise bound the step, not the GPU).
 // Gradients of the FOLDED weights come back per layer; mg_msd_wn_backward turns them into (d weight_v, d weight_g).
 #include "mg_common.cuh"
 

@@ -1,11 +1,11 @@
 // Discriminator grouped convs on the tensor cores: Conv1d(k41, stride 4, pad 20, 4 input / 16 output channels per group)
-// + LeakyReLU, layers 1..3 of models.py:78-81,89-95 (groups 4 / 16 / 64), tcgen05 + TMEM, split-bf16.
+// + LeakyReLU, layers 1..3 of models.py:78-81,89-95 (groups 4 / 16 / 64), wgmma, split-bf16.
 //
 // Toeplitz view.  Tap k = 4q + r of output t reads input position 4(t + q - 5) + r, so with the input of one group
 // de-interleaved by phase r into channels-last rows  U_r[u][ci] = x[ci][4u + r]  (8 B per u in bf16), one output is
 //     out[co][t] = sum_r sum_q sum_ci  U_r[t + q - 5][ci] * w[co][ci][4q + r].
-// A 16-byte unit of U_r holds two consecutive u (x 4 ci) = one 8-element k-panel, and rows of an UMMA operand are
-// 16 B = 2 u apart, so TMEM lane m of a tile is the output PAIR t = t0 + 2m + e (e = 0, 1) and both parities read the
+// A 16-byte unit of U_r holds two consecutive u (x 4 ci) = one 8-element k-panel, and rows of a wgmma operand are
+// 16 B = 2 u apart, so accumulator row m of a tile is the output PAIR t = t0 + 2m + e (e = 0, 1) and both parities read the
 // same A rows:  unit (m + kp) of U_r  x  weights of q = 2 kp + pos - 1 - e  (7 panels cover q = -2..11, zeros outside
 // 0..10; mg_layout.h d_gtc_index).  One K = 16 instruction contracts panel kp of phases r and r + 1 (LBO = the pitch
 // between phase buffers), with N = 64 columns = [w hi | w lo] x parity x 16 co:
@@ -13,6 +13,7 @@
 // = 28 instructions per (group, 256 outputs); the epilogue adds the hi and lo column blocks (fp32-grade: ~4e-6).
 // CTA = 2 groups x 256 outputs of one batch item, 93 KB of shared memory -> two CTAs per SM overlap each other's
 // load / convert, MMA and epilogue phases.  Weights (28 KB per group, contiguous in the packed blob) arrive by bulk TMA.
+// The two converter warpgroups then run the MMAs of rows 0..63 / 64..127 and the epilogue from their accumulator registers.
 #include "mg_common.cuh"
 #include "mg_tc.cuh"
 
@@ -21,14 +22,14 @@ using namespace tc;
 
 namespace dg {
 constexpr int NGRP = 2;                       // groups per CTA
-constexpr int TILE = 256;                     // outputs per CTA (128 TMEM lanes x 2 parities)
+constexpr int TILE = 256;                     // outputs per CTA (128 accumulator rows x 2 parities)
 constexpr int UNITS = 128 + kDgPanels - 1;    // 16-byte units per phase buffer
 constexpr int XP = UNITS * 16;                // phase-buffer pitch: 536 words = 24 (mod 32) -> conflict-free 8-byte stores
 constexpr int NPOS = UNITS * 8;               // input positions per channel per tile
 constexpr int WBYTES = 28672;                 // d_gtc_group_bytes()
 constexpr int XBYTES = NGRP * 2 * 4 * XP;     // [group][half][phase r][unit][pos 2][ci 4] bf16
 constexpr int NCONV = 256, NT = NCONV + 32;
-constexpr int SMEM_BYTES = NGRP * WBYTES + XBYTES + (1 + NGRP) * 8 + 16;
+constexpr int SMEM_BYTES = NGRP * WBYTES + XBYTES + 8;
 static_assert(WBYTES == (int)d_gtc_group_bytes(), "weight block");
 }  // namespace dg
 
@@ -40,24 +41,17 @@ disc_group_tc_kernel(const float *__restrict__ x, float *__restrict__ out, const
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *wsm = smem, *xsm = smem + NGRP * WBYTES;
     uint64_t *wbar = reinterpret_cast<uint64_t *>(xsm + XBYTES);
-    uint64_t *done = wbar + 1;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(done + NGRP);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // lanes are VIRTUAL when the sequence is short: ni items share the tile at a pitch of rp lanes / units (an item's
+    // rows are VIRTUAL when the sequence is short: ni items share the tile at a pitch of rp rows / units (an item's
     // ceil(Lout/2) output pairs + 6 halo units); ni == 1 (rp = 2^30): blockIdx.x walks the 256-output tiles of one item
     const int t0 = blockIdx.x * TILE, g0 = blockIdx.y * NGRP, b0 = blockIdx.z * ni;
 
-    if (warp == 0) tmem_alloc(tmem_slot, NGRP * 64);
-    if (tid == 32) {
+    if (tid == 0) {
         mbar_init(wbar, 1);
-        for (int g = 0; g < NGRP; ++g) mbar_init(&done[g], 1);
         fence_mbar_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
     if (warp == NCONV / 32) {
         if (lane == 0) {
@@ -97,16 +91,17 @@ disc_group_tc_kernel(const float *__restrict__ x, float *__restrict__ out, const
     }
     __syncthreads();
 
-    if (warp == NCONV / 32) {
-        // ================= MMA issuer (warp-uniform, one elected lane issues) =================
+    if (warp < NCONV / 32) {
+        // ================= MMA: warpgroup mw owns accumulator rows [64 mw, 64 mw + 64), both groups =================
+        const int mw = warp >> 2, t = tid & 127;
         bool ok = mbar_wait(wbar, 0);
-        tc_fence_after();
-        const uint32_t idesc64 = make_idesc_bf16(128, 64), idesc32 = make_idesc_bf16(128, 32);
         const uint64_t adesc_t = desc_template(XP, 128), bdesc_t = desc_template(64 * 16, 128);
-        const uint32_t x_addr = smem_u32(xsm), w_addr = smem_u32(wsm);
-#pragma unroll 1
+        const uint32_t x_addr = smem_u32(xsm) + mw * 64 * 16, w_addr = smem_u32(wsm);
+        float acc[NGRP][32];
+        wgmma_fence();
+#pragma unroll
         for (int g = 0; g < NGRP; ++g) {
-#pragma unroll 1
+#pragma unroll
             for (int pass = 0; pass < 2; ++pass) {
                 const uint64_t a0 = desc_at(adesc_t, x_addr + (g * 2 + pass) * 4 * XP);
                 const uint64_t b0 = desc_at(bdesc_t, w_addr + g * WBYTES);
@@ -116,50 +111,46 @@ disc_group_tc_kernel(const float *__restrict__ x, float *__restrict__ out, const
                     for (int rq = 0; rq < 2; ++rq) {  // phase pair (r = 2 rq, 2 rq + 1)
                         const uint64_t adesc = a0 + (uint64_t)((2 * rq * XP + 16 * kp) >> 4);
                         const uint64_t bdesc = b0 + (uint64_t)(((kp * 2 + rq) * 2048) >> 4);
-                        if (elect_one()) mma_bf16(tmem + g * 64, adesc, bdesc, pass ? idesc32 : idesc64, (pass | kp | rq) != 0);
+                        if (pass) wgmma_bf16<32>(acc[g], adesc, bdesc, 1);
+                        else wgmma_bf16<64>(acc[g], adesc, bdesc, (kp | rq) != 0);
                     }
                 }
             }
-            if (elect_one()) mma_commit(&done[g]);
         }
-        if (!ok && lane == 0) atomicExch(status, 31);
-    } else {
-        // ================= epilogue: lane m <-> outputs t0 + 2m, t0 + 2m + 1; warp half <-> 8 of the 16 co =================
-        const int q = warp & 3, ch = warp >> 2;
-        const int m = q * 32 + lane, jm = m / rp, b = b0 + jm;
-        const int t = (jm < ni && b < Bt) ? t0 + 2 * (m - jm * rp) : Lout;  // lanes of the inter-item gap store nothing
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence<32>(acc[0]);
+        acc_fence<32>(acc[1]);
+        if (!ok && t == 0) atomicExch(status, 31);
+        // ================= epilogue: row m <-> outputs t0 + 2m, t0 + 2m + 1 =================
+        // column 8k + 2q + e = [hi | lo] (k / 4) x parity ((k / 2) % 2) x co 8 (k % 2) + 2q + e
         const bool pair = (Lout & 1) == 0;
-#pragma unroll 1
-        for (int g = 0; g < NGRP; ++g) {
-            if (!mbar_wait(&done[g], 0)) { if (lane == 0) atomicExch(status, 32); break; }
-            tc_fence_after();
-            const uint32_t ta = tmem + ((uint32_t)(q * 32) << 16) + g * 64 + ch * 8;
-            uint32_t h0[8], h1[8], l0[8], l1[8];
-            tmem_ld8(ta, h0);
-            tmem_ld8(ta + 16, h1);
-            tmem_ld8(ta + 32, l0);
-            tmem_ld8(ta + 48, l1);
-            tmem_ld_wait();
-            const int co0 = (g0 + g) * 16 + ch * 8;
-            float *op = out + ((size_t)(t < Lout ? b : 0) * Cout + co0) * Lout + t;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float bv = __ldg(bias + co0 + j);
-                const float v0 = lrelu(__uint_as_float(h0[j]) + __uint_as_float(l0[j]) + bv);
-                const float v1 = lrelu(__uint_as_float(h1[j]) + __uint_as_float(l1[j]) + bv);
-                float *o = op + (size_t)j * Lout;
-                if (pair && t + 1 < Lout) {
-                    *reinterpret_cast<float2 *>(o) = make_float2(v0, v1);
-                } else {
-                    if (t < Lout) o[0] = v0;
-                    if (t + 1 < Lout) o[1] = v1;
-                }
-            }
+        for (int h = 0; h < 2; ++h) {
+            const int m = 64 * mw + frag_row(t, h), jm = m / rp, b = b0 + jm;
+            const int tt = (jm < ni && b < Bt) ? t0 + 2 * (m - jm * rp) : Lout;  // rows of the inter-item gap store nothing
+            if (tt >= Lout) continue;
+#pragma unroll
+            for (int g = 0; g < NGRP; ++g)
+#pragma unroll
+                for (int c8 = 0; c8 < 2; ++c8)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int co = (g0 + g) * 16 + 8 * c8 + 2 * (lane & 3) + e;
+                        const float bv = __ldg(bias + co);
+                        const int i0 = 2 * h + e;
+                        const float v0 = lrelu(acc[g][4 * c8 + i0] + acc[g][4 * (4 + c8) + i0] + bv);
+                        const float v1 = lrelu(acc[g][4 * (2 + c8) + i0] + acc[g][4 * (6 + c8) + i0] + bv);
+                        float *o = out + ((size_t)b * Cout + co) * Lout + tt;
+                        if (pair && tt + 1 < Lout) {
+                            *reinterpret_cast<float2 *>(o) = make_float2(v0, v1);
+                        } else {
+                            o[0] = v0;
+                            if (tt + 1 < Lout) o[1] = v1;
+                        }
+                    }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, NGRP * 64);
 }
 
 // x [Bt][Cin][Lin] -> out [Bt][Cout][Lout] = lrelu(grouped conv), layer l in 1..3;  wtc = blob + d_gtc_start() + d_gtc_offset(l)
@@ -182,7 +173,7 @@ int launch_disc_group_tc(const float *x, float *out, const uint8_t *wtc, const f
 
 // ------------------------------------------------------------------------------------------------------------------
 // Layer 4: Conv1d(1024 -> 1024, k41, stride 1, pad 20, groups 256: 4 -> 4 channels per group) + LeakyReLU, models.py:82.
-// With only 4 outputs per group the contraction is made dense along TIME instead: TMEM lane m owns the 8 consecutive
+// With only 4 outputs per group the contraction is made dense along TIME instead: accumulator row m owns the 8 consecutive
 // outputs t = 8 kb + e, the A operand of input channel ci is the plain bf16 signal cut into 16-byte units of 8 positions
 // (unit u = positions 8u - 20 .. 8u - 13, so lane kb reads units kb .. kb + 5: 48 positions for 8 outputs x 41 taps),
 // and B is the Toeplitz matrix  B[(e, co)][i of panel kp] = w[co][ci][8 kp + i - e]  (85 % dense; mg_layout.h).
@@ -199,7 +190,7 @@ constexpr int XP = UNITS * 16;                // channel-buffer pitch
 constexpr int WBYTES = 24576;                 // d_g4tc_group_bytes()
 constexpr int XBYTES = NGRP * 2 * 4 * XP;     // [group][half][ci][unit][8 positions] bf16
 constexpr int NCONV = 256, NT = NCONV + 32;
-constexpr int SMEM_BYTES = NGRP * WBYTES + XBYTES + (1 + NGRP) * 8 + 16;
+constexpr int SMEM_BYTES = NGRP * WBYTES + XBYTES + 8;
 static_assert(WBYTES == (int)d_g4tc_group_bytes(), "weight block");
 }  // namespace dg4
 
@@ -211,22 +202,15 @@ disc_group4_tc_kernel(const float *__restrict__ x, float *__restrict__ out, cons
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *wsm = smem, *xsm = smem + NGRP * WBYTES;
     uint64_t *wbar = reinterpret_cast<uint64_t *>(xsm + XBYTES);
-    uint64_t *done = wbar + 1;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(done + NGRP);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int item0 = (blockIdx.x / segs) * ni, kb0 = (blockIdx.x % segs) * 128, g0 = blockIdx.y * NGRP;
 
-    if (warp == 0) tmem_alloc(tmem_slot, NGRP * 64);
-    if (tid == 32) {
+    if (tid == 0) {
         mbar_init(wbar, 1);
-        for (int g = 0; g < NGRP; ++g) mbar_init(&done[g], 1);
         fence_mbar_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
     if (warp == NCONV / 32) {
         if (lane == 0) {
@@ -259,16 +243,17 @@ disc_group4_tc_kernel(const float *__restrict__ x, float *__restrict__ out, cons
     }
     __syncthreads();
 
-    if (warp == NCONV / 32) {
-        // ================= MMA issuer (warp-uniform, one elected lane issues) =================
+    if (warp < NCONV / 32) {
+        // ================= MMA: warpgroup mw owns accumulator rows [64 mw, 64 mw + 64), both groups =================
+        const int mw = warp >> 2, t = tid & 127;
         bool ok = mbar_wait(wbar, 0);
-        tc_fence_after();
-        const uint32_t idesc64 = make_idesc_bf16(128, 64), idesc32 = make_idesc_bf16(128, 32);
         const uint64_t adesc_t = desc_template(XP, 128), bdesc_t = desc_template(64 * 16, 128);
-        const uint32_t x_addr = smem_u32(xsm), w_addr = smem_u32(wsm);
-#pragma unroll 1
+        const uint32_t x_addr = smem_u32(xsm) + mw * 64 * 16, w_addr = smem_u32(wsm);
+        float acc[NGRP][32];
+        wgmma_fence();
+#pragma unroll
         for (int g = 0; g < NGRP; ++g) {
-#pragma unroll 1
+#pragma unroll
             for (int pass = 0; pass < 2; ++pass) {
                 const uint64_t a0 = desc_at(adesc_t, x_addr + (g * 2 + pass) * 4 * XP);
                 const uint64_t b0 = desc_at(bdesc_t, w_addr + g * WBYTES);
@@ -278,52 +263,40 @@ disc_group4_tc_kernel(const float *__restrict__ x, float *__restrict__ out, cons
                     for (int cp = 0; cp < 2; ++cp) {
                         const uint64_t adesc = a0 + (uint64_t)((2 * cp * XP + 16 * kp) >> 4);
                         const uint64_t bdesc = b0 + (uint64_t)(((kp * 2 + cp) * 2048) >> 4);
-                        if (elect_one()) mma_bf16(tmem + g * 64, adesc, bdesc, pass ? idesc32 : idesc64, (pass | kp | cp) != 0);
+                        if (pass) wgmma_bf16<32>(acc[g], adesc, bdesc, 1);
+                        else wgmma_bf16<64>(acc[g], adesc, bdesc, (kp | cp) != 0);
                     }
                 }
             }
-            if (elect_one()) mma_commit(&done[g]);
         }
-        if (!ok && lane == 0) atomicExch(status, 33);
-    } else {
-        // ================= epilogue: warp quadrant <-> 32 lanes (blocks of 8 outputs), warp half <-> group =================
-        const int q = warp & 3, g = warp >> 2;
-        const int m = q * 32 + lane, j = m / rp, item = item0 + j, kb = kb0 + m - j * rp;
-        const bool row_ok = item < Bt && j < ni && kb < nb;
-        if (!mbar_wait(&done[g], 0)) {
-            if (lane == 0) atomicExch(status, 34);
-        } else {
-            tc_fence_after();
-            const uint32_t ta = tmem + ((uint32_t)(q * 32) << 16) + g * 64;
-            uint32_t h[32], l[32];
-            tmem_ld32(ta, h);
-            tmem_ld32(ta + 32, l);
-            tmem_ld_wait();
-            if (row_ok) {
-                const int co0 = (g0 + g) * 4, t = 8 * kb;
-                const bool vec = (L & 3) == 0 && t + 8 <= L;
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence<32>(acc[0]);
+        acc_fence<32>(acc[1]);
+        if (!ok && t == 0) atomicExch(status, 33);
+        // ================= epilogue: row m <-> the 8 outputs t = 8 kb + e =================
+        // column 8k + 2q + e' = [hi | lo] (k / 4) x e (2 (k % 4) + q / 2) x co (2 (q % 2) + e'): this thread holds the
+        // outputs e = 2 kk + q / 2 (kk = 0..3) of channels co = 2 (q % 2) + e'
+        const int q = lane & 3;
 #pragma unroll
-                for (int co = 0; co < 4; ++co) {
-                    const float bv = __ldg(bias + co0 + co);
-                    float v[8];
+        for (int h = 0; h < 2; ++h) {
+            const int m = 64 * mw + frag_row(t, h), j = m / rp, item = item0 + j, kb = kb0 + m - j * rp;
+            if (!(item < Bt && j < ni && kb < nb)) continue;
 #pragma unroll
-                    for (int e = 0; e < 8; ++e) v[e] = lrelu(__uint_as_float(h[e * 4 + co]) + __uint_as_float(l[e * 4 + co]) + bv);
-                    float *o = out + ((size_t)item * C + co0 + co) * L + t;
-                    if (vec) {
-                        *reinterpret_cast<float4 *>(o) = make_float4(v[0], v[1], v[2], v[3]);
-                        *reinterpret_cast<float4 *>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
-                    } else {
+            for (int g = 0; g < NGRP; ++g)
 #pragma unroll
-                        for (int e = 0; e < 8; ++e)
-                            if (t + e < L) o[e] = v[e];
+                for (int ep = 0; ep < 2; ++ep) {
+                    const int co = (g0 + g) * 4 + 2 * (q & 1) + ep;
+                    const float bv = __ldg(bias + co);
+                    float *o = out + ((size_t)item * C + co) * L + 8 * kb + (q >> 1);
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) {
+                        const int i0 = 4 * kk + 2 * h + ep;
+                        if (8 * kb + 2 * kk + (q >> 1) < L) o[2 * kk] = lrelu(acc[g][i0] + acc[g][16 + i0] + bv);
                     }
                 }
-            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, NGRP * 64);
 }
 
 // x [Bt][1024][L] -> out [Bt][1024][L] = lrelu(grouped conv, layer 4);  wtc = blob + d_g4tc_start()

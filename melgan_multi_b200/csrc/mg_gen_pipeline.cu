@@ -9,16 +9,17 @@ namespace mg {
 
 // Pipeline shape.  TAIL mask: bit i (i = 1..3) set = ConvTranspose of stage i runs at the TAIL of ResBlock i-1's kernel
 // (mg_res_tc.cu, UPT): the chain is then  conv_pre, up0, res0+up1, res1+up2, res2+up3, res3+post  -- six kernels, no ResBlock
-// output ever written to HBM.  Default: stages 1 and 3 (measured at config 2: res0+up1 and res2+up3 beat their two-kernel
-// forms; res1+up2 does not -- the extra halo row a tail ConvT needs turns the 9 tiles of a 2048-position item into 10, i.e.
-// 640 CTAs = 5 waves instead of 576 = 4).  MG_GEN_TAIL=<digits> ("123", "0" for none) / mg_gen_set_pipeline() override it.  Where stage 3's ConvT is not at res2's tail it runs at the FRONT of the last
+// output ever written to HBM.  Default: none (H100 80GB HBM3 at 700 W, config 2, bench.py: 1.96 ms per forward with no tail
+// fusion, 1.99 with stage 3's, 2.04 with stage 1's, 2.06 with both, 2.07 with all three -- a tail ConvT's extra halo row
+// and its un-overlapped per-group stores cost more than the HBM round trip it saves).  MG_GEN_TAIL=<digits> ("123", "0"
+// for none) / mg_gen_set_pipeline() override it.  Where stage 3's ConvT is not at res2's tail it runs at the FRONT of the last
 // kernel (UPF, "up3+res3+post") unless MG_GEN_FUSE_UP says otherwise (bit 0: stage 2 front-fused, bit 1: stage 3).
 static thread_local int g_tail_override = -1;
 void generator_tc_set_tail(int mask) { g_tail_override = mask; }
 int generator_tc_tail() {
     static const int env_mask = [] {
         const char *e = getenv("MG_GEN_TAIL");
-        if (!e) return 0b1010;
+        if (!e) return 0;
         int m = 0;
         for (; *e; ++e) m |= (*e >= '1' && *e <= '3') ? 1 << (*e - '0') : 0;
         return m;
@@ -149,8 +150,8 @@ struct SliceStreams {
 
 // Whole generator.  The batch items are independent and every kernel's grid is a whole number of tiles per item (or per
 // 128 virtual rows), so the batch is cut into `slices` contiguous parts whose nine-kernel chains run on forked streams:
-// the block scheduler fills the SMs one chain's partial last wave leaves idle (stage 0 at config 2 is 192 one-per-SM
-// tiles on 148 SMs) with the other chain's tiles.  Same kernels, same per-item arithmetic: results are bit-identical
+// the block scheduler fills the SMs one chain's partial last wave leaves idle (stage 0 at config 2 is 512 one-per-SM
+// tiles on 132 SMs) with the other chain's tiles.  Same kernels, same per-item arithmetic: results are bit-identical
 // to the single-chain order.  ev != nullptr (per-kernel timing) keeps everything on one stream.
 int generator_tc_slices(int B, int T) {
     static const int forced = [] {  // MG_GEN_SLICES=n pins the slice count (experiments); default: chosen from the shape

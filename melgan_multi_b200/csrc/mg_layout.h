@@ -113,7 +113,7 @@ MG_HD constexpr size_t up_weight_index(int stage, int ci, int co, int k, int h) 
 // ---- tensor-core blob for stride-1 dense convs run by conv_rows_tc_kernel (mg_conv_tc.cu): conv_pre here, the
 // discriminators' conv_post1 in their own blob.  One ring slot = (NG-channel output group, 16-channel K chunk, tap):
 //   [cg = co/NG][chunk = ci/16][tap][half: hi, lo][k-panel = (ci%16)/8][co%NG][ci%8]   (bf16), 64 NG bytes per slot
-constexpr int kPreNG = 256;    // conv_pre: 512 output channels = 2 groups
+constexpr int kPreNG = 128;    // conv_pre: 512 output channels = 4 groups (an N = 256 register tile does not fit beside the converter)
 constexpr int kPost1NG = 128;  // conv_post1: 8 groups of 128 -> twice the CTAs of a 256-wide split at the same MMA efficiency
 MG_HD constexpr size_t conv_tc_weight_index(int CIN, int NTAP, int NG, int co, int ci, int tap, int h) {
     return (((((size_t)(co / NG) * (CIN / 16) + ci / 16) * NTAP + tap) * 2 + h) * 2 + (ci % 16) / 8) * NG * 8 +
@@ -194,7 +194,7 @@ MG_HD constexpr size_t d_gtc_offset(int l) {  // bytes from d_gtc_start(), l = 1
     return o;
 }
 MG_HD constexpr size_t d_gtc_bytes() { return d_gtc_offset(4); }
-// Tensor-core copy of the stride-1 grouped conv (layer 4: 256 groups of 4 -> 4 channels), 24 KB per group: one TMEM lane
+// Tensor-core copy of the stride-1 grouped conv (layer 4: 256 groups of 4 -> 4 channels), 24 KB per group: one accumulator row
 // owns a block of 8 consecutive outputs t = 8 m + e, a 16-byte unit of the A operand is 8 consecutive positions of ONE
 // input channel, and element i of k-panel kp (of channel ci) multiplies w[co][ci][tap = 8 kp + i - e] (zero outside 0..40):
 //   [kp 6][ci pair 2][ci & 1][n 64 = half 2 x e 8 x co 4][8 bf16] = one B operand (N = 64, K = 16) per (kp, ci pair).

@@ -1,6 +1,6 @@
 // Multi-tensor Adam: one launch updates every parameter tensor of an optimizer group (SURVEY 8f rank 1; the reference
 // calls torch.optim.Adam on 90 (G) / 63 (D) separate tensors, train.py:51-52,118,129 -- with torch's foreach path that is
-// ~1.5 ms of small launches per step at BASELINE config 3).  Same arithmetic as torch.optim.Adam (no amsgrad):
+// ~10 sequences of small launches per step).  Same arithmetic as torch.optim.Adam (no amsgrad):
 //   g += wd p;  m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g^2;  p -= lr / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps)
 #include "mg_common.cuh"
 

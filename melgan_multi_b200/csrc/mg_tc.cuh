@@ -1,14 +1,19 @@
-// sm_100a tensor-core plumbing: mbarrier, 1-D bulk TMA, TMEM allocation, tcgen05.mma / ld / commit,
-// shared-memory matrix descriptors (no-swizzle, K-major) and the instruction descriptor.
+// sm_90a tensor-core plumbing: mbarrier, 1-D bulk TMA, warpgroup MMA (wgmma) with shared-memory matrix descriptors
+// (no-swizzle, K-major) and fp32 accumulators in registers.
 //
 // Layout convention used everywhere in this engine ("row-linear K-major, no swizzle"):
 //   an operand tile of R rows (M or N index) by K bf16 elements is stored as K/8 "k-panels";
 //   panel kp holds, for every row r, the 8 consecutive K elements [8*kp, 8*kp+8) as one 16-byte unit at
 //       panel_base(kp) + r * 16.
-//   In UMMA terms the core matrix is 8 rows x 16 B = 128 contiguous bytes, the stride between 8-row
+//   In wgmma terms the core matrix is 8 rows x 16 B = 128 contiguous bytes, the stride between 8-row
 //   groups (SBO) is 128 B -- i.e. rows are simply 16 B apart -- and the stride between the two k-panels
-//   one K=16 MMA consumes (LBO) is the panel pitch.  Because rows are linear, a conv tap that shifts the
+//   one K = 16 MMA consumes (LBO) is the panel pitch.  Because rows are linear, a conv tap that shifts the
 //   operand by d rows is just "start address + 16*d": no swizzle phase to respect, any d is legal.
+//
+// Accumulators: one wgmma.m64nNk16 is issued by a whole warpgroup (128 threads) and leaves its 64 x N fp32 result in
+// the registers of that warpgroup.  Thread t (warp w = t / 32 of the group, lane l) holds, for every 8-column block k,
+//     d[4k + 2h + e] = D[16 w + l / 4 + 8 h][8 k + 2 (l % 4) + e]        (h, e in {0, 1})
+// frag_row() / frag_col() below name those coordinates.
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
@@ -40,8 +45,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded wait: returns false (and lets the caller bail out) instead of hanging the GPU if the
-// producer never arrives -- a hung box is a strike, a wrong answer is just a failed test.
+// Bounded wait: returns false (and lets the caller raise the status word and carry on) instead of hanging the GPU if the
+// producer never arrives.
 __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity, uint32_t max_spins = 1u << 24) {
     for (uint32_t i = 0; i < max_spins; ++i)
         if (mbar_try_wait(bar, parity)) return true;
@@ -55,212 +60,90 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, u
                  "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
-// ---- tensor-map TMA (cp.async.bulk.tensor): a 3-D box of a global tensor -> dense shared-memory tile, out-of-bounds elements
-// zero-filled, completes on an mbarrier.  tmap: address of a CUtensorMap kernel parameter (__grid_constant__).
-__device__ __forceinline__ void tma_load_3d(void *smem_dst, const void *tmap, int c0, int c1, int c2, uint64_t *bar) {
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];" ::"r"(
-                     smem_u32(smem_dst)),
-                 "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_desc(const void *tmap) { asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory"); }
-// ---- thread-block clusters: one bulk copy feeds the same shared-memory offset of every CTA in `cta_mask` (and completes on
-// the mbarrier at the same offset of each), so CTAs that stream the same weights read them from L2 once -----------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void bulk_g2s_multicast(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar, uint16_t cta_mask) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
-                     smem_u32(smem_dst)),
-                 "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
-                 : "memory");
-}
-// ---- distributed shared memory (CTA pairs that exchange tile-boundary rows, mg_res_tc.cu) ------------------------------------
-// address of the same shared-memory offset in CTA `cta_rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t cta_rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta_rank));
-    return r;
-}
-__device__ __forceinline__ void st_cluster_v4(uint32_t cluster_addr, uint4 v) {
-    asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(cluster_addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-// arrive on an mbarrier of another CTA of the cluster; release at cluster scope: this thread's earlier writes (to that CTA's
-// shared memory) are visible to whoever observes the arrival with an acquire.cluster wait
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t *bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ bool mbar_wait_cluster(uint64_t *bar, uint32_t parity, uint32_t max_spins = 1u << 24) {
-    for (uint32_t i = 0; i < max_spins; ++i)
-        if (mbar_try_wait_cluster(bar, parity)) return true;
-    return false;
-}
-// generic-proxy writes -> async proxy, every state space (used after stores into a PEER CTA's shared memory)
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-// generic-proxy writes (st.shared) -> visible to the async proxy (UMMA operand reads, bulk copies)
+// generic-proxy writes (st.shared) -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// named barrier over `count` threads (a multiple of 32); id 0 is __syncthreads
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // ---- programmatic dependent launch (PDL): the generator chain's kernels are launched with
-// cudaLaunchAttributeProgrammaticStreamSerialization, so kernel N+1's CTAs may start -- barrier init, TMEM allocation, the
-// weight stream of its first ring slots: everything that does not touch kernel N's output -- while kernel N's last wave is
+// cudaLaunchAttributeProgrammaticStreamSerialization, so kernel N+1's CTAs may start -- barrier init and the weight
+// stream of its first ring slots: everything that does not touch kernel N's output -- while kernel N's last wave is
 // still running.  pdl_trigger(): "my dependents may be scheduled" (they still wait for this whole grid's completion and
 // memory flush in pdl_wait()); pdl_wait(): executed by every thread that reads or writes activations, before it does.
 // Both are no-ops in a launch without the attribute.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// ---- TMEM ------------------------------------------------------------------------------------
-// One full warp executes these.  ncols: power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// ---- cta_group::2: a CTA PAIR executes one M = 256 MMA (verified by csrc/probe/tc_probe2sm.cu).  Each CTA's shared memory
-// holds its own 128 rows of A and HALF of B -- rows [rank*N/2, (rank+1)*N/2) -- at the descriptors' addresses, its own 128 x N
-// accumulator sits at the same TMEM address in both CTAs; one thread of the LEADER issues, commits go to both CTAs' barriers.
-__device__ __forceinline__ void tmem_alloc2(uint32_t *smem_result, uint32_t ncols) {  // warp 0 of BOTH CTAs, same smem offset
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma2_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void mma2_commit(uint64_t *bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 // ---- descriptors ------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, SWIZZLE_NONE, K-major (bit layout: cute/arch/mma_sm100_desc.hpp,
-// SmemDescriptor): [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=0.
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
-// Instruction descriptor for kind::f16, A/B = bf16 K-major, D = fp32 (InstrDescriptor in the same header):
-// [4,6) c_format=1(F32) | [7,10) a_format=1(BF16) | [10,13) b_format=1 | 15 a_major=0 | 16 b_major=0 |
-// [17,23) N>>3 | [24,29) M>>4.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// One lane of a fully converged warp.  Issue loops run warp-uniform (all 32 lanes compute the descriptors, so they
-// live in uniform registers) and only the tcgen05 instruction itself sits under this predicate; issuing from inside
-// an `if (lane == 0)` region makes ptxas emit a per-MMA R2UR/ELECT "waterfall" loop (~70 cycles per instruction).
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-// descriptor = constant high part (LBO, SBO, version) | 14-bit start-address field
+// Shared-memory matrix descriptor of wgmma, no swizzle (layout type 0), K-major:
+// [0,14) start >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [49,52) base offset = 0 | [62,64) layout = 0.
+// descriptor = constant high part (LBO, SBO) | 14-bit start-address field
 __device__ __forceinline__ uint64_t desc_template(uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
+    return ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
 }
 __device__ __forceinline__ uint64_t desc_at(uint64_t tmpl, uint32_t saddr) { return tmpl | (uint64_t)((saddr >> 4) & 0x3FFF); }
 
-// D[tmem] (+)= A[smem] * B[smem]; one thread issues.
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
+// ---- warpgroup MMA ------------------------------------------------------------------------------
+// Every thread of the warpgroup executes these, converged.  Order per accumulator tile:
+//   wgmma_fence() (registers written by ordinary instructions become visible to the MMA), wgmma_bf16() x n,
+//   wgmma_commit(), wgmma_wait<k>() (at most k committed groups still in flight), then acc_fence() before the
+//   registers are read or written by ordinary code.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// Arrive on an mbarrier when every previously issued tcgen05.mma of this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-// the same arrival delivered to the mbarrier at this offset in every CTA of `cta_mask` (a slot shared through multicast is
-// free only when every consumer CTA's MMAs have read it)
-__device__ __forceinline__ void mma_commit_multicast(uint64_t *bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMA window
+template <int R>
+__device__ __forceinline__ void acc_fence(float *d) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void mma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
+// thread `t` (0..127 of its warpgroup): row of accumulator element d[4k + 2h + e], and column of d[j]
+__device__ __forceinline__ int frag_row(int t, int h) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h; }
+__host__ __device__ constexpr int frag_col(int lane_q, int j) { return 8 * (j >> 2) + 2 * lane_q + (j & 1); }
 
-// TMEM -> registers: 32 lanes x 32-bit, 16 consecutive columns per call.  Warp w (w%4) may only touch
-// lanes [32*(w%4), 32*(w%4)+32); taddr = base + (lane0 << 16) + column.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands in shared memory (K-major descriptors), D in the N/2 registers
+// d[0 .. N/2); scale_d = 0 overwrites D.  N = 32 on the first 16 registers of an N = 64 tile accumulates onto its first
+// 32 columns (the register layout of a column block does not depend on N).
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float *d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d);
+#define MG_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float *d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+                 : MG_D8(0), MG_D8(8)
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr)
-                 : "memory");
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float *d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : MG_D8(0), MG_D8(8), MG_D8(16), MG_D8(24)
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
+template <> __device__ __forceinline__ void wgmma_bf16<128>(float *d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : MG_D8(0), MG_D8(8), MG_D8(16), MG_D8(24), MG_D8(32), MG_D8(40), MG_D8(48), MG_D8(56)
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
+template <> __device__ __forceinline__ void wgmma_bf16<160>(float *d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79}, %80, %81, p, 1, 1, 0, 0;\n\t}"
+                 : MG_D8(0), MG_D8(8), MG_D8(16), MG_D8(24), MG_D8(32), MG_D8(40), MG_D8(48), MG_D8(56), MG_D8(64), MG_D8(72)
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]),
-                 "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
+template <> __device__ __forceinline__ void wgmma_bf16<256>(float *d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+                 : MG_D8(0), MG_D8(8), MG_D8(16), MG_D8(24), MG_D8(32), MG_D8(40), MG_D8(48), MG_D8(56), MG_D8(64), MG_D8(72), MG_D8(80), MG_D8(88), MG_D8(96), MG_D8(104), MG_D8(112), MG_D8(120)
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+#undef MG_D8
 
 // ---- bf16 hi/lo split ----------------------------------------------------------------------------
 // x ~= hi + lo with hi = bf16(x) (round-to-nearest), lo = bf16(x - hi): 16 significant bits, so the

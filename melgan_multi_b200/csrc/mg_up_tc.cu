@@ -1,4 +1,4 @@
-// LeakyReLU -> ConvTranspose1d on the tensor cores (tcgen05 + TMEM, split-bf16).
+// LeakyReLU -> ConvTranspose1d on the tensor cores (wgmma, split-bf16).
 //
 // Reference: Generator.forward, models.py:64-65 -- x = ups[i](F.leaky_relu(x)); ConvTranspose1d(Cin, Cout, K=2S, stride S,
 // padding S/2), models.py:48-51.
@@ -6,21 +6,23 @@
 // A transposed conv with K = 2S is, per output phase phi = (t + pad) mod S, a 2-tap conv over the INPUT positions:
 //     out[co][S*s + phi - pad] = sum_ci  x[ci][s] * W[ci][co][phi]  +  x[ci][s-1] * W[ci][co][phi + S]
 // All S phases of a tap read the same activation rows, so they are stacked along the MMA N dimension:
-//     D[s, phi*NG + co] (+)= X[s - tap, :] * Wstack_tap[phi*NG + co, :]^T,   M = 128 input positions (TMEM lane = s),
-//     N = S*NG (256 for the stride-8 stages: the largest UMMA shape), K = 16 per instruction,
+//     D[s, phi*NG + co] (+)= X[s - tap, :] * Wstack_tap[phi*NG + co, :]^T,   M = 64 input positions per warpgroup,
+//     N = S*NG (256 for the stride-8 stages), K = 16 per instruction,
 // i.e. 2 taps x 3 split-bf16 passes = 6 instructions per 16 input channels cover every phase.  The s-1 tap is the same
-// A buffer read one row earlier (row-linear operand layout, mg_tc.cuh).  Because all S phases of a (row block, channel
-// group) sit in TMEM together, the epilogue thread of input position s owns the S consecutive output samples
-// [S*s - pad, S*s - pad + S) of each channel and stores them as contiguous, fully coalesced vectors.
+// A buffer read one row earlier (row-linear operand layout, mg_tc.cuh).  Because all S phases of a (row, channel) sit in
+// the same thread's accumulator registers, the epilogue stores the S consecutive output samples [S*s - pad, S*s - pad + S)
+// of a channel as contiguous vectors.
 //
 // Rows are VIRTUAL input positions: the B batch items are concatenated with one zero row after each item
 // (v = item*(Lin+1) + s, s in [0, Lin], row s = Lin is zero), so that x[-1] = x[Lin] = 0 falls out of the layout and short
-// sequences (stage 0: Lin = 32) still fill 128-row blocks.
-// One CTA = NB blocks of 128 virtual input positions x one group of NG output channels.  K (= Cin) is streamed: the A
+// sequences (stage 0: Lin = 32) still fill 64-row blocks.
+// One CTA = NMW blocks of 64 virtual input positions x one group of NG output channels.  K (= Cin) is streamed: the A
 // slots (KCA channels: LeakyReLU + hi/lo split of x) are produced in shared memory by the converter warps straight from
 // the fp32 NCL input (all KCA loads of a row in flight at once), the B slots (16 channels: both taps, hi and lo, all
 // phases) arrive by 1-D bulk TMA from the pre-packed blob (mg_layout.h).
-// Warp roles: converter/epilogue warps, TMA producer, MMA issuer warps (one per row block).
+// Warp roles: converter warpgroup, NMW MMA warpgroups (one per 64-row block; accumulators in registers, they also run
+// the epilogue), TMA producer warp.  An N = 256 tile is 128 accumulator registers per thread, so the stride-8 stages run
+// one MMA warpgroup per CTA.
 #include "mg_common.cuh"
 #include "mg_tc.cuh"
 
@@ -34,64 +36,94 @@ struct UpCfg {
     static constexpr int NG = up_ng(STAGE);
     static constexpr int NCG = COUT / NG;
     static constexpr int N = S * NG;                      // MMA N: every phase of the channel group
-    static constexpr int NB = (S == 8) ? 1 : 2;          // 128-row blocks per CTA
-    static constexpr int COLS = NB * N;                   // TMEM columns in use
-    static constexpr int TCOLS = COLS <= 128 ? 128 : COLS <= 256 ? 256 : 512;
-    // stride-8 stages: 32 KB B slots, so one CTA per SM with a deep ring and 64-channel A slots (one memory round trip
-    // per 64 channels); stride-2 stages: small slots, two CTAs per SM hide each other's loads and stores.
-    static constexpr int MINB = (S == 8) ? 1 : 2;
-    // channels per A slot = channels fetched per memory round trip of a converter thread (measured: 16 -> 32 helps the
-    // stride-2 stages; a single 64-channel slot for stage 3 loses the conversion/MMA overlap and is slower)
+    static constexpr int NMW = (N > 128) ? 1 : 2;         // MMA warpgroups = 64-row blocks per CTA
+    // channels per A slot = channels fetched per memory round trip of a converter thread
     static constexpr int KCA = (S == 8) ? 64 : 32;
-    static constexpr int ROWS = 128 * NB;
+    static constexpr int ROWS = 64 * NMW;
     static constexpr int AROWS = ROWS + 8;                // row index i <-> virtual position r0 - 1 + i, i in [0, ROWS]
     static constexpr int APITCH = AROWS * 16;             // bytes between k-panels
     static constexpr int ASLOT = 2 * (KCA / 8) * APITCH;  // [half: hi, lo][k-panel][AROWS][16 B]
     static constexpr int BSLOT = up_slot_bytes(STAGE);    // [tap][half][k-panel: 2][N][16 B]
     static constexpr int NSA = (CIN == KCA) ? 1 : 2, NSB = (S == 8) ? 4 : (CIN >= 128 ? 2 : 3);
     static constexpr int NCHUNK = CIN / 16;               // B slots per tile
-    static constexpr int NWG = NB >= 2 ? 2 : 1;
-    static constexpr int NCONV = 128 * NWG;               // converter / epilogue threads
-    static constexpr int NIW = NB;                        // MMA issuer warps (one per row block)
-    static constexpr int NT = NCONV + 32 + 32 * NIW;
-    static constexpr int SMEM_BYTES = NSA * ASLOT + NSB * BSLOT + (2 * NSA + 2 * NSB + 1) * 8 + 16;
-    static_assert(N <= 256 && N % 16 == 0, "UMMA N");
-    static_assert(MINB * TCOLS <= 512, "TMEM columns");
-    static_assert(MINB * (SMEM_BYTES + 1024) <= 228 * 1024, "shared memory budget");
+    static constexpr int NCONV = 128;                     // converter threads
+    static constexpr int NT = NCONV + 128 * NMW + 32;
+    static constexpr int SMEM_BYTES = NSA * ASLOT + NSB * BSLOT + (2 * NSA + 2 * NSB) * 8;
+    static_assert(N <= 256 && N % 16 == 0, "wgmma N");
+    static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "shared memory budget");
     static_assert(CIN % KCA == 0, "A slot");
 };
 
+// D[s, phi*NG + co] + bias -> out[co][S*s + phi - pad] for the two accumulator rows of this thread (block-local rows
+// 64 mw + frag_row(t, h)); r0: first virtual row of the tile
 template <class Cfg>
-__global__ void __launch_bounds__(Cfg::NT, Cfg::MINB)
+__device__ __forceinline__ void convt_store(const float *acc, float *__restrict__ y, const float *__restrict__ bias, int r0, int t,
+                                            int cg, int Lin, int B) {
+    constexpr int S = Cfg::S, NG = Cfg::NG, N = Cfg::N, COUT = Cfg::COUT, PAD = Cfg::PAD;
+    const int Lout = Lin * S, Lv = Lin + 1, q = t & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int v = r0 + frag_row(t, h);
+        const int item = v / Lv, s = v - item * Lv;
+        const bool row_ok = item < B;
+        const bool lo_ok = row_ok && s >= 1, hi_ok = row_ok && s <= Lin - 1;
+        float *yb = y + ((size_t)(row_ok ? item : 0) * COUT + cg * NG) * Lout + (S * s - PAD);
+        if constexpr (S == 8) {
+            // column 8k + 2q + e = phi * 32 + co: block k holds phase k / 4 of channels 8 (k % 4) + 2q + e
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int co = 8 * c + 2 * q + e;
+                    const float bj = __ldg(bias + co);
+                    float *yp = yb + (size_t)co * Lout;
+                    if (lo_ok)
+                        *reinterpret_cast<float4 *>(yp) =
+                            make_float4(acc[4 * (0 + c) + 2 * h + e] + bj, acc[4 * (4 + c) + 2 * h + e] + bj,
+                                        acc[4 * (8 + c) + 2 * h + e] + bj, acc[4 * (12 + c) + 2 * h + e] + bj);
+                    if (hi_ok)
+                        *reinterpret_cast<float4 *>(yp + 4) =
+                            make_float4(acc[4 * (16 + c) + 2 * h + e] + bj, acc[4 * (20 + c) + 2 * h + e] + bj,
+                                        acc[4 * (24 + c) + 2 * h + e] + bj, acc[4 * (28 + c) + 2 * h + e] + bj);
+                }
+        } else {  // S == 2: out[2s - 1] (phase 0) and out[2s] (phase 1)
+#pragma unroll
+            for (int k = 0; k < N / 8; ++k)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = frag_col(q, 4 * k + e), phi = col / NG, co = col % NG;
+                    const float o = acc[4 * k + 2 * h + e] + __ldg(bias + co);
+                    if (phi == 0 ? lo_ok : hi_ok) yb[(size_t)co * Lout + phi] = o;
+                }
+        }
+    }
+}
+
+template <class Cfg>
+__global__ void __launch_bounds__(Cfg::NT, 1)
 convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed, int Lin, int B,
                 int *__restrict__ status) {
-    constexpr int CIN = Cfg::CIN, COUT = Cfg::COUT, S = Cfg::S, PAD = Cfg::PAD, NG = Cfg::NG, NB = Cfg::NB, N = Cfg::N;
+    constexpr int CIN = Cfg::CIN, N = Cfg::N, NG = Cfg::NG;
     constexpr int ROWS = Cfg::ROWS, APITCH = Cfg::APITCH, ASLOT = Cfg::ASLOT, BSLOT = Cfg::BSLOT, KCA = Cfg::KCA;
-    constexpr int NSA = Cfg::NSA, NSB = Cfg::NSB, NCHUNK = Cfg::NCHUNK, NCONV = Cfg::NCONV, NWG = Cfg::NWG, NIW = Cfg::NIW;
+    constexpr int NSA = Cfg::NSA, NSB = Cfg::NSB, NCHUNK = Cfg::NCHUNK, NCONV = Cfg::NCONV, NMW = Cfg::NMW;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *aring = smem, *bring = smem + NSA * ASLOT;
     uint64_t *fullA = reinterpret_cast<uint64_t *>(bring + NSB * BSLOT);
-    uint64_t *emptyA = fullA + NSA, *fullB = emptyA + NSA, *emptyB = fullB + NSB, *done = emptyB + NSB;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(done + 1);
+    uint64_t *emptyA = fullA + NSA, *fullB = emptyA + NSA, *emptyB = fullB + NSB;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * ROWS;  // first virtual row of the tile
     const int cg = blockIdx.y;
-    const int Lout = Lin * S, Lv = Lin + 1;
+    const int Lv = Lin + 1;
 
-    if (warp == 0) tmem_alloc(tmem_slot, Cfg::TCOLS);
-    if (tid == 32) {
-        for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NIW); }
-        for (int s = 0; s < NSB; ++s) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], NIW); }
-        mbar_init(done, NIW);
+    if (tid == 0) {
+        for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NMW); }
+        for (int s = 0; s < NSB; ++s) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], NMW); }
         fence_mbar_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == NCONV / 32) {
+    if (warp == (NCONV + 128 * NMW) / 32) {
         // ================= TMA producer: one B slot per 16 input channels =================
         if (lane == 0) {
             const uint8_t *src = reinterpret_cast<const uint8_t *>(packed) + tc_region_start() + tc_up_offset(Cfg::STAGE) +
@@ -106,24 +138,23 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
             }
             if (!ok) atomicExch(status, 12);
         }
-    } else if (warp > NCONV / 32) {
-        // ================= MMA issuers: warp iw owns row block iw (warp-uniform loop, one elected lane issues) =========
-        const int blk = warp - (NCONV / 32 + 1);
-        const uint32_t idesc = make_idesc_bf16(128, N);
+    } else if (warp >= NCONV / 32) {
+        // ================= MMA warpgroup mw: rows [64 mw, 64 mw + 64) =================
+        const int mw = warp / 4 - NCONV / 128, t = tid & 127;
         const uint64_t adesc_t = desc_template(APITCH, 128), bdesc_t = desc_template(N * 16, 128);
-        const uint32_t aring_addr = smem_u32(aring), bring_addr = smem_u32(bring);
-        int sa = 0, pha = 0, sb = 0, phb = 0;
+        const uint32_t aring_addr = smem_u32(aring) + mw * 64 * 16, bring_addr = smem_u32(bring);
+        float acc[N / 2];
+        int sa = 0, pha = 0, sb = 0, phb = 0, psb = -1, psa = -1;
         bool ok = true;  // a timed-out wait only raises the status word: control flow stays uniform
 #pragma unroll 1
         for (int ca = 0; ca < CIN / KCA; ++ca) {
             ok &= mbar_wait(&fullA[sa], pha);
-            tc_fence_after();
-            const uint64_t abase = desc_at(adesc_t, aring_addr + sa * ASLOT + (blk * 128) * 16);
+            const uint64_t abase = desc_at(adesc_t, aring_addr + sa * ASLOT);
 #pragma unroll 1
             for (int j = 0; j < KCA / 16; ++j) {
                 ok &= mbar_wait(&fullB[sb], phb);
-                tc_fence_after();
                 const uint64_t bbase = desc_at(bdesc_t, bring_addr + sb * BSLOT);
+                wgmma_fence();
 #pragma unroll
                 for (int tap = 0; tap < 2; ++tap)
 #pragma unroll
@@ -132,17 +163,26 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
                         const uint64_t bdesc = bbase + (uint64_t)((((tap * 2 + bhalf) * 2) * N * 16) >> 4);
                         const uint64_t adesc =
                             abase + (uint64_t)((ahalf * (KCA / 8) * APITCH + (1 - tap) * 16) >> 4) + (uint64_t)(2 * j * (APITCH >> 4));
-                        const bool acc = !(ca == 0 && j == 0 && tap == 0 && pass == 0);
-                        if (elect_one()) mma_bf16(tmem + blk * N, adesc, bdesc, idesc, acc);
+                        wgmma_bf16<N>(acc, adesc, bdesc, (ca | j | tap | pass) != 0);
                     }
-                if (elect_one()) mma_commit(&emptyB[sb]);
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (t == 0 && psb >= 0) {
+                    mbar_arrive(&emptyB[psb]);
+                    if (psa >= 0) mbar_arrive(&emptyA[psa]);
+                }
+                psb = sb;
+                psa = (j == KCA / 16 - 1) ? sa : -1;
                 if (++sb == NSB) { sb = 0; phb ^= 1; }
             }
-            if (elect_one()) mma_commit(&emptyA[sa]);
             if (++sa == NSA) { sa = 0; pha ^= 1; }
         }
-        if (elect_one()) mma_commit(done);
-        if (!ok && lane == 0) atomicExch(status, 13);
+        wgmma_wait<0>();
+        acc_fence<N / 2>(acc);
+        if (!ok && t == 0) atomicExch(status, 13);
+        pdl_trigger();  // MMAs done, only the output store is left: the next kernel of the chain may be scheduled
+        pdl_wait();
+        convt_store<Cfg>(acc, y, packed + bias_offset(1 + Cfg::STAGE) + cg * NG, r0 + 64 * mw, t, cg, Lin, B);
     } else {
         // ================= converter warps: A slots = split(lrelu(x)), KCA channels of every row =================
         pdl_wait();  // x: the previous kernel's output
@@ -174,61 +214,7 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
             mbar_arrive(&fullA[sa]);
             if (++sa == NSA) { sa = 0; pha ^= 1; }
         }
-        // ================= epilogue: D[s, phi*NG + co] + bias -> out[co][S*s + phi - pad] =================
-        if (ok && !mbar_wait(done, 0)) { ok = false; if (lane == 0) atomicExch(status, 15); }
-        tc_fence_after();
-        pdl_trigger();  // MMAs done, only the output store is left: the next kernel of the chain may be scheduled
-        const int wg = warp >> 2, q = warp & 3;
-        const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-        const float *bias = packed + bias_offset(1 + Cfg::STAGE) + cg * NG;
-        for (int blk = wg; blk < NB; blk += NWG) {
-            const int v = r0 + blk * 128 + q * 32 + lane;
-            const int item = v / Lv, s = v - item * Lv;
-            const bool row_ok = item < B;
-            const int t0 = S * s - PAD;  // first output sample owned by this input position
-            float *yb = y + ((size_t)(row_ok ? item : 0) * COUT + cg * NG) * Lout;
-            if (S == 8) {
-                const bool lo_ok = row_ok && s >= 1, hi_ok = row_ok && s <= Lin - 1;
-#pragma unroll 1
-                for (int j0 = 0; j0 < NG; j0 += 8) {
-                    uint32_t w[8][8];
-#pragma unroll
-                    for (int phi = 0; phi < 8; ++phi) tmem_ld8(lane_addr + blk * N + phi * NG + j0, w[phi]);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float bj = __ldg(bias + j0 + j);
-                        float *yp = yb + (size_t)(j0 + j) * Lout + t0;
-                        if (lo_ok)
-                            *reinterpret_cast<float4 *>(yp) = make_float4(__uint_as_float(w[0][j]) + bj, __uint_as_float(w[1][j]) + bj,
-                                                                          __uint_as_float(w[2][j]) + bj, __uint_as_float(w[3][j]) + bj);
-                        if (hi_ok)
-                            *reinterpret_cast<float4 *>(yp + 4) = make_float4(__uint_as_float(w[4][j]) + bj, __uint_as_float(w[5][j]) + bj,
-                                                                              __uint_as_float(w[6][j]) + bj, __uint_as_float(w[7][j]) + bj);
-                    }
-                }
-            } else {  // S == 2: t0 = 2s - 1
-                const bool lo_ok = row_ok && s >= 1, hi_ok = row_ok && s <= Lin - 1;
-#pragma unroll 1
-                for (int j0 = 0; j0 < NG; j0 += 16) {
-                    uint32_t v0[16], v1[16];
-                    tmem_ld16(lane_addr + blk * N + j0, v0);
-                    tmem_ld16(lane_addr + blk * N + NG + j0, v1);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float bj = __ldg(bias + j0 + j);
-                        float *yp = yb + (size_t)(j0 + j) * Lout + t0;
-                        if (lo_ok) yp[0] = __uint_as_float(v0[j]) + bj;
-                        if (hi_ok) yp[1] = __uint_as_float(v1[j]) + bj;
-                    }
-                }
-            }
-        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, Cfg::TCOLS);
 }
 
 template <class Cfg>
@@ -240,48 +226,41 @@ static int launch_convt(const float *x, float *y, const float *packed, int B, in
     }
     const long long vrows = (long long)B * (Lin + 1);  // Lin + 1 rows per item: position s = Lin feeds the last `pad` outputs
     dim3 grid((unsigned)((vrows + Cfg::ROWS - 1) / Cfg::ROWS), Cfg::NCG);
-    MG_CUDA_TRY(launch_ex(convt_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, 1, true, x, y, packed, Lin, B, status));
+    MG_CUDA_TRY(launch_ex(convt_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, x, y, packed, Lin, B, status));
     return MG_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Variant for a stage whose whole activation tile fits in shared memory (stage 1: 129 rows x 256 channels, hi+lo =
-// 136 KB): the A operand is converted ONCE per row tile and stays resident, and the CTA loops over the NCG output-channel
-// groups with the accumulators double-buffered in TMEM (2 x 256 columns), so the epilogue (TMEM -> coalesced vector
-// stores) of group g overlaps the MMAs of group g+1 and no activation is loaded or converted twice.
+// Variant for a stage whose whole activation tile fits in shared memory (stage 1: 65 rows x 256 channels, hi+lo =
+// 72 KB): the A operand is converted ONCE per row tile and stays resident, and the CTA loops over the NCG output-channel
+// groups, so no activation is loaded or converted twice.  One MMA warpgroup (64 rows, N = 256) per CTA.
 template <class Cfg>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(Cfg::NCONV + 128 + 32, 1)
 convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed, int Lin, int B,
                          int *__restrict__ status) {
-    constexpr int CIN = Cfg::CIN, COUT = Cfg::COUT, S = Cfg::S, PAD = Cfg::PAD, NG = Cfg::NG, N = Cfg::N, NCG = Cfg::NCG;
-    constexpr int ROWS = 128, APITCH = Cfg::APITCH, BSLOT = Cfg::BSLOT, NCHUNK = Cfg::NCHUNK;
+    constexpr int CIN = Cfg::CIN, NG = Cfg::NG, N = Cfg::N, NCG = Cfg::NCG;
+    constexpr int ROWS = 64, APITCH = Cfg::APITCH, BSLOT = Cfg::BSLOT, NCHUNK = Cfg::NCHUNK;
     constexpr int KPT = CIN / 8;                    // k-panels of the resident A
     constexpr int AHALF = KPT * APITCH;             // bytes of one of {hi, lo}
-    constexpr int NSB = 2, NCONV = 128;
-    static_assert(S == 8 && N == 256 && 2 * AHALF + NSB * BSLOT + 256 <= 227 * 1024, "resident ConvT shape");
+    constexpr int NSB = 4, NCONV = Cfg::NCONV;
+    static_assert(Cfg::S == 8 && N == 256 && Cfg::NMW == 1 && 2 * AHALF + NSB * BSLOT + 256 <= 227 * 1024, "resident ConvT shape");
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *abuf = smem, *bring = smem + 2 * AHALF;
     uint64_t *fullA = reinterpret_cast<uint64_t *>(bring + NSB * BSLOT);  // [CIN/64]: a 64-channel slice of A is written
-    uint64_t *fullB = fullA + CIN / 64, *emptyB = fullB + NSB, *done = emptyB + NSB, *tfree = done + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tfree + 2);
+    uint64_t *fullB = fullA + CIN / 64, *emptyB = fullB + NSB;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * ROWS;
-    const int Lout = Lin * S, Lv = Lin + 1;
+    const int Lv = Lin + 1;
 
-    if (warp == 0) tmem_alloc(tmem_slot, 512);
-    if (tid == 32) {
+    if (tid == 0) {
         for (int s = 0; s < CIN / 64; ++s) mbar_init(&fullA[s], NCONV);
         for (int s = 0; s < NSB; ++s) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&done[s], 1); mbar_init(&tfree[s], NCONV); }
         fence_mbar_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == NCONV / 32) {
+    if (warp == NCONV / 32 + 4) {
         // ================= TMA producer: B slots of every channel group, in consumption order =================
         if (lane == 0) {
             const uint8_t *src = reinterpret_cast<const uint8_t *>(packed) + tc_region_start() + tc_up_offset(Cfg::STAGE);
@@ -295,46 +274,46 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
             }
             if (!ok) atomicExch(status, 32);
         }
-    } else if (warp == NCONV / 32 + 1) {
-        // ================= MMA issuer =================
-        const uint32_t idesc = make_idesc_bf16(128, N);
+    } else if (warp >= NCONV / 32) {
+        // ================= MMA warpgroup: one channel group after the other =================
+        const int t = tid & 127;
         const uint64_t adesc_t = desc_template(APITCH, 128), bdesc_t = desc_template(N * 16, 128);
         const uint32_t a_addr = smem_u32(abuf), bring_addr = smem_u32(bring);
-        int sb = 0, phb = 0;
+        float acc[N / 2];
+        int sb = 0, phb = 0, psb = -1;
         bool ok = true;
 #pragma unroll 1
         for (int cg = 0; cg < NCG; ++cg) {
-            const int buf = cg & 1, use = cg >> 1;
-            if (use > 0) {  // the epilogue must have drained this accumulator buffer (group cg - 2)
-                ok &= mbar_wait(&tfree[buf], (use - 1) & 1);
-                tc_fence_after();
-            }
 #pragma unroll 1
             for (int ch = 0; ch < NCHUNK; ++ch) {
-                if (cg == 0 && (ch & 3) == 0) {  // first pass only: wait for the 64-channel slice of A
-                    ok &= mbar_wait(&fullA[ch >> 2], 0);
-                    tc_fence_after();
-                }
+                if (cg == 0 && (ch & 3) == 0) ok &= mbar_wait(&fullA[ch >> 2], 0);  // first pass only: the 64-channel slice of A
                 ok &= mbar_wait(&fullB[sb], phb);
-                tc_fence_after();
                 const uint64_t bbase = desc_at(bdesc_t, bring_addr + sb * BSLOT);
                 const uint64_t abase = desc_at(adesc_t, a_addr + 2 * ch * APITCH);
+                wgmma_fence();
 #pragma unroll
                 for (int tap = 0; tap < 2; ++tap)
 #pragma unroll
                     for (int pass = 0; pass < 3; ++pass) {
                         const uint64_t bdesc = bbase + (uint64_t)((((tap * 2 + (pass == 2)) * 2) * N * 16) >> 4);
                         const uint64_t adesc = abase + (uint64_t)((((pass == 1) ? AHALF : 0) + (1 - tap) * 16) >> 4);
-                        const bool acc = !(ch == 0 && tap == 0 && pass == 0);
-                        if (elect_one()) mma_bf16(tmem + buf * N, adesc, bdesc, idesc, acc);
+                        wgmma_bf16<N>(acc, adesc, bdesc, (ch | tap | pass) != 0);
                     }
-                if (elect_one()) mma_commit(&emptyB[sb]);
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (t == 0 && psb >= 0) mbar_arrive(&emptyB[psb]);
+                psb = sb;
                 if (++sb == NSB) { sb = 0; phb ^= 1; }
             }
-            if (elect_one()) mma_commit(&done[buf]);
+            wgmma_wait<0>();
+            acc_fence<N / 2>(acc);
+            if (t == 0) { mbar_arrive(&emptyB[psb]); psb = -1; }
+            if (cg == NCG - 1) pdl_trigger();  // last channel group's MMAs done: the next kernel may be scheduled
+            if (cg == 0) pdl_wait();
+            convt_store<Cfg>(acc, y, packed + bias_offset(1 + Cfg::STAGE) + cg * NG, r0, t, cg, Lin, B);
         }
-        if (!ok && lane == 0) atomicExch(status, 33);
-    } else if (warp < NCONV / 32) {
+        if (!ok && t == 0) atomicExch(status, 33);
+    } else {
         // ================= converter: the whole A tile, once =================
         pdl_wait();  // x: the previous kernel's output
 #pragma unroll 1
@@ -360,61 +339,20 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
             fence_proxy_async();
             mbar_arrive(&fullA[ca]);
         }
-        // ================= epilogue per channel group (overlaps the next group's MMAs) =================
-        const int q = warp & 3;
-        const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-        const int v = r0 + q * 32 + lane;
-        const int item = v / Lv, s = v - item * Lv;
-        const bool row_ok = item < B;
-        const int t0 = S * s - PAD;
-        const bool lo_ok = row_ok && s >= 1, hi_ok = row_ok && s <= Lin - 1;
-        bool ok = true;
-#pragma unroll 1
-        for (int cg = 0; cg < NCG; ++cg) {
-            const int buf = cg & 1, use = cg >> 1;
-            if (ok && !mbar_wait(&done[buf], use & 1)) { ok = false; if (lane == 0) atomicExch(status, 35); }
-            tc_fence_after();
-            if (cg == NCG - 1) pdl_trigger();  // last channel group's MMAs done: the next kernel may be scheduled
-            const float *bias = packed + bias_offset(1 + Cfg::STAGE) + cg * NG;
-            float *yb = y + ((size_t)(row_ok ? item : 0) * COUT + cg * NG) * Lout;
-#pragma unroll 1
-            for (int j0 = 0; j0 < NG; j0 += 8) {
-                uint32_t w[8][8];
-#pragma unroll
-                for (int phi = 0; phi < 8; ++phi) tmem_ld8(lane_addr + buf * N + phi * NG + j0, w[phi]);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float bj = __ldg(bias + j0 + j);
-                    float *yp = yb + (size_t)(j0 + j) * Lout + t0;
-                    if (lo_ok)
-                        *reinterpret_cast<float4 *>(yp) = make_float4(__uint_as_float(w[0][j]) + bj, __uint_as_float(w[1][j]) + bj,
-                                                                      __uint_as_float(w[2][j]) + bj, __uint_as_float(w[3][j]) + bj);
-                    if (hi_ok)
-                        *reinterpret_cast<float4 *>(yp + 4) = make_float4(__uint_as_float(w[4][j]) + bj, __uint_as_float(w[5][j]) + bj,
-                                                                          __uint_as_float(w[6][j]) + bj, __uint_as_float(w[7][j]) + bj);
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&tfree[buf]);  // accumulator buffer may be overwritten by group cg + 2
-        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 512);
 }
 
 template <class Cfg>
 static int launch_convt_resident(const float *x, float *y, const float *packed, int B, int Lin, int *status, cudaStream_t s) {
-    constexpr int smem = 2 * (Cfg::CIN / 8) * Cfg::APITCH + 2 * Cfg::BSLOT + (Cfg::CIN / 64 + 2 * 2 + 4) * 8 + 16;
+    constexpr int smem = 2 * (Cfg::CIN / 8) * Cfg::APITCH + 4 * Cfg::BSLOT + (Cfg::CIN / 64 + 2 * 4) * 8;
     static bool configured = false;
     if (!configured) {
         MG_CUDA_TRY(cudaFuncSetAttribute(convt_resident_tc_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         configured = true;
     }
     const long long vrows = (long long)B * (Lin + 1);
-    MG_CUDA_TRY(launch_ex(convt_resident_tc_kernel<Cfg>, dim3((unsigned)((vrows + 127) / 128)), dim3(192), smem, s, 1, true, x, y,
-                          packed, Lin, B, status));
+    MG_CUDA_TRY(launch_ex(convt_resident_tc_kernel<Cfg>, dim3((unsigned)((vrows + 63) / 64)), dim3(Cfg::NCONV + 128 + 32), smem, s,
+                          true, x, y, packed, Lin, B, status));
     return MG_OK;
 }
 

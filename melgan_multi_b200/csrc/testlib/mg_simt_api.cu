@@ -1,5 +1,5 @@
 // C entry point of libmelgan_b200_simt_test.so: the first-generation fp32 SIMT generator (mg_gen_simt.cu), kept as an
-// independent second implementation that tests cross-check the tcgen05 product path against.  TEST INFRASTRUCTURE: nothing
+// independent second implementation that tests cross-check the wgmma product path against.  TEST INFRASTRUCTURE: nothing
 // in the product library or the package links or loads this; only tests/test_simt_crosscheck_gpu.py does.
 #include "../mg_common.cuh"
 

@@ -2,7 +2,7 @@
 
 PyTorch is plumbing here: it owns device memory and streams; every kernel that runs on the hot
 path lives in the shared library.  There is no CPU or eager-PyTorch fallback: if the library
-is missing, or the device is not sm_100, calls raise.
+is missing, or the device is not sm_90 (H100), calls raise.
 """
 import ctypes
 import os
@@ -149,7 +149,7 @@ def _ptr_array(ptrs):
 
 
 class _StatusWatch:
-    """The tcgen05 kernels bound every mbarrier wait and, on a timeout, raise a device status word and carry on (a hung
+    """The tensor-core kernels bound every mbarrier wait and, on a timeout, raise a device status word and carry on (a hung
     GPU box is worse than a failed call).  A forward must therefore never be trusted silently: after each one the status
     word is copied to pinned host memory on the same stream (4 bytes, asynchronous), and the copy is inspected at the
     next forward of the same module, or at the next host synchronisation point the training loop has anyway
@@ -208,7 +208,7 @@ class GeneratorDevice:
         self.torch = torch
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise EngineError("the B200 engine runs on CUDA devices only (got %s)" % (device,))
+            raise EngineError("the native engine runs on CUDA devices only (got %s)" % (device,))
         with torch.cuda.device(self.device):
             check(lib().mg_device_check())
         self.packed = torch.empty((lib().mg_gen_packed_bytes() + 3) // 4, dtype=torch.float32, device=self.device)
@@ -448,7 +448,7 @@ class DiscriminatorDevice:
         self.device = torch.device(device)
         self.ndisc = ndisc
         if self.device.type != "cuda":
-            raise EngineError("the B200 engine runs on CUDA devices only (got %s)" % (device,))
+            raise EngineError("the native engine runs on CUDA devices only (got %s)" % (device,))
         if ndisc not in (1, 3):
             raise EngineError("DiscriminatorDevice: ndisc must be 1 or 3")
         with torch.cuda.device(self.device):
@@ -552,7 +552,7 @@ class DiscriminatorDevice:
         return dx, dw, db
 
     def post1_dgrad(self, scale, dz):
-        """dx of conv_post1 of discriminator `scale` from dz [Bt, 1024, L] (tcgen05, transposed weight copy of the blob)."""
+        """dx of conv_post1 of discriminator `scale` from dz [Bt, 1024, L] (wgmma, transposed weight copy of the blob)."""
         torch = self.torch
         dz = dz.contiguous()
         Bt, C, L = dz.shape
@@ -586,7 +586,7 @@ class DiscriminatorDevice:
         return dx, dw, db
 
     def post1_wgrad(self, x, dz):
-        """(dW [1024, 1024, 5], db [1024]) of conv_post1 from its input x and dz, both [Bt, 1024, L] (tcgen05, split-bf16)."""
+        """(dW [1024, 1024, 5], db [1024]) of conv_post1 from its input x and dz, both [Bt, 1024, L] (wgmma, split-bf16)."""
         torch = self.torch
         x, dz = x.contiguous(), dz.contiguous()
         Bt, C, L = dz.shape

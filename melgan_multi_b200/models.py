@@ -8,18 +8,18 @@ registration order (so reference checkpoints and Adam state load, SURVEY 8b), an
 all-reduce wrapper (distributed.py:90-142) hooks them unchanged.
 
 What runs where
-  * ``Generator.forward`` (models.py:61-71 in the reference): eight hand-written sm_100a tcgen05 kernels in
+  * ``Generator.forward`` (models.py:61-71 in the reference): eight hand-written sm_90a wgmma kernels in
     libmelgan_b200.so -- conv_pre, then LeakyReLU -> ConvTranspose1d and the fused six-conv ResBlock of each stage,
     the last stage as ONE kernel (its stride-2 ConvT, the ResBlock and LeakyReLU -> conv_post -> tanh) -- plus one launch that folds weight-norm for all 30 layers
     whenever the parameters changed.  CUDA only; a CPU tensor raises (the reference's CPU path lives in oracle/ as
     test infrastructure).
   * ``MultiScaleDiscriminator.forward`` (models.py:119-135, Discriminator.forward :87-103) on CUDA: real and generated
     audio are stacked into one batch and run through hand-written kernels -- AvgPool chain fused into each scale's
-    conv_pre, grouped k41 convs and conv_post1 on tcgen05 -- after one launch that folds weight-norm for the 21 layers.
+    conv_pre, grouped k41 convs and conv_post1 on wgmma -- after one launch that folds weight-norm for the 21 layers.
   * ``feature_loss`` / ``generator_loss`` / ``discriminator_loss`` (models.py:138-167) on CUDA tensors: every term of a
     loss is a row of one fused reduction launch (forward) and one gradient launch (backward).
   * Backward: the generator's runs as recomputation through stock PyTorch ops; the discriminators' walks the saved
-    feature maps layer by layer on hand-written kernels only (grouped convs, conv_post1 dgrad / wgrad on tcgen05,
+    feature maps layer by layer on hand-written kernels only (grouped convs, conv_post1 dgrad / wgrad on wgmma,
     conv_pre / conv_post2, LeakyReLU, weight-norm): no cuDNN call in a discriminator's backward.
 """
 import torch
@@ -70,7 +70,7 @@ def _layer_modules(gen):
 
 
 class _GeneratorFunction(torch.autograd.Function):
-    """Forward on the fused sm_100a kernels; backward by recomputation through stock PyTorch ops (open row: native
+    """Forward on the fused sm_90a kernels; backward by recomputation through stock PyTorch ops (open row: native
     backward).  The recomputation -- 30 convs forward, their backward, weight-norm: ~600 launches that cost the host more
     than the GPU -- is captured ONCE per input shape as a pair of CUDA graphs (torch.cuda.make_graphed_callables) and
     replayed, so the step is no longer bound by eager launch overhead (MG_GEN_BWD_GRAPH=0: eager).
@@ -126,7 +126,7 @@ class Generator(nn.Module):
         dev = vs[0].device
         if dev.type != "cuda":
             raise _engine.EngineError(
-                "melgan_multi_b200.Generator runs on CUDA (sm_100a) only; move the module with .to('cuda'). "
+                "melgan_multi_b200.Generator runs on CUDA (sm_90a) only; move the module with .to('cuda'). "
                 "There is deliberately no CPU fallback.")
         if self._dev is None or self._dev.device != dev:
             self._dev = _engine.GeneratorDevice(dev)
@@ -163,8 +163,8 @@ class Generator(nn.Module):
 
     # -- stock-PyTorch restatement, used ONLY to differentiate (backward) ---------------------
     def _torch_forward(self, x, leaves):
-        # (the same graph on channels_last 4-D tensors through conv2d saves cuDNN's nchw<->nhwc conversions -- 0.7 ms eager,
-        #  ~0.2 ms under the CUDA graph, scripts/gen_bwd_layout_ab.py -- but picks TF32 kernels whose rounding puts the deepest
+        # (the same graph on channels_last 4-D tensors through conv2d saves cuDNN's nchw<->nhwc conversions --
+        #  scripts/gen_bwd_layout_ab.py -- but picks TF32 kernels whose rounding puts the deepest
         #  layers' weight_g gradients AT the 5e-3 digest tolerance of tests/test_train_gpu.py on the small case: not taken)
         ws = [torch._weight_norm(leaves[3 * i], leaves[3 * i + 1], 0) for i in range(30)]
         bs = [leaves[3 * i + 2] for i in range(30)]
@@ -196,7 +196,7 @@ class Generator(nn.Module):
 class Discriminator(nn.Module):
     """One discriminator (reference models.py:74-103).  Inside ``MultiScaleDiscriminator`` (its only caller in the
     reference, models.py:109-113) the three of them run as one fused pipeline on the stacked real + generated batch;
-    called on its own, ``forward(x)`` runs the same sm_100a kernels on this module's weights and returns
+    called on its own, ``forward(x)`` runs the same sm_90a kernels on this module's weights and returns
     ``(flattened logits, [7 feature maps])`` like the reference's.  CUDA only, no stock-op fallback."""
 
     def __init__(self):
@@ -248,10 +248,10 @@ class Discriminator(nn.Module):
 
 
 class _MSDFunction(torch.autograd.Function):
-    """ONE discriminator of the stack as an autograd node: forward on the fused sm_100a kernels, backward layer by layer on
+    """ONE discriminator of the stack as an autograd node: forward on the fused sm_90a kernels, backward layer by layer on
     the saved feature maps without recomputing the forward -- the grouped k41 convs (layers 1..4) and weight-norm on the
     hand-written kernels of csrc/mg_disc_bwd.cu (cuDNN launches one kernel per group for them), conv_post1 (88 % of the
-    FLOPs) on the tcgen05 kernels of csrc/mg_conv_tc.cu (dgrad, transposed weight copy) and csrc/mg_wgrad_tc.cu (wgrad),
+    FLOPs) on the wgmma kernels of csrc/mg_conv_tc.cu (dgrad, transposed weight copy) and csrc/mg_wgrad_tc.cu (wgrad),
     conv_pre / conv_post2 on the bandwidth-bound kernels of csrc/mg_disc_edge_bwd.cu.  No aten / cuDNN call is left.
 
     The three scales of a MultiScaleDiscriminator are three nodes that share one forward: the first node to run launches the
@@ -281,7 +281,7 @@ class _MSDFunction(torch.autograd.Function):
         for k in range(s):  # the scale's input: the AvgPool chain of models.py:114-117,125-127
             x0 = host.meanpools[k](x0)
         # one host call walks the seven layers and enqueues every kernel (csrc/mg_disc_bwd_chain.cu): LeakyReLU', grouped convs,
-        # conv_post1 dgrad / wgrad on tcgen05, conv_pre / conv_post2 -- the step was bound by per-kernel Python launches
+        # conv_post1 dgrad / wgrad on wgmma, conv_pre / conv_post2 -- the step was bound by per-kernel Python launches
         g, dws, dbs = dev.scale_backward(s, x0, fm, grads, need_y)
         gy = None
         if need_y and g is not None:  # back through the (linear) AvgPool chain: differentiate it on zeros
@@ -363,7 +363,7 @@ class MultiScaleDiscriminator(nn.Module):
         # The reference's four lists.  Every element is an ordinary autograd slice of the stacked map (any use of it
         # differentiates correctly), and is also tagged with the stacked tensor it is a half of: the package's own loss
         # functions then work on the stacked tensors directly -- one gradient tensor per map instead of two zero-padded
-        # slice gradients and their sum (SliceBackward + add_: ~1000 launches and 3 ms per training step).
+        # slice gradients and their sum (SliceBackward + add_: ~1000 launches per training step).
         def half(f, h, flat=False):
             t = f[h * B:(h + 1) * B]
             if flat:
@@ -487,7 +487,7 @@ def discriminator_loss(disc_real_outputs, disc_generated_outputs):
     means = _row_means(rows, [None] * (2 * k), [_engine.LOSS_ONE_MINUS_SQ] * k + [_engine.LOSS_SQ] * k)
     vals = means.detach().tolist()
     # the read-back above synchronised the stream: every forward enqueued before it has finished, so its pipeline status
-    # word (engine._StatusWatch) can be inspected here at no cost -- a stalled tcgen05 pipeline raises instead of training on
+    # word (engine._StatusWatch) can be inspected here at no cost -- a stalled tensor-core pipeline raises instead of training on
     _engine.poll_status()
     return means.sum(), vals[:k], vals[k:]
 

@@ -4,7 +4,7 @@ Drop-in for the ``torch.optim.Adam(model.parameters(), lr, betas=[b1, b2])`` the
 train.py:51-52: same constructor arguments, same update arithmetic (L2 weight decay, no amsgrad), same per-parameter
 state keys (``step``, ``exp_avg``, ``exp_avg_sq``), so optimizer checkpoints written by either load into the other
 (train.py:27-29,36-37).  The reference's optimizer issues ~10 foreach launches sequences over 90 / 63 tensors per step
-(1.5 ms at BASELINE config 3); here a step is one launch driven by a device-side pointer table that is rebuilt only when
+per step; here a step is one launch driven by a device-side pointer table that is rebuilt only when
 a tensor moved.  CUDA fp32 parameters only.
 """
 import ctypes

@@ -1,4 +1,4 @@
-"""Accuracy margin of the split-bf16 tcgen05 pipeline (context evidence; the parity tests proper are tests/ against the
+"""Accuracy margin of the split-bf16 wgmma pipeline (context evidence; the parity tests proper are tests/ against the
 oracle and the reference goldens): config 2 (B=64, T=32) generator forward and the MSD forward against the stock-PyTorch
 restatement of the same modules in strict fp32 on the same GPU, over several weight seeds and input distributions
 (standard normal, and log-mel-like U(-11.5, 2): meldataset.py:22).  Tolerance of BASELINE north_star: 1e-3."""

@@ -1,5 +1,5 @@
 """Context numbers (NOT part of bench.py's contract): the same forwards run by stock PyTorch ops (cuDNN/ATen) on the same
-B200, TF32 (PyTorch default) and strict fp32, next to this engine.  Uses the torch restatements that the autograd path
+GPU, TF32 (PyTorch default) and strict fp32, next to this engine.  Uses the torch restatements that the autograd path
 keeps anyway (Generator._torch_forward / MultiScaleDiscriminator._torch_forward).  CUDA events, L2 flushed between steps."""
 import json
 import sys

@@ -1,4 +1,4 @@
-"""conv_post1 (Conv1d 1024 -> 1024, k5) backward at the three training shapes (2 x 16 items of 8192 samples: 128 / 65 / 33 positions): the tcgen05
+"""conv_post1 (Conv1d 1024 -> 1024, k5) backward at the three training shapes (2 x 16 items of 8192 samples: 128 / 65 / 33 positions): the wgmma
 data- and weight-gradient kernels (split-bf16, fp32-grade) against aten.convolution_backward (cuDNN, TF32 default)."""
 import json
 import sys

@@ -23,13 +23,13 @@ with torch.no_grad():
     if os.environ.get("MG_GEN_SLICES"):  # two batch-slice chains on forked streams
         y2 = g(torch.from_numpy(synth.mel_input(2, 3, 6)).cuda())
         g._dev.check_status(2, 3)
-    # T = 40: stage 0 is 320 positions -> CTA pairs (DSMEM boundary exchange, multicast weights), tensor-map TMA input slabs
-    # (every stage length is a multiple of 4), tail ConvT with its fp32 fix-up, several tiles per item in the later stages
+    # T = 40: stage 0 is 320 positions -> several 64-position tiles per item, several tiles per item in the later stages,
+    # stage 3's ConvT fused at the front of the last kernel
     y3 = g(torch.from_numpy(synth.mel_input(1, 40, 9)).cuda())
     g._dev.check_status(1, 40)
-    # the unfused chain (one kernel per ConvT / ResBlock) and the mel front end
+    # the chain with stage 1's and 3's ConvTs at the tail of the previous ResBlock (fp32 fix-up included) and the mel front end
     from melgan_multi_b200 import engine, meldataset
-    engine.check(engine.lib().mg_gen_set_pipeline(0))
+    engine.check(engine.lib().mg_gen_set_pipeline(0b1010))
     y4 = g(torch.from_numpy(synth.mel_input(1, 5, 10)).cuda())
     g._dev.check_status(1, 5)
     engine.check(engine.lib().mg_gen_set_pipeline(-1))

@@ -1,9 +1,8 @@
 """Generate the golden fixtures in tests/golden/ by running the UNMODIFIED reference.
 
-Run in the build container only (it imports /root/reference/models.py, which does not exist
-on the GPU box):
+Needs a checkout of the reference repository (its models.py is imported):
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py --reference <reference checkout> [--config2 | --train-step | --train-step-b16]
 
 Weights come from melgan_multi_b200.synth (seeded numpy MT19937), loaded into the reference
 modules through load_state_dict, so the fixtures hold inputs' seeds and the reference's
@@ -19,7 +18,9 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+if "--reference" not in sys.argv[:-1]:
+    raise SystemExit(__doc__)
+sys.path.insert(0, os.path.abspath(sys.argv[sys.argv.index("--reference") + 1]))
 warnings.filterwarnings("ignore")
 
 import models as ref_models  # noqa: E402  (the reference)
@@ -65,15 +66,26 @@ def grad_digest(named_params):
 TRAIN_CASE_B16 = dict(B=16, T=32, mel_seed=0, audio_seed=0)  # BASELINE config 3: batch 16, 8192-sample segments
 
 
+def config2_positions():
+    return np.sort(np.random.RandomState(8192).choice(8192, 1536, replace=False))
+
+
+def fold_rows():
+    """the 64 of conv_pre's 512 output rows whose folded weights are stored (the whole tensor is 1.1 MB)"""
+    return np.sort(np.random.RandomState(512).choice(512, 64, replace=False))
+
+
 def config2_golden():
     """BASELINE config 2 at full size (B=64, 80x32 mel -> 64x8192 samples) through the unmodified reference on CPU, for
-    N(0,1) and log-mel-like inputs (2 x 2 MB): every item of the bench workload is pinned, not just item 0."""
+    N(0,1) and log-mel-like inputs: every item of the bench workload is pinned, not just item 0, at the same fixed, seeded
+    1536 of its 8192 positions (the whole output would be a 4 MB fixture)."""
     gen = load_state(ref_models.Generator(), synth.generator_state(1234))
-    out = {}
+    pos = config2_positions()
+    out = {"gen_B64_T32_positions": pos}
     with torch.no_grad():
         for realistic in (False, True):
             x = synth.mel_input(64, 32, 0, realistic)
-            out["gen_B64_T32_s0_r%d" % int(realistic)] = gen(torch.from_numpy(x)).numpy()
+            out["gen_B64_T32_s0_r%d" % int(realistic)] = gen(torch.from_numpy(x)).numpy()[:, :, pos].copy()
     path = os.path.join(HERE, "config2_outputs.npz")
     np.savez_compressed(path, **out)
     print("wrote", path, "%.2f MB" % (os.path.getsize(path) / 1e6), len(out), "arrays")
@@ -148,7 +160,8 @@ def main():
         out["gen_T1000_tail"] = y[-4096:].copy()
         out["gen_T1000_blocksum"] = y.astype(np.float64).reshape(250, 1024).sum(axis=1)
         # weight-norm fold as the reference modules apply it (pre-forward hook output)
-        out["fold_conv_pre"] = gen.conv_pre.weight.detach().numpy()
+        out["fold_conv_pre_rows"] = fold_rows()
+        out["fold_conv_pre"] = gen.conv_pre.weight.detach().numpy()[fold_rows()].copy()
         out["fold_ups3"] = gen.ups[3].weight.detach().numpy()
         out["fold_res2_c1_1"] = gen.resblocks[2].convs1[1].weight.detach().numpy()
 

@@ -1,6 +1,6 @@
 """GPU parity of the multi-scale discriminator forward (through the C ABI) against the reference's golden
 outputs and the C oracle.  fp32 SIMT layers are exact to summation order; conv_post1 runs split-bf16 on
-tcgen05 (~1e-5).  Asserted at 1e-4 (north_star tolerance: 1e-3)."""
+wgmma (~1e-5).  Asserted at 1e-4 (north_star tolerance: 1e-3)."""
 import numpy as np
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a generator (tcgen05 split-bf16 tensor-core kernels, through the C ABI) against the C oracle and
+"""GPU parity: the sm_90a generator (wgmma split-bf16 tensor-core kernels, through the C ABI) against the C oracle and
 the reference's golden outputs.  Tolerance (BASELINE.json north_star): 1e-3 relative fp32; asserted much tighter: 1e-4
 (3-pass split-bf16, measured ~1e-5).  (The fp32 SIMT second implementation is cross-checked in
 tests/test_simt_crosscheck_gpu.py from its own test-only library.)"""
@@ -64,8 +64,18 @@ def test_module_forward_matches_golden_and_stage_taps(golden, gen_module):
     torch.cuda.synchronize()
     m, l2 = rel_errors(y.cpu().numpy(), golden["gen_taps_T3_s5_audio"])
     assert m < TOL and l2 < TOL, (m, l2)
-    with pytest.raises(engine.EngineError):  # the default chain never writes the ResBlock outputs to memory
-        gen_module._dev.stage_output(1, 1, 3)
+    # a chain with the ConvTs of stages 1 and 3 fused at the tail of the previous ResBlock never writes those ResBlock outputs
+    engine.check(engine.lib().mg_gen_set_pipeline(0b1010))
+    try:
+        with torch.no_grad():
+            yf = gen_module(x)
+        torch.cuda.synchronize()
+        m, l2 = rel_errors(yf.cpu().numpy(), golden["gen_taps_T3_s5_audio"])
+        assert m < TOL and l2 < TOL, (m, l2)
+        with pytest.raises(engine.EngineError):
+            gen_module._dev.stage_output(1, 1, 3)
+    finally:
+        engine.check(engine.lib().mg_gen_set_pipeline(-1))
     # the per-stage taps exist in the unfused chain (one kernel per ConvT / ResBlock)
     engine.check(engine.lib().mg_gen_set_pipeline(0))
     try:
@@ -111,16 +121,18 @@ def config2_golden():
 @pytest.mark.parametrize("realistic", [False, True])
 def test_config2_full_size_matches_reference(host_engine, gen_module, config2_golden, realistic):
     """BASELINE config 2 at FULL size (B=64, 80x32 mel -> 64x8192 samples), every one of the 64 items against the
-    unmodified reference's CPU-fp32 output (tests/golden/config2_outputs.npz, written by make_golden.py --config2), for
-    N(0,1) and log-mel-like inputs, through both entry points (host buffers, torch module)."""
+    unmodified reference's CPU-fp32 output at a fixed, seeded sample of 1536 positions (tests/golden/config2_outputs.npz,
+    written by make_golden.py --config2), for N(0,1) and log-mel-like inputs, through both entry points (host buffers,
+    torch module)."""
     x = synth.mel_input(64, 32, 0, realistic)
     ref = config2_golden["gen_B64_T32_s0_r%d" % int(realistic)]
     y = host_engine.forward(x)
-    assert y.shape == ref.shape == (64, 1, 8192)
+    assert y.shape == (64, 1, 8192) and ref.shape == (64, 1, 1536)
+    ys = y[:, :, config2_golden["gen_B64_T32_positions"]]
     scale = np.abs(ref).max()
-    per_item = np.abs(y.astype(np.float64) - ref).reshape(64, -1).max(axis=1) / scale
+    per_item = np.abs(ys.astype(np.float64) - ref).reshape(64, -1).max(axis=1) / scale
     assert per_item.max() <= TOL, (int(per_item.argmax()), float(per_item.max()))
-    m, l2 = rel_errors(y, ref)
+    m, l2 = rel_errors(ys, ref)
     assert m <= TOL and l2 <= TOL, (m, l2)
     with torch.no_grad():
         yd = gen_module(torch.from_numpy(x).cuda()).cpu().numpy()

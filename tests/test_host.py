@@ -181,10 +181,11 @@ def test_cabi_argument_errors_are_reported_not_thrown():
     assert L.mg_gen_forward(ctypes.c_void_p(256), ctypes.c_void_p(256), ctypes.c_void_p(256), 1, 4,
                             ctypes.c_void_p(256), 16, None) == -4  # MG_ERR_WORKSPACE_TOO_SMALL
     assert L.mg_gen_kernel_name(0) == b"conv_pre" and L.mg_gen_kernel_name(99) == b""
-    assert L.mg_gen_forward_launches() == 7 and L.mg_gen_kernel_name(6) == b"res3+post" and L.mg_gen_kernel_name(2) == b"res0+up1"
-    assert L.mg_gen_set_pipeline(0) == 0 and L.mg_gen_forward_launches() == 8 and L.mg_gen_kernel_name(7) == b"up3+res3+post"
+    assert L.mg_gen_forward_launches() == 8 and L.mg_gen_kernel_name(7) == b"up3+res3+post" and L.mg_gen_kernel_name(2) == b"res0"
+    assert L.mg_gen_set_pipeline(10) == 0 and L.mg_gen_forward_launches() == 7 and L.mg_gen_kernel_name(6) == b"res3+post"
+    assert L.mg_gen_kernel_name(2) == b"res0+up1"
     assert L.mg_gen_set_pipeline(14) == 0 and L.mg_gen_forward_launches() == 6 and L.mg_gen_kernel_name(3) == b"res1+up2"
-    assert L.mg_gen_set_pipeline(99) == -1 and L.mg_gen_set_pipeline(-1) == 0 and L.mg_gen_forward_launches() == 7
+    assert L.mg_gen_set_pipeline(99) == -1 and L.mg_gen_set_pipeline(-1) == 0 and L.mg_gen_forward_launches() == 8
     assert L.mg_gen_resup(p0 := ctypes.c_void_p(256), 3, p0, ctypes.c_void_p(512), 1, 4, None) == -1  # stages 0..2 only
     # batch slices: config 2 runs as 4 chains, small or single-item batches as one
     assert [L.mg_gen_forward_slices(b, t) for b, t in ((64, 32), (40, 32), (16, 32), (1, 1000), (0, 5))] == [4, 2, 1, 1, 1]

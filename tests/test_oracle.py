@@ -38,9 +38,10 @@ def test_weight_norm_fold_matches_reference_hook(golden):
     st = synth.generator_state(1234)
     for key, name in (("fold_conv_pre", "conv_pre"), ("fold_ups3", "ups.3"),
                       ("fold_res2_c1_1", "resblocks.2.convs1.1")):
+        rows = golden[key + "_rows"] if key + "_rows" in golden.files else slice(None)  # conv_pre: a stored sample of rows
         w = cport.fold_weight_norm(st[name + ".weight_g"], st[name + ".weight_v"])
-        np.testing.assert_allclose(w, golden[key], rtol=2e-6, atol=1e-8)
-        np.testing.assert_allclose(synth.fold_weight_norm(st[name + ".weight_g"], st[name + ".weight_v"]),
+        np.testing.assert_allclose(w[rows], golden[key], rtol=2e-6, atol=1e-8)
+        np.testing.assert_allclose(synth.fold_weight_norm(st[name + ".weight_g"], st[name + ".weight_v"])[rows],
                                    golden[key], rtol=2e-6, atol=1e-8)
 
 
@@ -111,7 +112,8 @@ def test_torch_cpu_port_matches_reference(golden):
 
 def test_torch_cpu_port_matches_reference_at_config2():
     """The timed CPU arm of bench.py (oracle/torch_port.generator_forward_reference: per-forward weight-norm + the conv
-    graph) at BASELINE config 2 full size against the unmodified reference's output (tests/golden/config2_outputs.npz)."""
+    graph) at BASELINE config 2 full size against the unmodified reference's output (tests/golden/config2_outputs.npz: every
+    item at a fixed sample of 1536 positions)."""
     import os
     import torch
     from oracle import torch_port
@@ -119,7 +121,7 @@ def test_torch_cpu_port_matches_reference_at_config2():
     params = torch_port.reference_state(synth.generator_state(1234))
     for realistic in (False, True):
         y = torch_port.generator_forward_reference(params, torch.from_numpy(synth.mel_input(64, 32, 0, realistic))).numpy()
-        m, l2 = rel_errors(y, g["gen_B64_T32_s0_r%d" % int(realistic)])
+        m, l2 = rel_errors(y[:, :, g["gen_B64_T32_positions"]], g["gen_B64_T32_s0_r%d" % int(realistic)])
         assert m < TOL and l2 < TOL, (realistic, m, l2)
 
 

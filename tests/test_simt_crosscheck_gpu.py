@@ -1,4 +1,4 @@
-"""GPU cross-check of the product (tcgen05 split-bf16) generator against an independent second implementation: the
+"""GPU cross-check of the product (wgmma split-bf16) generator against an independent second implementation: the
 first-generation fp32 SIMT kernels, built into the TEST-ONLY library libmelgan_b200_simt_test.so (csrc/testlib).  The
 product library does not contain that code; this file is the only thing that loads it."""
 import ctypes
@@ -55,7 +55,7 @@ def test_simt_matches_reference_golden(golden, simt, dev, case):
 
 
 def test_config2_two_independent_implementations_agree(simt, dev):
-    """Config 2 (B=64, T=32): fp32 SIMT vs split-bf16 tcgen05."""
+    """Config 2 (B=64, T=32): fp32 SIMT vs split-bf16 wgmma."""
     x = torch.from_numpy(synth.mel_input(64, 32, 0)).cuda()
     y_simt = simt_forward(simt, dev, x).cpu().numpy()
     y_tc = dev.forward(x).cpu().numpy()

@@ -1,7 +1,7 @@
 """GPU: one training step (train.py:108-129) through the drop-in modules -- native forwards (generator, discriminators,
 fused losses and their fused backward), stock-op recomputation for the conv backward -- against the losses and
 parameter-gradient digests of the unmodified reference (tests/golden/train_step_grads.npz).  Convs of the recomputed
-backward run in strict fp32 here; the forward is the tcgen05 split-bf16 path (~1e-5).  Tolerance 5e-3 (SURVEY 8d: "set by
+backward run in strict fp32 here; the forward is the wgmma split-bf16 path (~1e-5).  Tolerance 5e-3 (SURVEY 8d: "set by
 measurement, expect ~1e-2"): the feature loss is an L1, whose gradient sign(r - g) flips wherever a 1e-5 forward
 difference crosses zero, so element-wise agreement of gradients is bounded by that, not by the arithmetic (the gradient
 norms agree to ~1e-4, printed below)."""
@@ -70,7 +70,7 @@ def test_train_step_losses_and_gradients_match_reference(strict_fp32, which):
 def test_backward_arithmetic_matches_float64_autograd_under_a_smooth_loss(strict_fp32):
     """The digest test above is bounded by the L1 feature loss (sign flips of r - g), not by arithmetic.  Here the loss is
     smooth -- the mean square of every feature map and logit, real and generated -- so the whole backward chain (the
-    discriminators' native kernels: grouped convs, conv_post1 dgrad / wgrad on tcgen05, conv_pre / conv_post2, LeakyReLU,
+    discriminators' native kernels: grouped convs, conv_post1 dgrad / wgrad on wgmma, conv_pre / conv_post2, LeakyReLU,
     weight-norm; the AvgPool chain; the generator's recompute) is compared ELEMENT-WISE with float64 autograd of the stock-op
     graph (models.py:61-71,87-135 of the reference restated in _torch_forward), on EVERY element.
     Discriminator parameters (native backward end to end): 1e-4 of each gradient's maximum (measured 3.8e-5).
