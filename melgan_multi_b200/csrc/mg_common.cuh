@@ -38,20 +38,29 @@ __device__ __forceinline__ void cp_async_wait() {
 }
 
 // Launch helper of the tensor-core kernels: optional programmatic dependent launch
-// (mg_tc.cuh pdl_*; MG_PDL=0 in the environment turns the attribute off for A/B runs).
+// (mg_tc.cuh pdl_*; MG_PDL=0 in the environment turns the attribute off for A/B runs); cluster > 1: thread-block clusters
+// of `cluster` consecutive CTAs along x (grid.x must be a multiple of it).
 bool pdl_enabled();
 template <class... KArgs, class... Args>
-inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl, Args... args) {
+inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, bool pdl, int cluster,
+                             Args... args) {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
-    cudaLaunchAttribute attr[1];
+    cudaLaunchAttribute attr[2];
     int n = 0;
     if (pdl && pdl_enabled()) {
         attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[n].val.programmaticStreamSerializationAllowed = 1;
+        ++n;
+    }
+    if (cluster > 1) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n].val.clusterDim.x = cluster;
+        attr[n].val.clusterDim.y = 1;
+        attr[n].val.clusterDim.z = 1;
         ++n;
     }
     cfg.attrs = attr;

@@ -217,7 +217,7 @@ static int launch_conv_rows(const float *x, float *y, const uint8_t *wtc, const 
     }
     const long long vrows = (long long)B * (L + Cfg::PAD);
     const unsigned tiles = (unsigned)((vrows + Cfg::ROWS - 1) / Cfg::ROWS);
-    MG_CUDA_TRY(launch_ex(conv_rows_tc_kernel<Cfg>, dim3(tiles, Cfg::NCG), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, x, y, wtc, bias,
+    MG_CUDA_TRY(launch_ex(conv_rows_tc_kernel<Cfg>, dim3(tiles, Cfg::NCG), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, 1, x, y, wtc, bias,
                           L, B, status));
     return MG_OK;
 }

@@ -4,7 +4,7 @@
 // c1 dilations 1/3/9 and c2 dilation 1, all k=3 "same" convs on C channels.
 //
 // One CTA owns P = 64*NRB consecutive positions of one batch item (16-position halo per side, recomputed by the
-// neighbours) and keeps the whole block on chip:
+// neighbours; in a cluster of CS CTAs only at the cluster's outer edges) and keeps the whole block on chip:
 //   registers  every consumer warpgroup owns RPW 64-position blocks x NCW = C/NCP channels of
 //                R   fp32 residual stream                     D   fp32 c1 accumulator
 //              (wgmma accumulator layout, mg_tc.cuh).  R + D are 2 * P * C floats per CTA: that product is what sizes the
@@ -48,9 +48,10 @@ using namespace tc;
 
 // C channels; NRB 64-position blocks per CTA, RPW of them per consumer warpgroup; NCP column parts (warpgroups that share
 // the same rows, each with C / NCP accumulator columns); NSTAGE weight-ring slots.  POST / UPF / UPT: see above.
-template <int C_, int NRB_, int RPW_, int NCP_, int NSTAGE_, bool POST_ = false, bool UPF_ = false, int UPT_ = 0>
+// CS > 1: thread-block clusters of CS CTAs (see the kernel).
+template <int C_, int NRB_, int RPW_, int NCP_, int NSTAGE_, bool POST_ = false, bool UPF_ = false, int UPT_ = 0, int CS_ = 1>
 struct RbCfg {
-    static constexpr int C = C_, NRB = NRB_, RPW = RPW_, NCP = NCP_, NSTAGE = NSTAGE_, UPT = UPT_;
+    static constexpr int C = C_, NRB = NRB_, RPW = RPW_, NCP = NCP_, NSTAGE = NSTAGE_, UPT = UPT_, CS = CS_;
     static constexpr bool POST = POST_;  // fuse LeakyReLU -> conv_post -> tanh into the final epilogue (last stage)
     static constexpr bool UPF = UPF_;
     static constexpr int P = 64 * NRB;
@@ -61,7 +62,6 @@ struct RbCfg {
     static constexpr int SLACK = 16;             // zero rows either side of X (dilation-9 taps reach 9 rows out)
     static constexpr int HALO = 16 + (POST ? 3 : 0);  // 1+1+3+1+9+1 (+3 for the fused k7 conv_post)
     static constexpr int HL = HALO + (UPT_ ? 1 : 0);  // left halo: a fused tail ConvT also reads x[s - 1]
-    static constexpr int PVALID = P - HALO - HL;
     static constexpr int ROWS = P + 2 * SLACK;
     static constexpr int XPITCH = ROWS * 16;  // bytes between k-panels
     static constexpr int KP = C / 8;
@@ -83,7 +83,13 @@ struct RbCfg {
     static_assert(!UPF || (NCP == 1 && NPB <= NWG && 2 * KP * UPITCH <= XBYTES && C * SPITCH * 4 <= 2 * XBYTES),
                   "fused ConvT must fit the X region");
     static_assert(!POST || (C == 32 && NCP == 1), "conv_post fusion is for the 32-channel stage");
-    static constexpr int SMEM_BYTES = 2 * XBYTES + NSTAGE * CHUNK + 2 * C * 4 + 2 * NSTAGE * 8;
+    // clusters: CS * P positions per cluster, halos only at the cluster's outer edges (PVB outputs kept by a cluster with
+    // more sequence on both sides); XCH rows (the largest dilation) of each cluster-internal border are copied into the
+    // neighbour's slack rows at every X hand-off
+    static constexpr int PVB = CS * P - HALO - HL, XCH = 9;
+    static_assert(CS == 1 || ((CS == 2 || CS == 4) && !POST_ && !UPF_ && UPT_ == 0 && XCH <= SLACK && 2 * XCH <= P),
+                  "clusters are for the plain ResBlock");
+    static constexpr int SMEM_BYTES = 2 * XBYTES + NSTAGE * CHUNK + 2 * C * 4 + (2 * NSTAGE + (CS > 1 ? 2 : 0)) * 8;
     static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "shared memory budget");
     static_assert(XPITCH / 16 < 16384, "LBO field");
     static_assert(NRB % RPW == 0 && C % NCP == 0 && NCW % 32 == 0, "warpgroup split");
@@ -99,23 +105,33 @@ template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NT, 1)
 resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed, int stage, int L, int nB,
                    int *__restrict__ status, long long *__restrict__ trace) {
-    constexpr int C = Cfg::C, P = Cfg::P, SLACK = Cfg::SLACK, HALO = Cfg::HALO, HL = Cfg::HL, PVS = Cfg::PVALID;
+    constexpr int C = Cfg::C, P = Cfg::P, SLACK = Cfg::SLACK, HALO = Cfg::HALO, HL = Cfg::HL;
     constexpr int XPITCH = Cfg::XPITCH, XBYTES = Cfg::XBYTES, KC = Cfg::KC, CHUNK = Cfg::CHUNK, NSTAGE = Cfg::NSTAGE;
     constexpr int NCONS = Cfg::NCONS, NCP = Cfg::NCP, NCW = Cfg::NCW, RPW = Cfg::RPW, KSL = Cfg::KSL, NA = NCW / 2;
+    constexpr int CS = Cfg::CS, XCH = Cfg::XCH;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *Xh = smem, *Xl = smem + XBYTES, *ring = smem + 2 * XBYTES;
     float *pend = reinterpret_cast<float *>(ring + NSTAGE * CHUNK);  // sum of the c2 biases folded so far
     float *b1s = pend + C;                                            // bias of the c1 in flight
     uint64_t *full = reinterpret_cast<uint64_t *>(b1s + C);
     uint64_t *empty = full + NSTAGE;
+    // clusters: hfull completes once every cluster neighbour's border rows have landed in this CTA's slack rows (one phase
+    // per X hand-off), hfree once every neighbour's MMAs have finished reading its X (one phase per conv): then the copies
+    // of this CTA's border rows have been read, and the neighbours' slack rows may be refilled
+    uint64_t *hfull = empty + NSTAGE, *hfree = hfull + 1;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int b = blockIdx.y, stile = blockIdx.x;
-    // Edge-aware tiling: a halo is only needed where the tile borders MORE sequence.  Tile 0 starts at position 0 (its
-    // left edge is the real zero padding) and keeps P - HALO outputs; later tiles keep P - HALO - HL, and a tile that
-    // reaches the end of the sequence keeps its right HALO rows too.
-    const int o = stile == 0 ? 0 : (P - HALO) + (stile - 1) * PVS - HL;  // position of tile row 0
-    const int p_lo = stile == 0 ? 0 : HL, p_hi = (o + P >= L) ? P : P - HALO;
+    // a cluster is CS consecutive CTAs along x (launch_resblock): rank crank of cluster clus owns the cluster's rows
+    // [crank P, (crank + 1) P)
+    const int b = blockIdx.y, clus = blockIdx.x / CS, crank = blockIdx.x % CS;
+    // Edge-aware tiling: a halo is only needed where the cluster (one CTA for CS = 1) borders MORE sequence.  Cluster 0
+    // starts at position 0 (its left edge is the real zero padding) and keeps CS P - HALO outputs; later clusters keep
+    // CS P - HALO - HL, and a cluster that reaches the end of the sequence keeps its right HALO rows too.  Cluster-internal
+    // borders need no halo: the neighbours exchange their border rows of X.  A CTA whose rows all lie past the end still
+    // runs the whole protocol (its neighbours write into its shared memory).
+    const int oc = clus == 0 ? 0 : (CS * P - HALO) + (clus - 1) * Cfg::PVB - HL;  // position of the cluster's row 0
+    const int o = oc + crank * P;                                                 // position of tile row 0
+    const int p_lo = (clus == 0 || crank > 0) ? 0 : HL, p_hi = (crank < CS - 1 || oc + CS * P >= L) ? P : P - HALO;
     const bool interior = (o >= 0 && o + P <= L);  // every row of the tile is a real position
     // consumption order of the six convs of ResBlock `stage`: c1[0], c2[0], c1[1], c2[1], c1[2], c2[2]
     const int l0 = 5 + 6 * stage;
@@ -124,7 +140,11 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     if (tid == 0) {
         for (int s = 0; s < NSTAGE; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], Cfg::NWG);  // one arrival per consumer warpgroup
+            mbar_init(&empty[s], Cfg::NWG * CS);  // one arrival per consumer warpgroup of every CTA of the cluster
+        }
+        if constexpr (CS > 1) {
+            mbar_init(hfull, 1);                                     // + the bytes of the neighbours' copies
+            mbar_init(hfree, (crank > 0) + (crank < CS - 1));        // one arrival per cluster neighbour
         }
         fence_mbar_init();
     }
@@ -137,6 +157,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     for (int i = tid; i < C; i += Cfg::NT) pend[i] = 0.f;
     fence_proxy_async();
     __syncthreads();
+    if constexpr (CS > 1) cluster_sync();  // every CTA's barriers are initialised before any remote access
     // optional timeline of one interior CTA (clock64 stamps of thread 0; see mg_gen_resblock_trace); per conv c = 0..5 the
     // slots 2 + 3c (X handed over), 3 + 3c (accumulator ready), 4 + 3c (next X written) are 2 + 6j .. 7 + 6j of conv pair j
     const bool tr = trace && blockIdx.y == 0 && blockIdx.x == (gridDim.x > 1 ? 1u : 0u) && tid == 0;
@@ -144,13 +165,17 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
 
     if (warp == NCONS / 32) {
         // ================= TMA producer: streams the weight chunks through the ring in consumption order =================
+        // (clusters: chunk j is read from L2 once, by rank j % CS, and multicast into the same slot of every CTA; each
+        // producer still posts its own CTA's expected bytes, after its empty[s] has seen every consumer of the cluster)
         if (lane == 0) {
-            int s = 0, ph = 0;
+            int s = 0, ph = 0, j = 0;
             bool ok = true;
             auto put = [&](const uint8_t *src, uint32_t bytes) {
                 if (!ok || !mbar_wait(&empty[s], ph ^ 1)) { ok = false; return; }
                 mbar_arrive_expect_tx(&full[s], bytes);
-                bulk_g2s(ring + s * CHUNK, src, bytes, &full[s]);
+                if constexpr (CS == 1) bulk_g2s(ring + s * CHUNK, src, bytes, &full[s]);
+                else if (j % CS == crank) bulk_g2s_multicast(ring + s * CHUNK, src, bytes, &full[s], (1 << CS) - 1);
+                ++j;
                 if (++s == NSTAGE) { s = 0; ph ^= 1; }
             };
             if constexpr (Cfg::UPF) {  // the fused ConvT's 4 taps x UKSL K-slices, in blob order
@@ -167,6 +192,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
             }
             if (!ok) atomicExch(status, 2);
         }
+        if constexpr (CS > 1) cluster_sync();  // no CTA leaves while a peer may still access its shared memory
         return;
     }
 
@@ -178,6 +204,15 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     float R[RPW][NA], D[RPW][NA];
     int s = 0, ph = 0, ps = -1;
     bool ok = true;  // a timed-out wait only raises the status word: control flow stays warpgroup-uniform
+    // a slot is free once every consumer warpgroup of every CTA of the cluster has released it (thread t < CS of the
+    // warpgroup arrives on CTA t's empty[], all of them in one instruction)
+    auto release = [&](int slot) {
+        if constexpr (CS == 1) {
+            if (t == 0) mbar_arrive(&empty[slot]);
+        } else if (t < CS) {
+            mbar_arrive_remote(&empty[slot], t);
+        }
+    };
     // ring protocol: chunk_begin() waits for the next slot; chunk_end() commits its MMAs and frees the slot of the previous
     // chunk once those have completed (one group stays in flight); drain() waits for everything and frees the last slot
     auto chunk_begin = [&]() -> uint32_t {
@@ -190,7 +225,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     auto chunk_end = [&]() {
         wgmma_commit();
         wgmma_wait<1>();
-        if (t == 0 && ps >= 0) mbar_arrive(&empty[ps]);
+        if (ps >= 0) release(ps);
         ps = s;
         if (++s == NSTAGE) { s = 0; ph ^= 1; }
     };
@@ -198,10 +233,19 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         wgmma_wait<0>();
         acc_fence2(R);
         acc_fence2(D);
-        if (t == 0 && ps >= 0) mbar_arrive(&empty[ps]);
+        if (ps >= 0) release(ps);
         ps = -1;
     };
     auto sync_cons = [&]() { named_bar_sync(1, NCONS); };
+    // after a conv: every warpgroup's MMAs have read X (its slack rows included, which the neighbours may now refill);
+    // thread 0 / 1 tells the left / right neighbour
+    const int nbr = tid == 0 ? crank - 1 : crank + 1;
+    const bool tells = tid < 2 && nbr >= 0 && nbr < CS;
+    auto x_read = [&]() {
+        sync_cons();
+        if constexpr (CS > 1)
+            if (tells) mbar_arrive_remote(hfree, nbr);
+    };
     // X <- split(lrelu(A + bias)) for this warpgroup's rows and columns, zero outside [0, L); keep_last: also park the
     // fp32 lrelu(x[L-1]) in b1s (the tail ConvT's fix-up)
     auto write_x = [&](float (&A)[RPW][NA], const float *bsrc, bool keep_last) {
@@ -226,8 +270,54 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                 }
             }
     };
+    // clusters: the XCH rows next to a cluster-internal border (all k-panels of hi and lo) are bulk-copied into the
+    // neighbour's slack rows after every hand-off.  A thread that writes such a row first waits until the neighbours'
+    // MMAs of the previous conv are done, which also means the previous copies out of this X have landed.
+    bool border = false;
+#pragma unroll
+    for (int r = 0; r < RPW; ++r)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int p = (rb0 + r) * 64 + frag_row(t, h);
+            border |= (crank > 0 && p < XCH) || (crank < CS - 1 && p >= P - XCH);
+        }
+    constexpr int NXC = 2 * Cfg::KP;        // copies per border: one per k-panel of hi and lo
+    constexpr uint32_t XCB = XCH * 16;      // bytes per copy
+    // (a warp issues bulk copies one lane at a time: they are spread over every consumer warp, copy i by warp i % NW)
+    constexpr int NW = NCONS / 32;
+    auto send_halo = [&]() {
+        for (int i = warp + NW * lane; i < 2 * NXC; i += NCONS) {
+            const int side = i / NXC, nb = side ? crank + 1 : crank - 1;
+            if (nb < 0 || nb >= CS) continue;
+            const uint32_t panel = xh_addr + (i % NXC) * XPITCH;  // k-panel i % NXC of Xh, continuing into Xl
+            const int src = side ? P - XCH : 0, dst = side ? -XCH : P;  // rows: mine, and the same positions in nb's tile
+            bulk_s2s_cluster(mapa(panel + (SLACK + dst) * 16, nb), panel + (SLACK + src) * 16, XCB, mapa(smem_u32(hfull), nb));
+        }
+    };
+    // X hand-off: X <- split(lrelu(A + bias)), visible to every warpgroup's MMAs (and, clusters, the neighbours')
+    int hand = 0;
+    auto hand_off = [&](float (&A)[RPW][NA], const float *bsrc, bool keep_last) {
+        if constexpr (CS > 1) {
+            if (border && hand > 0) {
+                MG_TR(100 + 2 * hand);
+                ok &= mbar_wait(hfree, (hand - 1) & 1);
+                MG_TR(101 + 2 * hand);
+            }
+            if (tid == 0) mbar_arrive_expect_tx(hfull, ((crank > 0) + (crank < CS - 1)) * NXC * XCB);  // this hand-off's rows in
+        }
+        write_x(A, bsrc, keep_last);
+        fence_proxy_async();
+        sync_cons();
+        if constexpr (CS > 1) send_halo();
+        ++hand;
+    };
     // one conv: every chunk (tap, K-slice) x 3 passes x KC/16 k-steps x RPW row blocks
     auto conv_mma = [&](float (&A)[RPW][NA], int dil, bool fresh, int conv) {
+        if constexpr (CS > 1) {  // the neighbours' border rows of this conv's input are in the slack rows
+            MG_TR(88 + 2 * conv);
+            ok &= mbar_wait(hfull, conv & 1);
+            MG_TR(89 + 2 * conv);
+        }
         MG_TR(64 + 3 * conv);
 #pragma unroll 1
         for (int ch = 0; ch < Cfg::NCHUNK; ++ch) {
@@ -349,9 +439,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                         R[r][4 * k + 2 * h + e] = inr ? __ldg(xp + (size_t)(c0 + frag_col(q, 4 * k + e)) * L) : 0.f;
             }
     }
-    write_x(R, pend, false);  // (pend is still all zeros)
-    fence_proxy_async();
-    sync_cons();
+    hand_off(R, pend, false);  // (pend is still all zeros)
     MG_TR(1);
 
 #pragma unroll 1
@@ -362,10 +450,8 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         MG_TR(2 + 6 * pr);
         conv_mma(D, pr == 0 ? 1 : pr == 1 ? 3 : 9, true, 2 * pr);
         MG_TR(3 + 6 * pr);
-        sync_cons();  // every warpgroup's MMAs have read X (and b1s is complete)
-        write_x(D, b1s, false);
-        fence_proxy_async();
-        sync_cons();
+        x_read();  // (and b1s is complete)
+        hand_off(D, b1s, false);
         MG_TR(4 + 6 * pr);
         // ---- c2 (dilation 1) accumulating onto R, then X <- split(lrelu(R + pend)) for the next c1 (or the tail ConvT)
         const float *bias2 = packed + bias_offset(l0 + 3 + pr);
@@ -373,12 +459,8 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         MG_TR(5 + 6 * pr);
         conv_mma(R, 1, false, 2 * pr + 1);
         MG_TR(6 + 6 * pr);
-        sync_cons();
-        if (pr < 2 || Cfg::UPT != 0) {
-            write_x(R, pend, Cfg::UPT != 0 && pr == 2);
-            fence_proxy_async();
-            sync_cons();
-        }
+        x_read();
+        if (pr < 2 || Cfg::UPT != 0) hand_off(R, pend, Cfg::UPT != 0 && pr == 2);
         MG_TR(7 + 6 * pr);
     }
 
@@ -555,6 +637,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
             }
     }
     if (!ok && t == 0) atomicExch(status, 3);
+    if constexpr (CS > 1) cluster_sync();  // no CTA leaves while a peer may still access its shared memory
     MG_TR(20);
 #undef MG_TR
 }
@@ -567,30 +650,49 @@ static int launch_resblock(const float *x, float *y, const float *packed, int st
         MG_CUDA_TRY(cudaFuncSetAttribute(resblock_tc_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         configured = true;
     }
-    constexpr int P = Cfg::P, PVS = Cfg::PVALID;  // edge-aware tiling, see the kernel
-    const int ntiles = 1 + (L > P ? (L - P + PVS - 1) / PVS : 0);
+    constexpr int CS = Cfg::CS, PC = CS * Cfg::P, PVB = Cfg::PVB;  // edge-aware tiling of CS * P-position clusters, see the kernel
+    const int nclusters = 1 + (L > PC ? (L - PC + PVB - 1) / PVB : 0);
     if (B > 65535) return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: batch %d exceeds the grid", B);
-    MG_CUDA_TRY(launch_ex(resblock_tc_kernel<Cfg>, dim3(ntiles, B), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, x, y, packed, stage,
-                          L, B, status, trace));
+    if (trace && CS > 1) {  // diagnostic: clusters resident at once (GPC boundaries can leave SMs idle), into trace[127]
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(CS * nclusters, B);
+        cfg.blockDim = dim3(Cfg::NT);
+        cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+        cudaLaunchAttribute attr;
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = CS;
+        attr.val.clusterDim.y = attr.val.clusterDim.z = 1;
+        cfg.attrs = &attr;
+        cfg.numAttrs = 1;
+        int n = 0;
+        MG_CUDA_TRY(cudaOccupancyMaxActiveClusters(&n, resblock_tc_kernel<Cfg>, &cfg));
+        const long long v = n;
+        MG_CUDA_TRY(cudaMemcpy(trace + 127, &v, sizeof(v), cudaMemcpyHostToDevice));
+    }
+    MG_CUDA_TRY(launch_ex(resblock_tc_kernel<Cfg>, dim3(CS * nclusters, B), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, CS, x, y, packed,
+                          stage, L, B, status, trace));
     return MG_OK;
 }
 
 template <class Cfg>
 static const char *cfg_name() {
     static char buf[96];
-    snprintf(buf, sizeof(buf), "resblock_tc_kernel<RbCfg<%d,%d,%d,%d,%d,%d,%d,%d>>", Cfg::C, Cfg::NRB, Cfg::RPW, Cfg::NCP, Cfg::NSTAGE,
-             (int)Cfg::POST, (int)Cfg::UPF, Cfg::UPT);
+    snprintf(buf, sizeof(buf), "resblock_tc_kernel<RbCfg<%d,%d,%d,%d,%d,%d,%d,%d,%d>>", Cfg::C, Cfg::NRB, Cfg::RPW, Cfg::NCP,
+             Cfg::NSTAGE, (int)Cfg::POST, (int)Cfg::UPF, Cfg::UPT, Cfg::CS);
     return buf;
 }
 
 // Configurations per stage code (C, 64-row blocks, blocks per warpgroup, column parts, ring slots): the tile is as long as
-// the register file allows (R and D of every position and channel: 2 * P * C floats), at one CTA per SM.
+// the register file allows (R and D of every position and channel: 2 * P * C floats), at one CTA per SM.  Stages 0 and 1
+// run as clusters (the last parameter; H100 80GB HBM3, config 2): stage 0 as 4 CTAs = 256 positions, one cluster per item
+// at L = 256 instead of 7 halo-overlapped tiles; stage 1 as pairs, 18 CTAs per item at L = 2048 instead of 21 (4-CTA
+// clusters would need 20).
 // stage 0..3: ResBlock `stage`; 4: ResBlock 3 with LeakyReLU -> conv_post -> tanh fused (y is the audio [B][1][L]);
 // 12 / 13 / 14 = stages 2 / 3 / 3+post with the stage's stride-2 ConvT fused in front (x is the PREVIOUS stage's output
 // [B][2C][L/2], L stays the output length); 20 / 21 / 22 = ResBlock 0 / 1 / 2 with the NEXT stage's LeakyReLU -> ConvT
 // at its tail (y is [B][C/2][S L]).
-using Rb0 = RbCfg<256, 1, 1, 2, 4>;
-using Rb1 = RbCfg<128, 2, 1, 1, 4>;
+using Rb0 = RbCfg<256, 1, 1, 2, 4, false, false, 0, 4>;
+using Rb1 = RbCfg<128, 2, 1, 1, 4, false, false, 0, 2>;
 using Rb2 = RbCfg<64, 4, 1, 1, 3>;
 using Rb3 = RbCfg<32, 8, 2, 1, 4>;
 using Rb3Post = RbCfg<32, 8, 2, 1, 4, true>;

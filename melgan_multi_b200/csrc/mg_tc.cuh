@@ -53,11 +53,47 @@ __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity, uint32
     return false;
 }
 
+// ---- thread-block clusters ------------------------------------------------------------------------
+// shared::cluster address of the object at shared::cta address `addr` in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+    return r;
+}
+// arrive on the mbarrier `bar` (own shared::cta address) of CTA `rank`, for a consumer that frees a buffer once its MMAs
+// (async proxy, completed by wgmma_wait) have read it.  No cluster-scope release: that fence would wait on the whole GPU
+// memory system; data for another CTA travels by bulk copy (bulk_s2s_cluster), which completes on the reader's mbarrier.
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t *bar, uint32_t rank) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(mapa(smem_u32(bar), rank)) : "memory");
+}
+// every thread of every CTA of the cluster; orders shared-memory accesses across the cluster (not bounded: used only
+// after barrier initialisation and before exit, where every CTA arrives on every path)
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+
 // ---- 1-D bulk async copy (TMA, no tensor map): global -> shared, completes on an mbarrier -------
 __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                      smem_u32(smem_dst)),
                  "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+                 : "memory");
+}
+// the same copy landing at the same shared-memory offset of every CTA in `cta_mask` (one L2 read), each completing on the
+// mbarrier at `bar`'s offset in that CTA
+__device__ __forceinline__ void bulk_g2s_multicast(void *smem_dst, const void *gmem_src, uint32_t bytes, uint64_t *bar,
+                                                   uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
+            smem_u32(smem_dst)),
+        "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
+        : "memory");
+}
+// 1-D bulk copy from this CTA's shared memory to another CTA's of the cluster (dst and bar: shared::cluster addresses,
+// mapa), completing on that CTA's mbarrier
+__device__ __forceinline__ void bulk_s2s_cluster(uint32_t dst, uint32_t src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "r"(src),
+                 "r"(bytes), "r"(bar)
                  : "memory");
 }
 // generic-proxy writes (st.shared) -> visible to the async proxy (wgmma operand reads, bulk copies)

@@ -226,7 +226,7 @@ static int launch_convt(const float *x, float *y, const float *packed, int B, in
     }
     const long long vrows = (long long)B * (Lin + 1);  // Lin + 1 rows per item: position s = Lin feeds the last `pad` outputs
     dim3 grid((unsigned)((vrows + Cfg::ROWS - 1) / Cfg::ROWS), Cfg::NCG);
-    MG_CUDA_TRY(launch_ex(convt_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, x, y, packed, Lin, B, status));
+    MG_CUDA_TRY(launch_ex(convt_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, 1, x, y, packed, Lin, B, status));
     return MG_OK;
 }
 
@@ -352,7 +352,7 @@ static int launch_convt_resident(const float *x, float *y, const float *packed, 
     }
     const long long vrows = (long long)B * (Lin + 1);
     MG_CUDA_TRY(launch_ex(convt_resident_tc_kernel<Cfg>, dim3((unsigned)((vrows + 63) / 64)), dim3(Cfg::NCONV + 128 + 32), smem, s,
-                          true, x, y, packed, Lin, B, status));
+                          true, 1, x, y, packed, Lin, B, status));
     return MG_OK;
 }
 

@@ -194,7 +194,7 @@ int launch_disc_post1_wgrad_tc(const float *x, const float *dz, float *dw, float
         MG_CUDA_TRY(cudaFuncSetAttribute(post1_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, wg::SMEM_BYTES));
         configured = true;
     }
-    MG_CUDA_TRY(launch_ex(post1_wgrad_tc_kernel, dim3(wg::C / wg::MT, wg::C / wg::NTILE), dim3(wg::NT), wg::SMEM_BYTES, s, false, x, dz,
+    MG_CUDA_TRY(launch_ex(post1_wgrad_tc_kernel, dim3(wg::C / wg::MT, wg::C / wg::NTILE), dim3(wg::NT), wg::SMEM_BYTES, s, false, 1, x, dz,
                           dw, db, Bt, L, status));
     return MG_OK;
 }

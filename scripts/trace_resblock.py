@@ -1,4 +1,5 @@
-"""Print the phase timeline (SM cycles) of one interior CTA of the tensor-core ResBlock kernel, per stage."""
+"""Print the phase timeline (SM cycles) of one interior CTA of the tensor-core ResBlock kernel, per stage (clustered
+stages: also the waits on the cluster neighbours' halo rows, and how many clusters the GPU keeps resident)."""
 import ctypes
 import sys
 
@@ -27,8 +28,12 @@ for stage in range(4):
         engine.check(L.mg_gen_resblock_trace(gd.packed.data_ptr(), stage, x.data_ptr(), y.data_ptr(), 64, Lp, tr.ctypes.data))
     t0 = tr[0]
     e = lambda i: int(tr[i] - t0)
-    print("stage %d (C=%d): load %d | total %d cycles" % (stage, C, e(1), e(20)))
+    clustered = tr[127] > 0
+    print("stage %d (C=%d): load %d | total %d cycles" % (stage, C, e(1), e(20))
+          + (" | max active clusters %d" % tr[127] if clustered else ""))
     for c in range(6):
         print("  conv %d: X handed @%7d | mma: recv +%5d, weights +%5d, issued +%6d | acc ready @%7d (mma phase %6d) | epilogue %6d"
               % (c, e(2 + 3 * c), tr[64 + 3 * c] - tr[2 + 3 * c], tr[65 + 3 * c] - tr[64 + 3 * c], tr[66 + 3 * c] - tr[65 + 3 * c],
-                 e(3 + 3 * c), tr[3 + 3 * c] - tr[2 + 3 * c], (tr[4 + 3 * c] - tr[3 + 3 * c]) if c < 5 else (tr[20] - tr[18])))
+                 e(3 + 3 * c), tr[3 + 3 * c] - tr[2 + 3 * c], (tr[4 + 3 * c] - tr[3 + 3 * c]) if c < 5 else (tr[20] - tr[18]))
+              + (" | halo: wait full %5d, wait free %5d" % (tr[89 + 2 * c] - tr[88 + 2 * c],
+                                                         (tr[101 + 2 * c] - tr[100 + 2 * c]) if c > 0 else 0) if clustered else ""))
