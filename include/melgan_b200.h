@@ -101,6 +101,14 @@ int mg_gen_resblock(const void *packed, int stage, const float *x, float *y, int
  * (models.py:64-66); x [B][2C][Lin] is the previous stage's output, y [B][C][2 Lin] (C = 64 / 32).  Synchronous, like
  * mg_gen_resblock: a per-kernel parity entry point. */
 int mg_gen_upres(const void *packed, int stage, const float *x, float *y, int B, int Lin, void *stream);
+/* The default chain's last kernel: stage 3's LeakyReLU -> ConvTranspose1d(k4, s2), the ResBlock and LeakyReLU -> conv_post
+ * -> tanh in ONE kernel (models.py:64-69); x [B][64][Lin] is stage 2's output, audio [B][1][2 Lin].  Synchronous parity
+ * entry point. */
+int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, int Lin, void *stream);
+/* Template configuration of the ResBlock kernel behind a stage code (0..3 ResBlock, 4 + conv_post, 12 / 13 / 14 ConvT fused in
+ * front, 20 / 21 / 22 next ConvT fused at the tail), "resblock_tc_kernel<RbCfg<C,NRB,RPW,NCP,NSTAGE,POST,UPF,UPT,CS>>";
+ * "" for an unknown code.  Tests derive the tile and cluster borders from it. */
+const char *mg_gen_resblock_config(int code);
 
 /* ResBlock `stage` (0..2) with the NEXT stage's LeakyReLU -> ConvTranspose1d fused at its tail, as the default pipeline runs it
  * (models.py:66 followed by :64-65 of the next loop iteration): x [B][C][L] is stage `stage`'s ConvT output, y
@@ -269,7 +277,7 @@ int mg_gen_forward_launches(void);
 int mg_gen_forward_slices(int B, int T);
 /* Selects the generator chain for the calling thread: bit i (1..3) of tail_mask = stage i's ConvT fused at the tail of
  * ResBlock i-1's kernel; 0 = one kernel per ConvT / ResBlock (all stage outputs materialised: mg_gen_stage_output works for
- * which = 1..3); -1 = the default (environment MG_GEN_TAIL, else all three).  For tests and A/B measurements. */
+ * which = 1..3); -1 = the default (environment MG_GEN_TAIL, else none).  For tests and A/B measurements. */
 int mg_gen_set_pipeline(int tail_mask);
 const char *mg_gen_kernel_name(int i);
 /* Template configuration of the i-th chain kernel at T mel frames per item (e.g. "resblock_tc_kernel<RbCfg<128,2,4,4,1,0,0,1,0,1>>/NH4"):

@@ -326,6 +326,16 @@ int mg_gen_upres(const void *packed, int stage, const float *x, float *y, int B,
     });
 }
 
+int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, int Lin, void *stream) {
+    if (!packed || !x || !audio || (const void *)x == (const void *)audio || B < 1 || Lin < 1)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_upres_post: bad argument");
+    return run_one_kernel("mg_gen_upres_post", (cudaStream_t)stream, [&](int *st) {
+        return launch_resblock_tc(x, audio, (const float *)packed, 14, B, 2 * Lin, st, (cudaStream_t)stream);
+    });
+}
+
+const char *mg_gen_resblock_config(int code) { return resblock_config_name(code, 0); }
+
 /* ------------------------------- multi-scale discriminator ------------------------------- */
 
 size_t mg_msd_packed_bytes(void) { return msd_packed_bytes(); }

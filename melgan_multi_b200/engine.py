@@ -55,6 +55,10 @@ def lib():
         L.mg_gen_upres.restype = ctypes.c_int
         L.mg_gen_upres.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                    ctypes.c_int, ctypes.c_void_p]
+        L.mg_gen_upres_post.restype = ctypes.c_int
+        L.mg_gen_upres_post.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
+        L.mg_gen_resblock_config.restype = ctypes.c_char_p
+        L.mg_gen_resblock_config.argtypes = [ctypes.c_int]
         L.mg_gen_conv_pre.restype = ctypes.c_int
         L.mg_gen_conv_pre.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
         L.mg_gen_resblock_post.restype = ctypes.c_int
@@ -322,6 +326,20 @@ class GeneratorDevice:
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
             check(lib().mg_gen_upres(self.packed.data_ptr(), stage, x.data_ptr(), y.data_ptr(), B, L, stream))
+        return y
+
+    def upres_post(self, x):
+        """The default chain's last kernel: LeakyReLU -> ConvTranspose1d(k4, s2) of stage 3 -> ResBlock -> LeakyReLU ->
+        conv_post -> tanh on x [B, 64, Lin] -> audio [B, 1, 2 Lin]; synchronous."""
+        torch = self.torch
+        x = x.contiguous()
+        B, C, L = x.shape
+        if C != 64:
+            raise EngineError("upres_post expects 64 input channels")
+        y = torch.empty((B, 1, 2 * L), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream().cuda_stream
+            check(lib().mg_gen_upres_post(self.packed.data_ptr(), x.data_ptr(), y.data_ptr(), B, L, stream))
         return y
 
     def resup(self, stage, x):

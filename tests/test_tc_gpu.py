@@ -42,8 +42,10 @@ def oracle_resblock(state, stage, x):
 
 @pytest.mark.parametrize("stage,B,L", [(3, 2, 2100), (2, 2, 1000), (1, 2, 500), (0, 2, 200), (3, 1, 5), (0, 1, 8),
                                        (1, 1, 224), (1, 1, 225),
-                                       # stage 0 (64-position tiles, 32 of them kept between halos): one tile with a partly /
-                                       # fully used tail, exactly one, the tile borders of several, odd tails
+                                       # stage 0 (4-CTA clusters of 64-position tiles, 256 positions with a 16-row halo
+                                       # only at the cluster's outer edges): lengths inside one cluster, one cluster and
+                                       # one over, several clusters, odd tails; test_kernel_borders_gpu.py derives the
+                                       # border lengths of every stage from the kernels' configuration
                                        (0, 1, 129), (0, 2, 144), (0, 3, 256), (0, 1, 257), (0, 2, 480), (0, 1, 481), (0, 2, 1000),
                                        (0, 1, 128), (0, 64, 256)])
 def test_resblock_tc_matches_oracle(state, dev, stage, B, L):
