@@ -77,6 +77,21 @@ size_t mg_gen_workspace_bytes(int B, int T);
 int mg_gen_forward(const void *packed, const float *mel, float *audio, int B, int T,
                    void *workspace, size_t workspace_bytes, void *stream);
 
+/* Ragged batch: B utterances of different lengths in one forward (inference only).
+ *   mel   [B, 80, T_max]        device, fp32; item i's frames t >= lengths[i] are never read (they may hold NaN)
+ *   audio [B, 1, 256*T_max]     device, fp32; audio[i, 0, :256*lengths[i]] is bit-identical to the mg_gen_forward of
+ *                               mel[i:i+1, :, :lengths[i]] alone under the same chain (mg_gen_set_pipeline), the rest 0.0
+ *   lengths: HOST array of B ints, 1 <= lengths[i] <= T_max (the grids depend on them: no device read, no sync)
+ *   workspace: mg_gen_workspace_bytes(B, T_max) bytes, so mg_gen_check_status(workspace, B, T_max, ...) and
+ *   mg_gen_stage_output(workspace, which, out, B, T_max, ...) work as after mg_gen_forward (a tap's values past each item's
+ *   valid prefix are unspecified).
+ * Every activation keeps the padded [B][C][T_max * scale] layout; the kernels run tiles only inside each item, with the
+ * item's own zero padding at its own end.  1 <= B <= MG_GEN_RAGGED_MAX_B (the per-launch tables travel as kernel
+ * parameters).  mg_gen_forward is this call with every length equal to T.  Asynchronous on `stream`, no allocation. */
+#define MG_GEN_RAGGED_MAX_B 256
+int mg_gen_forward_ragged(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
+                          void *workspace, size_t workspace_bytes, void *stream);
+
 /* Same as mg_gen_forward, but brackets each of the mg_gen_forward_launches() kernels with CUDA
  * events on `stream`, waits for the last one and returns the per-kernel device times in
  * kernel_ms[0 .. mg_gen_forward_launches()-1] (names: mg_gen_kernel_name(i)).  Used by bench.py for the
@@ -192,6 +207,11 @@ int mg_gen_engine_load_state(mg_gen_engine *e, const float *const *v, const floa
  * buffer.  The copies are cut with the batch slices (mg_gen_forward_slices): a slice's audio goes
  * back to the host while the other slices are still computing. */
 int mg_gen_engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T);
+/* Ragged twin of mg_gen_engine_forward (semantics and limits of mg_gen_forward_ragged): mel_host [B,80,T_max] ->
+ * audio_host [B,1,256 T_max].  Each slice uploads only its items' valid mel prefixes and downloads its audio rows (the
+ * valid prefix and the zero tail). */
+int mg_gen_engine_forward_ragged(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max,
+                                 const int *lengths);
 /* Device time of the last forward in milliseconds (CUDA events on the engine's stream around the sliced
  * upload -> kernels -> download sequence). */
 int mg_gen_engine_last_kernel_ms(mg_gen_engine *e, float *ms);
@@ -272,7 +292,8 @@ int mg_loss_backward(const float *const *a, const float *const *b, const long lo
 
 /* Number of kernels in the generator's chain (at most 16) and the name of the i-th one.  mg_gen_forward cuts
  * the batch into mg_gen_forward_slices(B, T) contiguous slices whose chains run concurrently on forked streams
- * (joined back into `stream` before it returns), so one forward enqueues slices x launches kernels. */
+ * (joined back into `stream` before it returns), so one forward enqueues slices x launches kernels.  A ragged batch is cut
+ * by the same rule applied to its total frames, into groups of about equal frames. */
 int mg_gen_forward_launches(void);
 int mg_gen_forward_slices(int B, int T);
 /* Selects the generator chain for the calling thread: bit i (1..3) of tail_mask = stage i's ConvT fused at the tail of

@@ -14,17 +14,31 @@ static int *status_ptr(void *workspace, int B, int T) {
     return reinterpret_cast<int *>(reinterpret_cast<float *>(workspace) + ws_offset(6, (size_t)B, (size_t)T));
 }
 
-// mel_host / audio_host: optional pinned host buffers (the engine entry point); the copies ride on the batch slices' streams
-static int run_generator(const float *packed, const float *mel, float *audio, int B, int T, float *ws, cudaStream_t s,
+// batch: mel lengths (stride T); mel_host / audio_host: optional pinned host buffers (the engine entry point); the copies
+// ride on the batch slices' streams
+static int run_generator(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, cudaStream_t s,
                          cudaEvent_t *ev, const float *mel_host = nullptr, float *audio_host = nullptr) {
-    int *st = status_ptr(ws, B, T);
+    int *st = status_ptr(ws, batch.items(), batch.stride);
     MG_CUDA_TRY(cudaMemsetAsync(st, 0, sizeof(int), s));
-    return launch_generator_tc(packed, mel, audio, B, T, ws, st, s, ev, mel_host, audio_host);
+    return launch_generator_tc(packed, mel, audio, batch, ws, st, s, ev, mel_host, audio_host);
 }
 
 static int check_shape(const char *fn, int B, int T) {
     if (B < 1 || T < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: need B >= 1 and T >= 1 (got B=%d, T=%d)", fn, B, T);
     if ((long long)B * T > (1ll << 24)) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: B*T = %lld too large", fn, (long long)B * T);
+    return MG_OK;
+}
+
+// the ragged entry points' own arguments: B within the parameter tables' capacity, every length in [1, T_max]
+static int check_lengths(const char *fn, int B, int T_max, const int *lengths) {
+    int rc = check_shape(fn, B, T_max);
+    if (rc) return rc;
+    if (B > MG_GEN_RAGGED_MAX_B)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: B = %d exceeds MG_GEN_RAGGED_MAX_B = %d", fn, B, MG_GEN_RAGGED_MAX_B);
+    if (!lengths) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null lengths", fn);
+    for (int i = 0; i < B; ++i)
+        if (lengths[i] < 1 || lengths[i] > T_max)
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: lengths[%d] = %d is outside [1, T_max = %d]", fn, i, lengths[i], T_max);
     return MG_OK;
 }
 
@@ -80,17 +94,32 @@ size_t mg_gen_workspace_bytes(int B, int T) {
     return ws_offset(6, (size_t)B, (size_t)T) * sizeof(float) + 256;  // + pipeline status word
 }
 
+static int check_forward(const char *fn, const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
+                         size_t workspace_bytes) {
+    if (!packed || !mel || !audio || !workspace) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
+    if (workspace_bytes < mg_gen_workspace_bytes(B, T))
+        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "%s: workspace %zu < %zu bytes", fn, workspace_bytes, mg_gen_workspace_bytes(B, T));
+    if ((uintptr_t)packed % 16 || (uintptr_t)workspace % 16)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed/workspace must be 16-byte aligned", fn);
+    return MG_OK;
+}
+
 int mg_gen_forward(const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
                    size_t workspace_bytes, void *stream) {
     int rc = check_shape("mg_gen_forward", B, T);
+    if (!rc) rc = check_forward("mg_gen_forward", packed, mel, audio, B, T, workspace, workspace_bytes);
     if (rc) return rc;
-    if (!packed || !mel || !audio || !workspace) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_forward: null argument");
-    if (workspace_bytes < mg_gen_workspace_bytes(B, T))
-        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "mg_gen_forward: workspace %zu < %zu bytes", workspace_bytes,
-                         mg_gen_workspace_bytes(B, T));
-    if ((uintptr_t)packed % 16 || (uintptr_t)workspace % 16)
-        return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_forward: packed/workspace must be 16-byte aligned");
-    return run_generator((const float *)packed, mel, audio, B, T, (float *)workspace, (cudaStream_t)stream, nullptr);
+    return run_generator((const float *)packed, mel, audio, RunTable::uniform(B, T), (float *)workspace, (cudaStream_t)stream,
+                         nullptr);
+}
+
+int mg_gen_forward_ragged(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
+                          void *workspace, size_t workspace_bytes, void *stream) {
+    int rc = check_lengths("mg_gen_forward_ragged", B, T_max, lengths);
+    if (!rc) rc = check_forward("mg_gen_forward_ragged", packed, mel, audio, B, T_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    return run_generator((const float *)packed, mel, audio, RunTable::ragged(lengths, B, T_max), (float *)workspace,
+                         (cudaStream_t)stream, nullptr);
 }
 
 int mg_gen_forward_timed(const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
@@ -104,7 +133,7 @@ int mg_gen_forward_timed(const void *packed, const float *mel, float *audio, int
     const int n = mg_gen_forward_launches();  // events: one before each launch + one after the last
     cudaEvent_t ev[17];  // at most 12 kernels
     for (int i = 0; i <= n; ++i) MG_CUDA_TRY(cudaEventCreate(&ev[i]));
-    rc = run_generator((const float *)packed, mel, audio, B, T, (float *)workspace, (cudaStream_t)stream, ev);
+    rc = run_generator((const float *)packed, mel, audio, RunTable::uniform(B, T), (float *)workspace, (cudaStream_t)stream, ev);
     if (rc == MG_OK) {
         cudaError_t e = cudaEventSynchronize(ev[n]);
         if (e != cudaSuccess) rc = set_error(MG_ERR_CUDA, "mg_gen_forward_timed: %s", cudaGetErrorString(e));
@@ -244,7 +273,7 @@ int mg_loss_backward(const float *const *a, const float *const *b, const long lo
 
 int mg_gen_forward_launches(void) { return generator_tc_num_launches(); }
 
-int mg_gen_forward_slices(int B, int T) { return (B >= 1 && T >= 1) ? generator_tc_slices(B, T) : 1; }
+int mg_gen_forward_slices(int B, int T) { return (B >= 1 && T >= 1) ? generator_tc_slices(B, (long long)B * T) : 1; }
 
 int mg_gen_check_status(const void *workspace, int B, int T, void *stream) {
     int rc = check_shape("mg_gen_check_status", B, T);
@@ -261,21 +290,21 @@ int mg_gen_convt(const void *packed, int stage, const float *x, float *y, int B,
     if (!packed || !x || !y || x == y || stage < 0 || stage > 3 || B < 1 || Lin < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_convt: bad argument");
     return run_one_kernel("mg_gen_convt", (cudaStream_t)stream, [&](int *st) {
-        return launch_convt_tc(x, y, (const float *)packed, stage, B, Lin, st, (cudaStream_t)stream);
+        return launch_convt_tc(x, y, (const float *)packed, stage, RunTable::uniform(B, Lin), st, (cudaStream_t)stream);
     });
 }
 
 int mg_gen_conv_pre(const void *packed, const float *mel, float *y, int B, int T, void *stream) {
     if (!packed || !mel || !y || B < 1 || T < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_conv_pre: bad argument");
     return run_one_kernel("mg_gen_conv_pre", (cudaStream_t)stream, [&](int *st) {
-        return launch_gen_pre_tc(mel, y, (const float *)packed, B, T, st, (cudaStream_t)stream);
+        return launch_gen_pre_tc(mel, y, (const float *)packed, RunTable::uniform(B, T), st, (cudaStream_t)stream);
     });
 }
 
 int mg_gen_resblock_post(const void *packed, const float *x, float *audio, int B, int L, void *stream) {
     if (!packed || !x || !audio || B < 1 || L < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_resblock_post: bad argument");
     return run_one_kernel("mg_gen_resblock_post", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, audio, (const float *)packed, 4, B, L, st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, audio, (const float *)packed, 4, RunTable::uniform(B, L), st, (cudaStream_t)stream);
     });
 }
 
@@ -294,7 +323,7 @@ int mg_gen_resblock_trace(const void *packed, int stage, const float *x, float *
     MG_CUDA_TRY(cudaMalloc(&tr, 128 * sizeof(long long)));
     cudaMemset(st, 0, sizeof(int));
     cudaMemset(tr, 0, 128 * sizeof(long long));
-    int rc = launch_resblock_tc(x, y, (const float *)packed, stage, B, L, st, 0, tr);
+    int rc = launch_resblock_tc(x, y, (const float *)packed, stage, RunTable::uniform(B, L), st, 0, tr);
     if (rc == MG_OK && cudaDeviceSynchronize() != cudaSuccess) rc = set_error(MG_ERR_CUDA, "mg_gen_resblock_trace: kernel failed");
     if (rc == MG_OK) cudaMemcpy(trace_host, tr, 128 * sizeof(long long), cudaMemcpyDeviceToHost);
     cudaFree(st);
@@ -306,7 +335,7 @@ int mg_gen_resblock(const void *packed, int stage, const float *x, float *y, int
     if (!packed || !x || !y || x == y || stage < 0 || stage > 3 || B < 1 || L < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_resblock: bad argument");
     return run_one_kernel("mg_gen_resblock", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, y, (const float *)packed, stage, B, L, st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, y, (const float *)packed, stage, RunTable::uniform(B, L), st, (cudaStream_t)stream);
     });
 }
 
@@ -314,7 +343,7 @@ int mg_gen_resup(const void *packed, int stage, const float *x, float *y, int B,
     if (!packed || !x || !y || x == y || stage < 0 || stage > 2 || B < 1 || L < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_resup: bad argument");
     return run_one_kernel("mg_gen_resup", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, y, (const float *)packed, 20 + stage, B, L, st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, y, (const float *)packed, 20 + stage, RunTable::uniform(B, L), st, (cudaStream_t)stream);
     });
 }
 
@@ -322,7 +351,7 @@ int mg_gen_upres(const void *packed, int stage, const float *x, float *y, int B,
     if (!packed || !x || !y || x == y || (stage != 2 && stage != 3) || B < 1 || Lin < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_upres: bad argument");
     return run_one_kernel("mg_gen_upres", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, y, (const float *)packed, 10 + stage, B, 2 * Lin, st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, y, (const float *)packed, 10 + stage, RunTable::uniform(B, 2 * Lin), st, (cudaStream_t)stream);
     });
 }
 
@@ -330,7 +359,7 @@ int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, i
     if (!packed || !x || !audio || (const void *)x == (const void *)audio || B < 1 || Lin < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_upres_post: bad argument");
     return run_one_kernel("mg_gen_upres_post", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, audio, (const float *)packed, 14, B, 2 * Lin, st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, audio, (const float *)packed, 14, RunTable::uniform(B, 2 * Lin), st, (cudaStream_t)stream);
     });
 }
 
@@ -481,13 +510,17 @@ int mg_gen_engine_load_state(mg_gen_engine *e, const float *const *v, const floa
     return MG_OK;
 }
 
-int mg_gen_engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T) {
-    if (!e || !mel_host || !audio_host) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_engine_forward: null argument");
-    int rc = check_shape("mg_gen_engine_forward", B, T);
-    if (rc) return rc;
-    if (!e->loaded) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_engine_forward: no weights loaded");
+static int engine_check(const char *fn, mg_gen_engine *e, const float *mel_host, float *audio_host) {
+    if (!e || !mel_host || !audio_host) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
+    if (!e->loaded) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: no weights loaded", fn);
+    return MG_OK;
+}
+
+static int engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, const RunTable &batch) {
+    const int B = batch.items(), T = batch.stride;
     const size_t frames = (size_t)B * T;
-    if ((rc = engine_reserve(e, frames))) return rc;
+    int rc = engine_reserve(e, frames);
+    if (rc) return rc;
     const size_t nin = frames * kMelBins * sizeof(float), nout = frames * 256 * sizeof(float);
     cudaPointerAttributes at;
     const bool in_pinned = cudaPointerGetAttributes(&at, mel_host) == cudaSuccess && at.type == cudaMemoryTypeHost;
@@ -498,7 +531,7 @@ int mg_gen_engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_
     if (!e->pin_status) MG_CUDA_TRY(cudaMallocHost(&e->pin_status, sizeof(int)));
     MG_CUDA_TRY(cudaEventRecord(e->ev0, e->stream));
     // upload, kernels and download are enqueued per batch slice (launch_generator_tc); one synchronisation at the end
-    rc = run_generator(e->packed, e->mel, e->audio, B, T, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : e->pin_out);
+    rc = run_generator(e->packed, e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : e->pin_out);
     if (rc) return rc;
     MG_CUDA_TRY(cudaEventRecord(e->ev1, e->stream));
     *e->pin_status = 0;
@@ -509,6 +542,18 @@ int mg_gen_engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_
         return set_error(MG_ERR_CUDA, "mg_gen_engine_forward: tensor-core pipeline wait timed out (code %d)", *e->pin_status);
     MG_CUDA_TRY(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
     return MG_OK;
+}
+
+int mg_gen_engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T) {
+    int rc = engine_check("mg_gen_engine_forward", e, mel_host, audio_host);
+    if (!rc) rc = check_shape("mg_gen_engine_forward", B, T);
+    return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::uniform(B, T));
+}
+
+int mg_gen_engine_forward_ragged(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max, const int *lengths) {
+    int rc = check_lengths("mg_gen_engine_forward_ragged", B, T_max, lengths);
+    if (!rc) rc = engine_check("mg_gen_engine_forward_ragged", e, mel_host, audio_host);
+    return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::ragged(lengths, B, T_max));
 }
 
 int mg_gen_engine_last_kernel_ms(mg_gen_engine *e, float *ms) {

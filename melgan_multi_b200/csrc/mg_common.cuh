@@ -37,6 +37,88 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
 
+// A generator batch as runs of consecutive items of equal length: items [item0[r], item0[r+1]) hold len[r] positions
+// each, stored `stride` positions apart (the longest item's length, at the tensor's scale).  A uniform batch is one run,
+// a ragged one (mg_gen_forward_ragged) at most MG_GEN_RAGGED_MAX_B.  Each generator kernel takes the table BY VALUE
+// (__grid_constant__: read in place from the parameter bank) once its launcher has filled in the kernel's units -- ResBlock
+// clusters, or virtual rows for conv_pre and the ConvTs: run r has per[r] units per item and starts at unit first[r].
+// A grid of first[n] units covers every item and nothing past any item's end.
+struct RunPos {
+    int item, unit, len;  // item -1: the unit lies past the last run
+};
+struct RunTable {
+    int n, stride;
+    int item0[MG_GEN_RAGGED_MAX_B + 1], len[MG_GEN_RAGGED_MAX_B];
+    int first[MG_GEN_RAGGED_MAX_B + 1], per[MG_GEN_RAGGED_MAX_B];
+
+    static RunTable uniform(int B, int L) {
+        RunTable t;
+        t.n = 1;
+        t.stride = L;
+        t.item0[0] = 0;
+        t.item0[1] = B;
+        t.len[0] = L;
+        return t;
+    }
+    // lengths[0..B) (B <= MG_GEN_RAGGED_MAX_B, every length in [1, stride]), equal neighbours merged
+    static RunTable ragged(const int *lengths, int B, int stride) {
+        RunTable t;
+        t.n = 0;
+        t.stride = stride;
+        for (int i = 0; i < B; ++i)
+            if (i == 0 || lengths[i] != lengths[i - 1]) {
+                t.item0[t.n] = i;
+                t.len[t.n++] = lengths[i];
+            }
+        t.item0[t.n] = B;
+        return t;
+    }
+    int items() const { return item0[n]; }
+    // items [i0, i1) as a batch of their own (item i0 becomes item 0)
+    RunTable slice(int i0, int i1) const {
+        RunTable t;
+        t.n = 0;
+        t.stride = stride;
+        for (int r = 0; r < n; ++r) {
+            const int a = item0[r] > i0 ? item0[r] : i0, b = item0[r + 1] < i1 ? item0[r + 1] : i1;
+            if (a < b) {
+                t.item0[t.n] = a - i0;
+                t.len[t.n++] = len[r];
+            }
+        }
+        t.item0[t.n] = i1 - i0;
+        return t;
+    }
+    // every length and the stride times k (the same batch at a later stage's scale)
+    RunTable scaled(int k) const {
+        RunTable t = *this;
+        t.stride *= k;
+        for (int r = 0; r < n; ++r) t.len[r] *= k;
+        return t;
+    }
+    // per[r] = units(len[r]) units per item; first[] follows
+    template <class F>
+    void set_units(F units) {
+        first[0] = 0;
+        for (int r = 0; r < n; ++r) {
+            per[r] = units(len[r]);
+            first[r + 1] = first[r] + (item0[r + 1] - item0[r]) * per[r];
+        }
+    }
+    // unit f -> (item, unit within the item, the item's length)
+    __device__ __forceinline__ RunPos find(int f) const {
+        if (f < 0 || f >= first[n]) return {-1, 0, 0};
+        int lo = 0, hi = n;  // first[lo] <= f < first[hi]
+        while (hi - lo > 1) {
+            const int m = (lo + hi) >> 1;
+            if (first[m] <= f) lo = m;
+            else hi = m;
+        }
+        const int u = f - first[lo], k = (int)((unsigned)u / (unsigned)per[lo]);  // (unsigned: the shorter division)
+        return {item0[lo] + k, u - k * per[lo], len[lo]};
+    }
+};
+
 // Launch helper of the tensor-core kernels: optional programmatic dependent launch
 // (mg_tc.cuh pdl_*; MG_PDL=0 in the environment turns the attribute off for A/B runs); cluster > 1: thread-block clusters
 // of `cluster` consecutive CTAs along x (grid.x must be a multiple of it).
@@ -82,10 +164,11 @@ void generator_tc_set_tail(int mask);
 const char *generator_tc_kernel_name(int i);
 const char *generator_tc_kernel_config(int i, int T);
 const char *resblock_config_name(int stage, int L);
-int generator_tc_slices(int B, int T);  // batch slices (concurrent kernel chains) one forward is cut into
-int launch_generator_tc(const float *packed, const float *mel, float *audio, int B, int T, float *ws, int *status,
+int generator_tc_slices(int B, long long frames);  // batch slices (concurrent kernel chains) one forward is cut into
+// batch: the items' mel lengths, stride T_max (the layout of mel, audio and every workspace buffer)
+int launch_generator_tc(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
                         cudaStream_t s, cudaEvent_t *ev = nullptr, const float *mel_host = nullptr, float *audio_host = nullptr);
-int launch_gen_pre_tc(const float *mel, float *y, const float *packed, int B, int T, int *status, cudaStream_t s);
+int launch_gen_pre_tc(const float *mel, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s);
 int launch_disc_post1_tc(const float *x, float *y, const uint8_t *wtc, const float *bias, int Bt, int L, int *status,
                          cudaStream_t s);
 int launch_disc_post1_dgrad_tc(const float *dz, float *dx, const uint8_t *wtcT, const float *zero_bias, int Bt, int L, int *status,
@@ -124,8 +207,9 @@ int mel_tables_build(int sr, int n_mels, float fmin, float fmax, int norm, MelTa
 int mel_frames(int L);
 int launch_mel(const void *tables, const float *audio, float *mel, int B, int L, cudaStream_t s);
 int launch_msd_forward(const void *packed, const float *y, int Bt, int L, float *const *fmaps, int *status, cudaStream_t s);
-int launch_convt_tc(const float *x, float *y, const float *packed, int stage, int B, int Lin, int *status, cudaStream_t s);
-int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, int B, int L, int *status, cudaStream_t s,
+// batch: lengths and stride of the kernel's input (ConvT) / of the ResBlock itself (the output length for codes 12..14)
+int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s);
+int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
                        long long *trace = nullptr);
 
 }  // namespace mg

@@ -42,10 +42,21 @@ struct ConvCfg {
 
 // packed weights for this kernel: conv_tc_weight_index() in mg_layout.h
 
-template <class Cfg>
+// Virtual row -> (item, position, the item's length); item -1: no item.  The discriminators' batches are dense: B items of
+// L positions, PAD zero rows after each.  The generator's conv_pre takes a RunTable instead (ragged batches; one unit
+// per virtual row, L_i + PAD of them per item, items `stride` positions apart).
+struct DenseRows {
+    int stride, B, pad;
+    __device__ __forceinline__ RunPos find(int v) const {
+        const int Lv = stride + pad, item = v >= 0 ? v / Lv : 0;
+        return (v >= 0 && item < B) ? RunPos{item, v - item * Lv, stride} : RunPos{-1, 0, 0};
+    }
+};
+
+template <class Cfg, class Rows>
 __global__ void __launch_bounds__(Cfg::NT, 1)
 conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const uint8_t *__restrict__ wtc,
-                    const float *__restrict__ bias, int L, int B, int *__restrict__ status) {
+                    const float *__restrict__ bias, const __grid_constant__ Rows rows, int *__restrict__ status) {
     constexpr int CIN = Cfg::CIN, COUT = Cfg::COUT, NTAP = Cfg::NTAP, PAD = Cfg::PAD, KCA = Cfg::KCA, N = Cfg::N;
     constexpr int ROWS = Cfg::ROWS, APITCH = Cfg::APITCH, ASLOT = Cfg::ASLOT, BSLOT = Cfg::BSLOT;
     constexpr int NSA = Cfg::NSA, NSB = Cfg::NSB, NCONV = Cfg::NCONV, NMW = Cfg::NMW;
@@ -56,7 +67,7 @@ conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const ui
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * ROWS, cg = blockIdx.y;
-    const int Lv = L + PAD;  // virtual rows per item: L positions + PAD zero rows
+    const int L = rows.stride;  // positions between items in x and y
 
     if (tid == 0) {
         for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NMW); }
@@ -129,10 +140,9 @@ conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const ui
         const float *bp = bias + cg * N;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            const int v = r0 + 64 * mw + frag_row(t, h);
-            const int item = v / Lv, s = v - item * Lv;
-            if (item < B && s < L) {
-                float *yp = y + ((size_t)item * COUT + cg * N) * L + s;
+            const RunPos p = rows.find(r0 + 64 * mw + frag_row(t, h));
+            if (p.item >= 0 && p.unit < p.len) {
+                float *yp = y + ((size_t)p.item * COUT + cg * N) * L + p.unit;
 #pragma unroll
                 for (int k = 0; k < N / 8; ++k)
 #pragma unroll
@@ -153,10 +163,9 @@ conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const ui
         int sa = 0, pha = 0;
         bool ok = true;
         constexpr int NCH = CIN / KCA;
-        const int v0 = r0 - PAD + tid;
-        const int item0 = v0 >= 0 ? v0 / Lv : 0, s0 = v0 - item0 * Lv;
-        const bool inr0 = (v0 >= 0 && item0 < B && s0 < L);
-        const float *xrow = x + (size_t)(inr0 ? item0 : 0) * CIN * L + (inr0 ? s0 : 0);
+        const RunPos p0 = rows.find(r0 - PAD + tid);
+        const bool inr0 = p0.item >= 0 && p0.unit < p0.len;
+        const float *xrow = x + (size_t)(inr0 ? p0.item : 0) * CIN * L + (inr0 ? p0.unit : 0);
         auto store_row = [&](uint8_t *slot, int i, const float *f) {
 #pragma unroll
             for (int kp = 0; kp < KCA / 8; ++kp) {
@@ -170,10 +179,9 @@ conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const ui
         auto tail_rows = [&](uint8_t *slot, int ca) {
 #pragma unroll 1
             for (int i = NCONV + tid; i < ROWS + 2 * PAD; i += NCONV) {
-                const int v = r0 - PAD + i;
-                const int item = v >= 0 ? v / Lv : 0, s = v - item * Lv;
-                const bool inr = (v >= 0 && item < B && s < L);
-                const float *xp = x + ((size_t)(inr ? item : 0) * CIN + ca * KCA) * L + (inr ? s : 0);
+                const RunPos p = rows.find(r0 - PAD + i);
+                const bool inr = p.item >= 0 && p.unit < p.len;
+                const float *xp = x + ((size_t)(inr ? p.item : 0) * CIN + ca * KCA) * L + (inr ? p.unit : 0);
                 float f[KCA];
 #pragma unroll
                 for (int j = 0; j < KCA; ++j) f[j] = inr ? __ldg(xp + (size_t)j * L) : 0.f;
@@ -207,19 +215,26 @@ conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const ui
     }
 }
 
-template <class Cfg>
-static int launch_conv_rows(const float *x, float *y, const uint8_t *wtc, const float *bias, int B, int L, int *status,
-                            cudaStream_t s) {
+// vrows: virtual rows of the batch (the grid covers them in 128-row tiles)
+template <class Cfg, class Rows>
+static int launch_conv_rows(const float *x, float *y, const uint8_t *wtc, const float *bias, const Rows &rows, long long vrows,
+                            int *status, cudaStream_t s) {
     static bool configured = false;
     if (!configured) {
-        MG_CUDA_TRY(cudaFuncSetAttribute(conv_rows_tc_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        MG_CUDA_TRY(cudaFuncSetAttribute(conv_rows_tc_kernel<Cfg, Rows>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         Cfg::SMEM_BYTES));
         configured = true;
     }
-    const long long vrows = (long long)B * (L + Cfg::PAD);
     const unsigned tiles = (unsigned)((vrows + Cfg::ROWS - 1) / Cfg::ROWS);
-    MG_CUDA_TRY(launch_ex(conv_rows_tc_kernel<Cfg>, dim3(tiles, Cfg::NCG), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, 1, x, y, wtc, bias,
-                          L, B, status));
+    MG_CUDA_TRY(launch_ex(conv_rows_tc_kernel<Cfg, Rows>, dim3(tiles, Cfg::NCG), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, 1, x, y, wtc,
+                          bias, rows, status));
     return MG_OK;
+}
+
+template <class Cfg>
+static int launch_conv_dense(const float *x, float *y, const uint8_t *wtc, const float *bias, int B, int L, int *status,
+                             cudaStream_t s) {
+    return launch_conv_rows<Cfg>(x, y, wtc, bias, DenseRows{L, B, Cfg::PAD}, (long long)B * (L + Cfg::PAD), status, s);
 }
 
 using PreCfg = ConvCfg<80, 512, 7, 80, false, kPreNG>;  // generator conv_pre
@@ -228,22 +243,24 @@ using PreCfg = ConvCfg<80, 512, 7, 80, false, kPreNG>;  // generator conv_pre
 using Post1Cfg = ConvCfg<1024, 1024, 5, 32, true, kPost1NG>;
 using Post1DgradCfg = ConvCfg<1024, 1024, 5, 32, false, kPost1NG>;  // the same contraction on the transposed blob, no activation
 
-// mel [B][80][T] -> y [B][512][T]   (Generator.conv_pre)
-int launch_gen_pre_tc(const float *mel, float *y, const float *packed, int B, int T, int *status, cudaStream_t s) {
+// mel [B][80][T_max] -> y [B][512][T_max]   (Generator.conv_pre), item i's first len_i positions
+int launch_gen_pre_tc(const float *mel, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s) {
     const uint8_t *wtc = reinterpret_cast<const uint8_t *>(packed) + tc_region_start() + tc_pre_offset();
-    return launch_conv_rows<PreCfg>(mel, y, wtc, packed + bias_offset(0), B, T, status, s);
+    RunTable rows = batch;
+    rows.set_units([](int L) { return L + PreCfg::PAD; });
+    return launch_conv_rows<PreCfg>(mel, y, wtc, packed + bias_offset(0), rows, rows.first[rows.n], status, s);
 }
 
 // x [Bt][1024][L] -> y [Bt][1024][L] = lrelu(conv_post1(x))   (Discriminator.conv_post1)
 int launch_disc_post1_tc(const float *x, float *y, const uint8_t *wtc, const float *bias, int Bt, int L, int *status,
                          cudaStream_t s) {
-    return launch_conv_rows<Post1Cfg>(x, y, wtc, bias, Bt, L, status, s);
+    return launch_conv_dense<Post1Cfg>(x, y, wtc, bias, Bt, L, status, s);
 }
 
 // dz [Bt][1024][L] -> dx [Bt][1024][L]: data gradient of conv_post1 (autograd of models.py:96), wtcT = blob + d_tcT_start()
 int launch_disc_post1_dgrad_tc(const float *dz, float *dx, const uint8_t *wtcT, const float *zero_bias, int Bt, int L, int *status,
                                cudaStream_t s) {
-    return launch_conv_rows<Post1DgradCfg>(dz, dx, wtcT, zero_bias, Bt, L, status, s);
+    return launch_conv_dense<Post1DgradCfg>(dz, dx, wtcT, zero_bias, Bt, L, status, s);
 }
 
 }  // namespace mg

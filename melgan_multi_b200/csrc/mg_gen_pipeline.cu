@@ -87,10 +87,11 @@ const char *generator_tc_kernel_config(int i, int T) {
     return st[i].kind == 0 ? "conv_rows_tc_kernel<ConvCfg<80,512,7>>" : "convt_tc_kernel";
 }
 
-// Tensor-core pipeline of one contiguous slice of the batch.  a0: conv_pre output; a[0]: ResBlock-0 output (unfused chains);
-// a[1], a[2], u: three buffers of 8192 T floats per item that the stages rotate through (a kernel never writes its input).
-static int generator_tc_chain(const float *packed, const float *mel, float *audio, int B, int T, float *a0, float *const *a,
-                              float *u, int *status, cudaStream_t s, cudaEvent_t *ev) {
+// Tensor-core pipeline of one contiguous slice of the batch (mel lengths, stride T_max).  a0: conv_pre output; a[0]:
+// ResBlock-0 output (unfused chains); a[1], a[2], u: three buffers of 8192 T_max floats per item that the stages rotate
+// through (a kernel never writes its input).  Every kernel gets the batch at its own scale.
+static int generator_tc_chain(const float *packed, const float *mel, float *audio, const RunTable &batch, float *a0,
+                              float *const *a, float *u, int *status, cudaStream_t s, cudaEvent_t *ev) {
     ChainStep st[12];
     const int n = build_chain(st);
     int rc;
@@ -101,16 +102,16 @@ static int generator_tc_chain(const float *packed, const float *mel, float *audi
         return nullptr;
     };
     const float *cur = mel;
-    int len = T;  // length of `cur`
+    int len = 1;  // positions of `cur` per mel frame
     for (int i = 0; i < n; ++i) {
         if (ev) MG_CUDA_TRY(cudaEventRecord(ev[i], s));
         const ChainStep &k = st[i];
         if (k.kind == 0) {
-            if ((rc = launch_gen_pre_tc(cur, a0, packed, B, T, status, s))) return rc;
+            if ((rc = launch_gen_pre_tc(cur, a0, packed, batch, status, s))) return rc;
             cur = a0;
         } else if (k.kind == 1) {
             float *out = cur != u ? u : other(cur, nullptr);  // (unfused chain: ConvT outputs live in u, ResBlock i's in a[i])
-            if ((rc = launch_convt_tc(cur, out, packed, k.arg, B, len, status, s))) return rc;
+            if ((rc = launch_convt_tc(cur, out, packed, k.arg, batch.scaled(len), status, s))) return rc;
             cur = out;
             len *= stage_stride(k.arg);
         } else {
@@ -119,7 +120,7 @@ static int generator_tc_chain(const float *packed, const float *mel, float *audi
             const bool front = k.arg >= 12 && k.arg <= 14, tailf = k.arg >= 20;
             float *out = last ? audio : (k.arg <= 2 && cur != a[k.arg]) ? a[k.arg] : other(cur, nullptr);
             const int Lk = front ? 2 * len : len;  // the ResBlock's own length
-            if ((rc = launch_resblock_tc(cur, out, packed, k.arg, B, Lk, status, s))) return rc;
+            if ((rc = launch_resblock_tc(cur, out, packed, k.arg, batch.scaled(Lk), status, s))) return rc;
             cur = out;
             len = tailf ? Lk * stage_stride(k.arg - 20 + 1) : Lk;
         }
@@ -153,7 +154,8 @@ struct SliceStreams {
 // the block scheduler fills the SMs one chain's partial last wave leaves idle (stage 0 at config 2 is 512 one-per-SM
 // tiles on 132 SMs) with the other chain's tiles.  Same kernels, same per-item arithmetic: results are bit-identical
 // to the single-chain order.  ev != nullptr (per-kernel timing) keeps everything on one stream.
-int generator_tc_slices(int B, int T) {
+// frames: mel frames of the whole batch (B T for a uniform one); the parts hold about equal shares of them.
+int generator_tc_slices(int B, long long frames) {
     static const int forced = [] {  // MG_GEN_SLICES=n pins the slice count (experiments); default: chosen from the shape
         const char *e = getenv("MG_GEN_SLICES");
         const int v = e ? atoi(e) : 0;
@@ -161,16 +163,33 @@ int generator_tc_slices(int B, int T) {
     }();
     // slicing pays while a slice still fills the machine: >= 512 mel frames per slice (stage-0 tiles ~ frames / 11)
     int slices = forced ? forced : 4;
-    while (slices > 1 && ((!forced && (long long)B * T < 512ll * slices) || B < slices)) --slices;
+    while (slices > 1 && ((!forced && frames < 512ll * slices) || B < slices)) --slices;
     return slices;
 }
 
 // mel_host / audio_host (both or neither; pinned): the host-buffer entry point's copies, cut the same way -- each slice's
-// stream uploads its mel slice before its chain and downloads its audio slice after it, so all but the last download
-// overlap the other chains' kernels.
-int launch_generator_tc(const float *packed, const float *mel, float *audio, int B, int T, float *ws, int *status,
+// stream uploads its items' valid mel prefixes before its chain and downloads its audio rows (valid prefix and zero tail)
+// after it, so all but the last download overlap the other chains' kernels.
+int launch_generator_tc(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
                         cudaStream_t s, cudaEvent_t *ev, const float *mel_host, float *audio_host) {
-    const int slices = ev ? 1 : generator_tc_slices(B, T);
+    const int B = batch.items(), T = batch.stride;
+    long long frames = 0;
+    for (int r = 0; r < batch.n; ++r) frames += (long long)(batch.item0[r + 1] - batch.item0[r]) * batch.len[r];
+    int slices = ev ? 1 : generator_tc_slices(B, frames);
+    // slice k = items [cut[k], cut[k + 1]): cut where the running frame count passes k / slices of the total, leaving at
+    // least one item for every later slice
+    int cut[SliceStreams::kMax + 1] = {0};
+    {
+        long long acc = 0;
+        int k = 0;
+        for (int r = 0; r < batch.n; ++r)
+            for (int i = batch.item0[r]; i < batch.item0[r + 1]; ++i) {
+                acc += batch.len[r];
+                if (k < slices - 1 && acc * slices >= frames * (k + 1) && B - (i + 1) >= slices - 1 - k) cut[++k] = i + 1;
+            }
+        slices = k + 1;
+        cut[slices] = B;
+    }
     float *base[6];
     for (int i = 0; i < 6; ++i) base[i] = ws + ws_offset(i, B, T);
     const size_t per_item[6] = {(size_t)512 * T, (size_t)256 * 8 * T, (size_t)128 * 64 * T, (size_t)64 * 128 * T, 0, (size_t)8192 * T};
@@ -187,19 +206,26 @@ int launch_generator_tc(const float *packed, const float *mel, float *audio, int
         MG_CUDA_TRY(cudaEventRecord(ss.fork, s));
     }
     int forked = 0;  // side streams that wait on `fork` so far: all of them are joined back, also on the error path
-    for (int k = 0, b0 = 0; k < slices && rc == MG_OK; ++k) {
-        const int nb = B / slices + (k < B % slices);
+    for (int k = 0; k < slices && rc == MG_OK; ++k) {
+        const int b0 = cut[k], nb = cut[k + 1] - b0;
+        const RunTable part = batch.slice(b0, cut[k + 1]);
         cudaStream_t q = k == 0 ? s : ss.st[k - 1];
         auto slice = [&]() -> int {
             if (k > 0) {
                 MG_CUDA_TRY(cudaStreamWaitEvent(q, ss.fork, 0));
                 forked = k;
             }
-            if (mel_host)
-                MG_CUDA_TRY(cudaMemcpyAsync(const_cast<float *>(mel) + b0 * mel_item, mel_host + b0 * mel_item,
-                                            nb * mel_item * sizeof(float), cudaMemcpyHostToDevice, q));
+            for (int r = 0; mel_host && r < part.n; ++r) {  // one copy per run: rows of len floats, T apart
+                const size_t off = (b0 + part.item0[r]) * mel_item, rows = (size_t)(part.item0[r + 1] - part.item0[r]) * kMelBins;
+                float *dst = const_cast<float *>(mel) + off;
+                if (part.len[r] == T)
+                    MG_CUDA_TRY(cudaMemcpyAsync(dst, mel_host + off, rows * T * sizeof(float), cudaMemcpyHostToDevice, q));
+                else
+                    MG_CUDA_TRY(cudaMemcpy2DAsync(dst, T * sizeof(float), mel_host + off, T * sizeof(float), part.len[r] * sizeof(float),
+                                                  rows, cudaMemcpyHostToDevice, q));
+            }
             float *a[3] = {base[1] + b0 * per_item[1], base[2] + b0 * per_item[2], base[3] + b0 * per_item[3]};
-            int r = generator_tc_chain(packed, mel + b0 * mel_item, audio + b0 * audio_item, nb, T, base[0] + b0 * per_item[0], a,
+            int r = generator_tc_chain(packed, mel + b0 * mel_item, audio + b0 * audio_item, part, base[0] + b0 * per_item[0], a,
                                        base[5] + b0 * per_item[5], status, q, ev);
             if (r) return r;
             if (audio_host)
@@ -208,7 +234,6 @@ int launch_generator_tc(const float *packed, const float *mel, float *audio, int
             return MG_OK;
         };
         rc = slice();
-        b0 += nb;
     }
     for (int k = 1; k <= forked; ++k) {  // join (best effort after an error: the caller's stream must not outrun a forked one)
         cudaError_t e = cudaEventRecord(ss.join[k - 1], ss.st[k - 1]);

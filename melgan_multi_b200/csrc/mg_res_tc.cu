@@ -89,7 +89,7 @@ struct RbCfg {
     static constexpr int PVB = CS * P - HALO - HL, XCH = 9;
     static_assert(CS == 1 || ((CS == 2 || CS == 4) && !POST_ && !UPF_ && UPT_ == 0 && XCH <= SLACK && 2 * XCH <= P),
                   "clusters are for the plain ResBlock");
-    static constexpr int SMEM_BYTES = 2 * XBYTES + NSTAGE * CHUNK + 2 * C * 4 + (2 * NSTAGE + (CS > 1 ? 2 : 0)) * 8;
+    static constexpr int SMEM_BYTES = 2 * XBYTES + NSTAGE * CHUNK + 2 * C * 4 + (2 * NSTAGE + (CS > 1 ? 2 : 0) + 1) * 8;
     static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "shared memory budget");
     static_assert(XPITCH / 16 < 16384, "LBO field");
     static_assert(NRB % RPW == 0 && C % NCP == 0 && NCW % 32 == 0, "warpgroup split");
@@ -103,8 +103,8 @@ __device__ __forceinline__ void acc_fence2(float (&a)[RPW][R]) {
 
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NT, 1)
-resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed, int stage, int L, int nB,
-                   int *__restrict__ status, long long *__restrict__ trace) {
+resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed, int stage,
+                   const __grid_constant__ RunTable clusters, int *__restrict__ status, long long *__restrict__ trace) {
     constexpr int C = Cfg::C, P = Cfg::P, SLACK = Cfg::SLACK, HALO = Cfg::HALO, HL = Cfg::HL;
     constexpr int XPITCH = Cfg::XPITCH, XBYTES = Cfg::XBYTES, KC = Cfg::KC, CHUNK = Cfg::CHUNK, NSTAGE = Cfg::NSTAGE;
     constexpr int NCONS = Cfg::NCONS, NCP = Cfg::NCP, NCW = Cfg::NCW, RPW = Cfg::RPW, KSL = Cfg::KSL, NA = NCW / 2;
@@ -119,11 +119,19 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     // per X hand-off), hfree once every neighbour's MMAs have finished reading its X (one phase per conv): then the copies
     // of this CTA's border rows have been read, and the neighbours' slack rows may be refilled
     uint64_t *hfull = empty + NSTAGE, *hfree = hfull + 1;
+    // (item, its length), read back by each phase: held in registers they would stay live across every MMA loop, and the
+    // stage-0 configuration is at its register cap
+    int *item_len = reinterpret_cast<int *>(empty + NSTAGE + (CS > 1 ? 2 : 0));
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // a cluster is CS consecutive CTAs along x (launch_resblock): rank crank of cluster clus owns the cluster's rows
-    // [crank P, (crank + 1) P)
-    const int b = blockIdx.y, clus = blockIdx.x / CS, crank = blockIdx.x % CS;
+    // a cluster is CS consecutive CTAs along x (launch_resblock): rank crank of cluster clus of item b owns the cluster's
+    // rows [crank P, (crank + 1) P).  The grid is item-major; an item's clusters never reach into the next item.  L: the
+    // item's own length (every edge decision), Ls: positions between items in x and y.
+    const int crank = blockIdx.x % CS;
+    const RunPos cp = clusters.find(blockIdx.x / CS);
+    const int clus = cp.unit, Ls = clusters.stride;
+    auto item = [&]() { return *reinterpret_cast<volatile int *>(&item_len[0]); };
+    auto len = [&]() { return *reinterpret_cast<volatile int *>(&item_len[1]); };
     // Edge-aware tiling: a halo is only needed where the cluster (one CTA for CS = 1) borders MORE sequence.  Cluster 0
     // starts at position 0 (its left edge is the real zero padding) and keeps CS P - HALO outputs; later clusters keep
     // CS P - HALO - HL, and a cluster that reaches the end of the sequence keeps its right HALO rows too.  Cluster-internal
@@ -131,13 +139,15 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     // runs the whole protocol (its neighbours write into its shared memory).
     const int oc = clus == 0 ? 0 : (CS * P - HALO) + (clus - 1) * Cfg::PVB - HL;  // position of the cluster's row 0
     const int o = oc + crank * P;                                                 // position of tile row 0
-    const int p_lo = (clus == 0 || crank > 0) ? 0 : HL, p_hi = (crank < CS - 1 || oc + CS * P >= L) ? P : P - HALO;
-    const bool interior = (o >= 0 && o + P <= L);  // every row of the tile is a real position
+    const int p_lo = (clus == 0 || crank > 0) ? 0 : HL, p_hi = (crank < CS - 1 || oc + CS * P >= cp.len) ? P : P - HALO;
+    const bool interior = (o >= 0 && o + P <= cp.len);  // every row of the tile is a real position
     // consumption order of the six convs of ResBlock `stage`: c1[0], c2[0], c1[1], c2[1], c1[2], c2[2]
     const int l0 = 5 + 6 * stage;
     const uint8_t *tc_base = reinterpret_cast<const uint8_t *>(packed) + tc_region_start();
 
     if (tid == 0) {
+        item_len[0] = cp.item;
+        item_len[1] = cp.len;
         for (int s = 0; s < NSTAGE; ++s) {
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], Cfg::NWG * CS);  // one arrival per consumer warpgroup of every CTA of the cluster
@@ -160,7 +170,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     if constexpr (CS > 1) cluster_sync();  // every CTA's barriers are initialised before any remote access
     // optional timeline of one interior CTA (clock64 stamps of thread 0; see mg_gen_resblock_trace); per conv c = 0..5 the
     // slots 2 + 3c (X handed over), 3 + 3c (accumulator ready), 4 + 3c (next X written) are 2 + 6j .. 7 + 6j of conv pair j
-    const bool tr = trace && blockIdx.y == 0 && blockIdx.x == (gridDim.x > 1 ? 1u : 0u) && tid == 0;
+    const bool tr = trace && blockIdx.x == (gridDim.x > 1 ? 1u : 0u) && tid == 0;
 #define MG_TR(slot) do { if (tr) trace[slot] = clock64(); } while (0)
 
     if (warp == NCONS / 32) {
@@ -249,6 +259,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     // X <- split(lrelu(A + bias)) for this warpgroup's rows and columns, zero outside [0, L); keep_last: also park the
     // fp32 lrelu(x[L-1]) in b1s (the tail ConvT's fix-up)
     auto write_x = [&](float (&A)[RPW][NA], const float *bsrc, bool keep_last) {
+        const int L = len();
 #pragma unroll
         for (int r = 0; r < RPW; ++r)
 #pragma unroll
@@ -345,17 +356,18 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     MG_TR(0);
     if constexpr (Cfg::UPF) {
         constexpr int UROWS = Cfg::UROWS, UPITCH = Cfg::UPITCH, SPITCH = Cfg::SPITCH, UKSL = Cfg::UKSL;
-        const int Lin = L >> 1, s0 = (o >> 1) - 1;  // A row i <-> input position s0 + i (o is even)
+        const int b = item(), L = len();
+        const int Lin = L >> 1, Lins = Ls >> 1, s0 = (o >> 1) - 1;  // A row i <-> input position s0 + i (o is even)
         // ---- ConvT operand: A <- split(lrelu(x_in)), 2C channels of UROWS input positions; consecutive threads take
         // consecutive positions of one 8-channel k-panel
 #pragma unroll 1
         for (int idx = tid; idx < UROWS * 2 * Cfg::KP; idx += NCONS) {
             const int i = idx % UROWS, kp = idx / UROWS, sp = s0 + i;
             const bool inr = (sp >= 0 && sp < Lin);
-            const float *xp = x + ((size_t)b * 2 * C + 8 * kp) * Lin + (inr ? sp : 0);
+            const float *xp = x + ((size_t)b * 2 * C + 8 * kp) * Lins + (inr ? sp : 0);
             float f[8];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] = inr ? lrelu(__ldg(xp + (size_t)j * Lin)) : 0.f;
+            for (int j = 0; j < 8; ++j) f[j] = inr ? lrelu(__ldg(xp + (size_t)j * Lins)) : 0.f;
             uint32_t h[4], l[4];
 #pragma unroll
             for (int e = 0; e < 4; ++e) split2_bf16(f[2 * e], f[2 * e + 1], h[e], l[e]);
@@ -425,18 +437,19 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         }
     } else {
         // ---- load the input tile: R <- x (fp32, exact), X <- split(lrelu(x))
+        const int b = item(), L = len();
 #pragma unroll
         for (int r = 0; r < RPW; ++r)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int p = (rb0 + r) * 64 + frag_row(t, h), tp = o + p;
                 const bool inr = (tp >= 0 && tp < L);
-                const float *xp = x + (size_t)b * C * L + (inr ? tp : 0);
+                const float *xp = x + (size_t)b * C * Ls + (inr ? tp : 0);
 #pragma unroll
                 for (int k = 0; k < NCW / 8; ++k)
 #pragma unroll
                     for (int e = 0; e < 2; ++e)
-                        R[r][4 * k + 2 * h + e] = inr ? __ldg(xp + (size_t)(c0 + frag_col(q, 4 * k + e)) * L) : 0.f;
+                        R[r][4 * k + 2 * h + e] = inr ? __ldg(xp + (size_t)(c0 + frag_col(q, 4 * k + e)) * Ls) : 0.f;
             }
     }
     hand_off(R, pend, false);  // (pend is still all zeros)
@@ -480,7 +493,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int p = (rb0 + r) * 64 + frag_row(t, h), tp = o + p;
-                const bool inr = (tp >= 0 && tp < L);
+                const bool inr = (tp >= 0 && tp < len());
                 float qk[kPostK];
 #pragma unroll
                 for (int k = 0; k < kPostK; ++k) qk[k] = 0.f;
@@ -507,6 +520,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                 }
             }
         sync_cons();
+        const int b = item(), L = len();
         const float bpost = __ldg(packed + bias_offset(29));
 #pragma unroll 1
         for (int p = tid; p < P; p += NCONS) {
@@ -518,13 +532,16 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                     const int pp = p + k - 3;  // outside the tile only where it is outside the sequence too (zero padding)
                     if (pp >= 0 && pp < P) acc += Q[k * P + pp];
                 }
-                y[(size_t)b * L + tp] = tanhf(acc);
+                y[(size_t)b * Ls + tp] = tanhf(acc);
             }
         }
+        if (oc + P >= L)  // the item's last CTA: the audio past the item's end reads 0 (ragged batches)
+            for (int p = L + tid; p < Ls; p += NCONS) y[(size_t)b * Ls + p] = 0.f;
     } else if constexpr (Cfg::UPT != 0) {
         // ---- tail ConvT: D[s, phi*TNG + co] (+)= X[s - tap, :] * Wstack_tap^T over the C channels of X = split(lrelu(x_out))
         constexpr int S = Cfg::UPT, TNG = Cfg::TNG, TN = Cfg::TN, PADT = S / 2, COT = C / 2;
-        const int Lout = S * L;
+        const int b = item(), L = len();
+        const int Lout = S * Ls;  // output positions between items
         const float *tbias = packed + bias_offset(1 + stage + 1);
         // ---- fix-up first (it only needs b1s[]): out[co][S L - pad + j] = bias + sum_ci lrelu(x[ci][L-1]) * W[ci][co][j + S],
         // j < pad (the outputs position L would own: x[L] = 0 leaves only the x[L-1] tap), by the CTA whose owned rows include
@@ -619,19 +636,20 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     } else {
         // ---- store the valid part of R + pend
         pdl_trigger();
+        const int b = item(), L = len();
 #pragma unroll
         for (int r = 0; r < RPW; ++r)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int p = (rb0 + r) * 64 + frag_row(t, h), tp = o + p;
                 if (p >= p_lo && p < p_hi && tp < L) {
-                    float *yp = y + (size_t)b * C * L + tp;
+                    float *yp = y + (size_t)b * C * Ls + tp;
 #pragma unroll
                     for (int k = 0; k < NCW / 8; ++k)
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int col = c0 + frag_col(q, 4 * k + e);
-                            yp[(size_t)col * L] = R[r][4 * k + 2 * h + e] + pend[col];
+                            yp[(size_t)col * Ls] = R[r][4 * k + 2 * h + e] + pend[col];
                         }
                 }
             }
@@ -643,7 +661,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
 }
 
 template <class Cfg>
-static int launch_resblock(const float *x, float *y, const float *packed, int stage, int B, int L, int *status,
+static int launch_resblock(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status,
                            long long *trace, cudaStream_t s) {
     static bool configured = false;
     if (!configured) {
@@ -651,11 +669,12 @@ static int launch_resblock(const float *x, float *y, const float *packed, int st
         configured = true;
     }
     constexpr int CS = Cfg::CS, PC = CS * Cfg::P, PVB = Cfg::PVB;  // edge-aware tiling of CS * P-position clusters, see the kernel
-    const int nclusters = 1 + (L > PC ? (L - PC + PVB - 1) / PVB : 0);
-    if (B > 65535) return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: batch %d exceeds the grid", B);
+    RunTable clusters = batch;
+    clusters.set_units([](int L) { return 1 + (L > PC ? (L - PC + PVB - 1) / PVB : 0); });
+    const dim3 grid(CS * clusters.first[clusters.n]);
     if (trace && CS > 1) {  // diagnostic: clusters resident at once (GPC boundaries can leave SMs idle), into trace[127]
         cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(CS * nclusters, B);
+        cfg.gridDim = grid;
         cfg.blockDim = dim3(Cfg::NT);
         cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
         cudaLaunchAttribute attr;
@@ -669,8 +688,8 @@ static int launch_resblock(const float *x, float *y, const float *packed, int st
         const long long v = n;
         MG_CUDA_TRY(cudaMemcpy(trace + 127, &v, sizeof(v), cudaMemcpyHostToDevice));
     }
-    MG_CUDA_TRY(launch_ex(resblock_tc_kernel<Cfg>, dim3(CS * nclusters, B), dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, CS, x, y, packed,
-                          stage, L, B, status, trace));
+    MG_CUDA_TRY(launch_ex(resblock_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, CS, x, y, packed, stage, clusters,
+                          status, trace));
     return MG_OK;
 }
 
@@ -703,21 +722,22 @@ using Rb0Up1 = RbCfg<256, 1, 1, 2, 4, false, false, 8>;
 using Rb1Up2 = RbCfg<128, 2, 1, 1, 4, false, false, 2>;
 using Rb2Up3 = RbCfg<64, 4, 1, 1, 3, false, false, 2>;
 
-// x, y: [B][C][L] fp32 NCL with C = 256 >> stage; status: device int, set non-zero if a pipeline wait timed out.
-int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, int B, int L, int *status, cudaStream_t s,
+// x, y: [B][C][L] fp32 NCL with C = 256 >> stage, L = batch.stride, item i's first len_i positions its own; status: device
+// int, set non-zero if a pipeline wait timed out.
+int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
                        long long *trace) {
     switch (stage) {
-        case 0: return launch_resblock<Rb0>(x, y, packed, 0, B, L, status, trace, s);
-        case 1: return launch_resblock<Rb1>(x, y, packed, 1, B, L, status, trace, s);
-        case 2: return launch_resblock<Rb2>(x, y, packed, 2, B, L, status, trace, s);
-        case 3: return launch_resblock<Rb3>(x, y, packed, 3, B, L, status, trace, s);
-        case 4: return launch_resblock<Rb3Post>(x, y, packed, 3, B, L, status, trace, s);
-        case 12: return launch_resblock<Up2Rb2>(x, y, packed, 2, B, L, status, trace, s);
-        case 13: return launch_resblock<Up3Rb3>(x, y, packed, 3, B, L, status, trace, s);
-        case 14: return launch_resblock<Up3Rb3Post>(x, y, packed, 3, B, L, status, trace, s);
-        case 20: return launch_resblock<Rb0Up1>(x, y, packed, 0, B, L, status, trace, s);
-        case 21: return launch_resblock<Rb1Up2>(x, y, packed, 1, B, L, status, trace, s);
-        case 22: return launch_resblock<Rb2Up3>(x, y, packed, 2, B, L, status, trace, s);
+        case 0: return launch_resblock<Rb0>(x, y, packed, 0, batch, status, trace, s);
+        case 1: return launch_resblock<Rb1>(x, y, packed, 1, batch, status, trace, s);
+        case 2: return launch_resblock<Rb2>(x, y, packed, 2, batch, status, trace, s);
+        case 3: return launch_resblock<Rb3>(x, y, packed, 3, batch, status, trace, s);
+        case 4: return launch_resblock<Rb3Post>(x, y, packed, 3, batch, status, trace, s);
+        case 12: return launch_resblock<Up2Rb2>(x, y, packed, 2, batch, status, trace, s);
+        case 13: return launch_resblock<Up3Rb3>(x, y, packed, 3, batch, status, trace, s);
+        case 14: return launch_resblock<Up3Rb3Post>(x, y, packed, 3, batch, status, trace, s);
+        case 20: return launch_resblock<Rb0Up1>(x, y, packed, 0, batch, status, trace, s);
+        case 21: return launch_resblock<Rb1Up2>(x, y, packed, 1, batch, status, trace, s);
+        case 22: return launch_resblock<Rb2Up3>(x, y, packed, 2, batch, status, trace, s);
     }
     return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: stage %d", stage);
 }

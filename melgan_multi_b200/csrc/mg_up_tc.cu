@@ -13,9 +13,10 @@
 // the same thread's accumulator registers, the epilogue stores the S consecutive output samples [S*s - pad, S*s - pad + S)
 // of a channel as contiguous vectors.
 //
-// Rows are VIRTUAL input positions: the B batch items are concatenated with one zero row after each item
-// (v = item*(Lin+1) + s, s in [0, Lin], row s = Lin is zero), so that x[-1] = x[Lin] = 0 falls out of the layout and short
-// sequences (stage 0: Lin = 32) still fill 64-row blocks.
+// Rows are VIRTUAL input positions: the batch items are concatenated with one zero row after each item (item i's rows
+// s in [0, Lin_i], row s = Lin_i is zero; RunTable maps a row to its item), so that x[-1] = x[Lin_i] = 0 falls out of the
+// layout, short sequences (stage 0: Lin = 32) still fill 64-row blocks, and no row lies past an item's end in a ragged
+// batch.  In memory every item keeps the padded layout: items `stride` input positions apart.
 // One CTA = NMW blocks of 64 virtual input positions x one group of NG output channels.  K (= Cin) is streamed: the A
 // slots (KCA channels: LeakyReLU + hi/lo split of x) are produced in shared memory by the converter warps straight from
 // the fp32 NCL input (all KCA loads of a row in flight at once), the B slots (16 channels: both taps, hi and lo, all
@@ -55,19 +56,23 @@ struct UpCfg {
 };
 
 // D[s, phi*NG + co] + bias -> out[co][S*s + phi - pad] for the two accumulator rows of this thread (block-local rows
-// 64 mw + frag_row(t, h)); r0: first virtual row of the tile
-template <class Cfg>
-__device__ __forceinline__ void convt_store(const float *acc, float *__restrict__ y, const float *__restrict__ bias, int r0, int t,
-                                            int cg, int Lin, int B) {
+// m = 64 mw + frag_row(t, h)); row(m): the row's RunPos; Lout: output positions between items
+template <class Cfg, class Row>
+__device__ __forceinline__ void convt_store(const float *acc, float *__restrict__ y, const float *__restrict__ bias, int mw, int t,
+                                            int cg, int Lout, Row row) {
     constexpr int S = Cfg::S, NG = Cfg::NG, N = Cfg::N, COUT = Cfg::COUT, PAD = Cfg::PAD;
-    const int Lout = Lin * S, Lv = Lin + 1, q = t & 3;
+    const int q = t & 3;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const int v = r0 + frag_row(t, h);
-        const int item = v / Lv, s = v - item * Lv;
-        const bool row_ok = item < B;
-        const bool lo_ok = row_ok && s >= 1, hi_ok = row_ok && s <= Lin - 1;
-        float *yb = y + ((size_t)(row_ok ? item : 0) * COUT + cg * NG) * Lout + (S * s - PAD);
+        // one row's lookup at a time, after the previous row's stores: overlapped, the lookups would be live next to the
+        // whole accumulator
+        int m = 64 * mw + frag_row(t, h);
+        asm volatile("" : "+r"(m) : : "memory");
+        const RunPos p = row(m);
+        const int s = p.unit;
+        const bool row_ok = p.item >= 0;
+        const bool lo_ok = row_ok && s >= 1, hi_ok = row_ok && s <= p.len - 1;
+        float *yb = y + ((size_t)(row_ok ? p.item : 0) * COUT + cg * NG) * Lout + (S * s - PAD);
         if constexpr (S == 8) {
             // column 8k + 2q + e = phi * 32 + co: block k holds phase k / 4 of channels 8 (k % 4) + 2q + e
 #pragma unroll
@@ -101,8 +106,8 @@ __device__ __forceinline__ void convt_store(const float *acc, float *__restrict_
 
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NT, 1)
-convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed, int Lin, int B,
-                int *__restrict__ status) {
+convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed,
+                const __grid_constant__ RunTable rows, int *__restrict__ status) {
     constexpr int CIN = Cfg::CIN, N = Cfg::N, NG = Cfg::NG;
     constexpr int ROWS = Cfg::ROWS, APITCH = Cfg::APITCH, ASLOT = Cfg::ASLOT, BSLOT = Cfg::BSLOT, KCA = Cfg::KCA;
     constexpr int NSA = Cfg::NSA, NSB = Cfg::NSB, NCHUNK = Cfg::NCHUNK, NCONV = Cfg::NCONV, NMW = Cfg::NMW;
@@ -114,7 +119,7 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * ROWS;  // first virtual row of the tile
     const int cg = blockIdx.y;
-    const int Lv = Lin + 1;
+    const int Lin = rows.stride;  // input positions between items
 
     if (tid == 0) {
         for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NMW); }
@@ -182,7 +187,8 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
         if (!ok && t == 0) atomicExch(status, 13);
         pdl_trigger();  // MMAs done, only the output store is left: the next kernel of the chain may be scheduled
         pdl_wait();
-        convt_store<Cfg>(acc, y, packed + bias_offset(1 + Cfg::STAGE) + cg * NG, r0 + 64 * mw, t, cg, Lin, B);
+        convt_store<Cfg>(acc, y, packed + bias_offset(1 + Cfg::STAGE) + cg * NG, mw, t, cg, Cfg::S * Lin,
+                         [&](int m) { return rows.find(r0 + m); });
     } else {
         // ================= converter warps: A slots = split(lrelu(x)), KCA channels of every row =================
         pdl_wait();  // x: the previous kernel's output
@@ -194,10 +200,9 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
             uint8_t *slot = aring + sa * ASLOT;
 #pragma unroll 1
             for (int i = tid; i <= ROWS; i += NCONV) {
-                const int v = r0 - 1 + i;
-                const int item = v >= 0 ? v / Lv : 0, s = v - item * Lv;
-                const bool inr = (v >= 0 && item < B && s < Lin);
-                const float *xp = x + ((size_t)(inr ? item : 0) * CIN + ca * KCA) * Lin + (inr ? s : 0);
+                const RunPos p = rows.find(r0 - 1 + i);
+                const bool inr = p.item >= 0 && p.unit < p.len;
+                const float *xp = x + ((size_t)(inr ? p.item : 0) * CIN + ca * KCA) * Lin + (inr ? p.unit : 0);
                 float f[KCA];
 #pragma unroll
                 for (int j = 0; j < KCA; ++j) f[j] = inr ? __ldg(xp + (size_t)j * Lin) : 0.f;  // all in flight together
@@ -217,41 +222,51 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
     }
 }
 
+// Lin + 1 virtual rows per item: position s = Lin feeds the last `pad` outputs
+static RunTable convt_rows(const RunTable &batch) {
+    RunTable rows = batch;
+    rows.set_units([](int Lin) { return Lin + 1; });
+    return rows;
+}
+
 template <class Cfg>
-static int launch_convt(const float *x, float *y, const float *packed, int B, int Lin, int *status, cudaStream_t s) {
+static int launch_convt(const float *x, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s) {
     static bool configured = false;
     if (!configured) {
         MG_CUDA_TRY(cudaFuncSetAttribute(convt_tc_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         configured = true;
     }
-    const long long vrows = (long long)B * (Lin + 1);  // Lin + 1 rows per item: position s = Lin feeds the last `pad` outputs
-    dim3 grid((unsigned)((vrows + Cfg::ROWS - 1) / Cfg::ROWS), Cfg::NCG);
-    MG_CUDA_TRY(launch_ex(convt_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, 1, x, y, packed, Lin, B, status));
+    const RunTable rows = convt_rows(batch);
+    dim3 grid((unsigned)((rows.first[rows.n] + Cfg::ROWS - 1) / Cfg::ROWS), Cfg::NCG);
+    MG_CUDA_TRY(launch_ex(convt_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, 1, x, y, packed, rows, status));
     return MG_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Variant for a stage whose whole activation tile fits in shared memory (stage 1: 65 rows x 256 channels, hi+lo =
 // 72 KB): the A operand is converted ONCE per row tile and stays resident, and the CTA loops over the NCG output-channel
-// groups, so no activation is loaded or converted twice.  One MMA warpgroup (64 rows, N = 256) per CTA.
+// groups, so no activation is loaded or converted twice.  One MMA warpgroup (64 rows, N = 256) per CTA.  The converter
+// also parks the tile's 64 row lookups in shared memory for the epilogue, which runs once per channel group.
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NCONV + 128 + 32, 1)
-convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed, int Lin, int B,
-                         int *__restrict__ status) {
+convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed,
+                         const __grid_constant__ RunTable rows, int *__restrict__ status) {
     constexpr int CIN = Cfg::CIN, NG = Cfg::NG, N = Cfg::N, NCG = Cfg::NCG;
     constexpr int ROWS = 64, APITCH = Cfg::APITCH, BSLOT = Cfg::BSLOT, NCHUNK = Cfg::NCHUNK;
     constexpr int KPT = CIN / 8;                    // k-panels of the resident A
     constexpr int AHALF = KPT * APITCH;             // bytes of one of {hi, lo}
     constexpr int NSB = 4, NCONV = Cfg::NCONV;
-    static_assert(Cfg::S == 8 && N == 256 && Cfg::NMW == 1 && 2 * AHALF + NSB * BSLOT + 256 <= 227 * 1024, "resident ConvT shape");
+    static_assert(Cfg::S == 8 && N == 256 && Cfg::NMW == 1 && 2 * AHALF + NSB * BSLOT + 256 + ROWS * 12 <= 227 * 1024,
+                  "resident ConvT shape");
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *abuf = smem, *bring = smem + 2 * AHALF;
     uint64_t *fullA = reinterpret_cast<uint64_t *>(bring + NSB * BSLOT);  // [CIN/64]: a 64-channel slice of A is written
     uint64_t *fullB = fullA + CIN / 64, *emptyB = fullB + NSB;
+    RunPos *srow = reinterpret_cast<RunPos *>(emptyB + NSB);  // [ROWS]: virtual row r0 + m, written with A's first slice
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * ROWS;
-    const int Lv = Lin + 1;
+    const int Lin = rows.stride;  // input positions between items
 
     if (tid == 0) {
         for (int s = 0; s < CIN / 64; ++s) mbar_init(&fullA[s], NCONV);
@@ -310,7 +325,8 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
             if (t == 0) { mbar_arrive(&emptyB[psb]); psb = -1; }
             if (cg == NCG - 1) pdl_trigger();  // last channel group's MMAs done: the next kernel may be scheduled
             if (cg == 0) pdl_wait();
-            convt_store<Cfg>(acc, y, packed + bias_offset(1 + Cfg::STAGE) + cg * NG, r0, t, cg, Lin, B);
+            convt_store<Cfg>(acc, y, packed + bias_offset(1 + Cfg::STAGE) + cg * NG, 0, t, cg, Cfg::S * Lin,
+                             [&](int m) { return ok ? srow[m] : RunPos{-1, 0, 0}; });  // (after fullA[0]: srow is complete)
         }
         if (!ok && t == 0) atomicExch(status, 33);
     } else {
@@ -320,10 +336,10 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
         for (int ca = 0; ca < CIN / 64; ++ca) {
 #pragma unroll 1
             for (int i = tid; i <= ROWS; i += NCONV) {
-                const int v = r0 - 1 + i;
-                const int item = v >= 0 ? v / Lv : 0, s = v - item * Lv;
-                const bool inr = (v >= 0 && item < B && s < Lin);
-                const float *xp = x + ((size_t)(inr ? item : 0) * CIN + ca * 64) * Lin + (inr ? s : 0);
+                const RunPos p = rows.find(r0 - 1 + i);
+                if (ca == 0 && i > 0) srow[i - 1] = p;
+                const bool inr = p.item >= 0 && p.unit < p.len;
+                const float *xp = x + ((size_t)(inr ? p.item : 0) * CIN + ca * 64) * Lin + (inr ? p.unit : 0);
                 float f[64];
 #pragma unroll
                 for (int j = 0; j < 64; ++j) f[j] = inr ? __ldg(xp + (size_t)j * Lin) : 0.f;
@@ -343,26 +359,27 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
 }
 
 template <class Cfg>
-static int launch_convt_resident(const float *x, float *y, const float *packed, int B, int Lin, int *status, cudaStream_t s) {
-    constexpr int smem = 2 * (Cfg::CIN / 8) * Cfg::APITCH + 4 * Cfg::BSLOT + (Cfg::CIN / 64 + 2 * 4) * 8;
+static int launch_convt_resident(const float *x, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s) {
+    constexpr int smem = 2 * (Cfg::CIN / 8) * Cfg::APITCH + 4 * Cfg::BSLOT + (Cfg::CIN / 64 + 2 * 4) * 8 + 64 * sizeof(RunPos);
     static bool configured = false;
     if (!configured) {
         MG_CUDA_TRY(cudaFuncSetAttribute(convt_resident_tc_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         configured = true;
     }
-    const long long vrows = (long long)B * (Lin + 1);
-    MG_CUDA_TRY(launch_ex(convt_resident_tc_kernel<Cfg>, dim3((unsigned)((vrows + 63) / 64)), dim3(Cfg::NCONV + 128 + 32), smem, s,
-                          true, 1, x, y, packed, Lin, B, status));
+    const RunTable rows = convt_rows(batch);
+    MG_CUDA_TRY(launch_ex(convt_resident_tc_kernel<Cfg>, dim3((unsigned)((rows.first[rows.n] + 63) / 64)), dim3(Cfg::NCONV + 128 + 32),
+                          smem, s, true, 1, x, y, packed, rows, status));
     return MG_OK;
 }
 
-// x [B][Cin][Lin] -> y [B][Cout][S*Lin], fp32 NCL, (Cin, Cout, S) of generator stage `stage`.
-int launch_convt_tc(const float *x, float *y, const float *packed, int stage, int B, int Lin, int *status, cudaStream_t s) {
+// x [B][Cin][Lin] -> y [B][Cout][S*Lin], fp32 NCL, (Cin, Cout, S) of generator stage `stage`; Lin = batch.stride, item i's
+// first len_i input positions (and S len_i output positions) are its own.
+int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s) {
     switch (stage) {
-        case 0: return launch_convt<UpCfg<0>>(x, y, packed, B, Lin, status, s);
-        case 1: return launch_convt_resident<UpCfg<1>>(x, y, packed, B, Lin, status, s);
-        case 2: return launch_convt<UpCfg<2>>(x, y, packed, B, Lin, status, s);
-        case 3: return launch_convt<UpCfg<3>>(x, y, packed, B, Lin, status, s);
+        case 0: return launch_convt<UpCfg<0>>(x, y, packed, batch, status, s);
+        case 1: return launch_convt_resident<UpCfg<1>>(x, y, packed, batch, status, s);
+        case 2: return launch_convt<UpCfg<2>>(x, y, packed, batch, status, s);
+        case 3: return launch_convt<UpCfg<3>>(x, y, packed, batch, status, s);
     }
     return set_error(MG_ERR_INVALID_ARGUMENT, "launch_convt_tc: stage %d", stage);
 }

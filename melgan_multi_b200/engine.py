@@ -42,6 +42,9 @@ def lib():
         L.mg_gen_forward.restype = ctypes.c_int
         L.mg_gen_forward.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                      ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+        L.mg_gen_forward_ragged.restype = ctypes.c_int
+        L.mg_gen_forward_ragged.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
         L.mg_gen_forward_timed.restype = ctypes.c_int
         L.mg_gen_forward_timed.argtypes = L.mg_gen_forward.argtypes + [ctypes.POINTER(ctypes.c_float)]
         L.mg_gen_check_status.restype = ctypes.c_int
@@ -135,6 +138,9 @@ def lib():
         L.mg_gen_engine_forward.restype = ctypes.c_int
         L.mg_gen_engine_forward.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                             ctypes.c_int]
+        L.mg_gen_engine_forward_ragged.restype = ctypes.c_int
+        L.mg_gen_engine_forward_ragged.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                                   ctypes.c_void_p]
         L.mg_gen_engine_last_kernel_ms.restype = ctypes.c_int
         L.mg_gen_engine_last_kernel_ms.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float)]
         L.mg_gen_engine_destroy.restype = None
@@ -150,6 +156,24 @@ def check(rc):
 
 def _ptr_array(ptrs):
     return (ctypes.c_void_p * len(ptrs))(*ptrs)
+
+
+def _lengths(lengths, B, T_max):
+    """Per-item mel lengths of a ragged batch as a C int array: a list, a tuple or a CPU integer tensor of B values in
+    [1, T_max].  A CUDA tensor is refused: reading it would synchronise the stream."""
+    if hasattr(lengths, "device") and hasattr(lengths, "is_floating_point"):
+        if lengths.device.type != "cpu":
+            raise EngineError("lengths must be a list, a tuple or a CPU tensor (reading a CUDA tensor would synchronise)")
+        if lengths.is_floating_point() or lengths.dim() != 1:
+            raise EngineError("lengths must be a 1-D integer tensor")
+        lengths = lengths.tolist()
+    lengths = [int(v) for v in lengths]
+    if len(lengths) != B:
+        raise EngineError("lengths has %d entries for a batch of %d" % (len(lengths), B))
+    bad = [v for v in lengths if not 1 <= v <= T_max]
+    if bad:
+        raise EngineError("lengths must lie in [1, T_max = %d] (got %d)" % (T_max, bad[0]))
+    return (ctypes.c_int * B)(*lengths)
 
 
 class _StatusWatch:
@@ -264,6 +288,30 @@ class GeneratorDevice:
             check(lib().mg_gen_forward(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T,
                                        ws.data_ptr(), ws.numel() * 4, stream))
             off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4  # the status word sits after the activation buffers
+            self._watch.arm(ws.view(torch.int32)[off:off + 1])
+        return out
+
+    def forward_ragged(self, mel, lengths, out=None):
+        """Ragged batch (inference): mel [B, 80, T_max] with item i's frames [0, lengths[i]) valid (the rest is never read)
+        -> audio [B, 1, 256 T_max]; item i's first 256 lengths[i] samples equal its own forward bit for bit, the rest are 0.
+        lengths: a list, a tuple or a CPU integer tensor.  Asynchronous, like forward."""
+        torch = self.torch
+        if mel.dim() != 3 or mel.shape[1] != 80:
+            raise EngineError("mel must be [B, 80, T_max], got %s" % (tuple(mel.shape),))
+        if mel.device != self.device or mel.dtype != torch.float32:
+            raise EngineError("mel must be an fp32 tensor on %s" % (self.device,))
+        mel = mel.contiguous()
+        B, _, T = mel.shape
+        lens = _lengths(lengths, B, T)
+        if out is None:
+            out = torch.empty((B, 1, 256 * T), dtype=torch.float32, device=self.device)
+        self._watch.check()
+        ws = self.workspace(B, T)
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream().cuda_stream
+            check(lib().mg_gen_forward_ragged(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens,
+                                              ws.data_ptr(), ws.numel() * 4, stream))
+            off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4
             self._watch.arm(ws.view(torch.int32)[off:off + 1])
         return out
 
@@ -688,6 +736,19 @@ class GeneratorHost:
         if out is None:
             out = np.empty((B, 1, 256 * T), np.float32)
         check(lib().mg_gen_engine_forward(self._h, mel.ctypes.data, out.ctypes.data, B, T))
+        return out
+
+    def forward_ragged(self, mel, lengths, out=None):
+        """Ragged batch from host memory (mg_gen_engine_forward_ragged): mel [B, 80, T_max], lengths as for
+        GeneratorDevice.forward_ragged -> audio [B, 1, 256 T_max]."""
+        mel = np.ascontiguousarray(mel, dtype=np.float32)
+        if mel.ndim != 3 or mel.shape[1] != 80:
+            raise EngineError("mel must be [B, 80, T_max]")
+        B, _, T = mel.shape
+        lens = _lengths(lengths, B, T)
+        if out is None:
+            out = np.empty((B, 1, 256 * T), np.float32)
+        check(lib().mg_gen_engine_forward_ragged(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens))
         return out
 
     def forward_ptr(self, mel_ptr, out_ptr, B, T):

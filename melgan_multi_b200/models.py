@@ -140,6 +140,16 @@ class Generator(nn.Module):
     def _engine_forward(self, mel):
         return self._ensure_packed().forward(mel)
 
+    def generate(self, x, lengths):
+        """Vocodes a batch of utterances of different lengths in one forward (inference only: no autograd graph is built).
+        x [B, 80, T_max] fp32 CUDA, lengths: B mel lengths in [1, T_max] as a list, a tuple or a CPU integer tensor; the
+        frames past each length are never read.  Returns audio [B, 1, 256 T_max] whose item i starts with exactly the
+        256 lengths[i] samples of self(x[i:i+1, :, :lengths[i]]) and is 0 after them."""
+        if not x.is_cuda:
+            raise _engine.EngineError("melgan_multi_b200.Generator.generate needs a CUDA tensor (no CPU fallback)")
+        with torch.no_grad():
+            return self._ensure_packed().forward_ragged(x.detach().float(), lengths)
+
     def _graphed_recompute(self, mel, params):
         """(graphed stock-op forward+backward, mel_requires_grad) for this input shape, or None.  Cached per shape / dtype
         policy; the graphs own static copies of nothing but activations -- parameters are call arguments."""

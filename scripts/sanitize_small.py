@@ -1,4 +1,4 @@
-"""Tiny generator + discriminator forwards, a sliced generator forward, one training step (fused losses, native
+"""Tiny generator + discriminator forwards, a sliced generator forward, a ragged batch, one training step (fused losses, native
 discriminator backward, multi-tensor Adam) for compute-sanitizer (memcheck / racecheck / synccheck)."""
 import os
 import sys
@@ -33,6 +33,12 @@ with torch.no_grad():
     y4 = g(torch.from_numpy(synth.mel_input(1, 5, 10)).cuda())
     g._dev.check_status(1, 5)
     engine.check(engine.lib().mg_gen_set_pipeline(-1))
+    # a ragged batch of three items (NaN past each length), cut into two slices when MG_GEN_SLICES=2
+    mr = torch.from_numpy(synth.mel_input(3, 40, 11)).cuda()
+    mr[0, :, 5:] = float("nan")
+    mr[2, :, 17:] = float("nan")
+    yr = g.generate(mr, [5, 40, 17])
+    g._dev.check_status(3, 40)
     m = meldataset.mel_spectrogram(y3[0, 0].clamp(-1, 1), 1024, 80, 22050, 256, 1024, 55, 9000)
 # one train.py:108-129 step on a 512-sample segment
 g.train(); d.train()
