@@ -179,11 +179,14 @@ def test_grouped_conv_backward_matches_torch(msd_module, layer, Bt, Lin):
         torch.backends.cudnn.conv.fp32_precision = old
 
 
-@pytest.mark.parametrize("Bt,L", [(32, 32), (32, 16), (32, 8), (3, 17), (2, 20), (5, 7), (1, 3), (2, 130)])
+@pytest.mark.parametrize("Bt,L", [(32, 128), (32, 65), (32, 17), (32, 32), (32, 16), (32, 8), (3, 17), (2, 20), (5, 7), (1, 3),
+                                  (2, 130)])
 def test_conv_post1_gradients_match_fp64(msd_module, Bt, L):
     """csrc/mg_wgrad_tc.cu (dW, db) and the transposed-blob dgrad of conv_post1 (models.py:84,96) against autograd of F.conv1d
-    in float64: the three training lengths (32 / 16 / 8 positions, 2 x 16 items) and ragged ones (L % 4 != 0: scalar loads;
-    L % 8 != 0: padded k-panels; L < 5: every tap touches the zero padding; K extent not a multiple of 32)."""
+    in float64: the lengths conv_post1 sees at config 3 (32 stacked items of 8192 samples: 128 / 65 / 17 positions at
+    scales 0 / 1 / 2; at 65 every item's last k-panel is padded and items meet inside a stage), other 32-item lengths, and
+    ragged ones (L % 4 != 0: scalar loads; L % 8 != 0: padded k-panels; L < 5: every tap touches the zero padding; K extent
+    not a multiple of 32)."""
     import torch.nn.functional as F
     with torch.no_grad():
         msd_module(torch.zeros(1, 1, 64).cuda(), torch.zeros(1, 1, 64).cuda())  # makes sure the weights are packed
