@@ -124,6 +124,11 @@ int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, i
  * front, 20 / 21 / 22 next ConvT fused at the tail), "resblock_tc_kernel<RbCfg<C,NRB,RPW,NCP,NSTAGE,POST,UPF,UPT,CS>>";
  * "" for an unknown code.  Tests derive the tile and cluster borders from it. */
 const char *mg_gen_resblock_config(int code);
+/* Tile geometry of the streaming ConvT kernel of stage 2 or 3, "convt_stream_tc_kernel<StreamCfg<STAGE,ROWS,MAXSEG,NSX>>":
+ * ROWS input positions per tile (the batch's items concatenated with one zero row after each), at most MAXSEG item
+ * segments of a tile staged by bulk copy, NSX staging slots; persistent grid of min(tiles, SMs) CTAs.  "" for stages
+ * 0 and 1.  Tests derive tile borders from it. */
+const char *mg_gen_convt_config(int stage);
 
 /* ResBlock `stage` (0..2) with the NEXT stage's LeakyReLU -> ConvTranspose1d fused at its tail, as the default pipeline runs it
  * (models.py:66 followed by :64-65 of the next loop iteration): x [B][C][L] is stage `stage`'s ConvT output, y
@@ -138,7 +143,8 @@ int mg_gen_conv_pre(const void *packed, const float *mel, float *y, int B, int T
 int mg_gen_resblock_post(const void *packed, const float *x, float *audio, int B, int L, void *stream);
 
 /* Diagnostic twin of mg_gen_resblock: also returns 128 clock64 stamps (host buffer) of one interior CTA's
- * hand-off and MMA phases (slot meaning documented at the definition in csrc/mg_api.cu). */
+ * hand-off and MMA phases (slot meaning documented at the definition in csrc/mg_api.cu).  `stage` is any stage code of
+ * mg_gen_resblock_config, with that kernel's shapes: L is the ResBlock's own length (codes 12..14: x [B][2C][L/2]). */
 int mg_gen_resblock_trace(const void *packed, int stage, const float *x, float *y, int B, int L, long long *trace_host);
 
 /* Debug/parity tap: copies the activation after stage `which` (0 = conv_pre output [B,512,T],

@@ -309,13 +309,15 @@ int mg_gen_resblock_post(const void *packed, const float *x, float *audio, int B
 }
 
 /* Diagnostic: runs one tensor-core ResBlock and returns clock64 stamps of thread 0 of one interior CTA in trace[0..127]
- * (host buffer): [0] start, [1] input loaded, per conv c: [2+3c] X handed to the MMAs, [3+3c] accumulator ready,
+ * (host buffer) for any stage code of resblock_config_name: [0] start, [1] input loaded, per conv c: [2+3c] X handed to the
+ * MMAs (the interval from [1+3c] holds only shared-memory work: the conv biases are staged before griddepcontrol.wait),
+ * [3+3c] accumulator ready,
  * [4+3c] next X written, [20] output stored; the same thread's MMA issue: [64+3c] X received, [65+3c] first weights
  * landed, [66+3c] last MMA issued.  Clustered stages (0, 1): [88+2c] / [89+2c] before / after the wait for the cluster
  * neighbours' border rows of conv c's input, [100+2k] / [101+2k] before / after the wait until the neighbours' MMAs of
  * conv k-1 have released their slack rows (hand-off k = 1..5), and [127] = cudaOccupancyMaxActiveClusters of the launch. */
 int mg_gen_resblock_trace(const void *packed, int stage, const float *x, float *y, int B, int L, long long *trace_host) {
-    if (!packed || !x || !y || x == y || !trace_host || stage < 0 || stage > 3)
+    if (!packed || !x || !y || x == y || !trace_host || !*resblock_config_name(stage, 0) || B < 1 || L < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_resblock_trace: bad argument");
     int *st = nullptr;
     long long *tr = nullptr;
@@ -364,6 +366,7 @@ int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, i
 }
 
 const char *mg_gen_resblock_config(int code) { return resblock_config_name(code, 0); }
+const char *mg_gen_convt_config(int stage) { return convt_config_name(stage); }
 
 /* ------------------------------- multi-scale discriminator ------------------------------- */
 

@@ -89,7 +89,13 @@ struct RbCfg {
     static constexpr int PVB = CS * P - HALO - HL, XCH = 9;
     static_assert(CS == 1 || ((CS == 2 || CS == 4) && !POST_ && !UPF_ && UPT_ == 0 && XCH <= SLACK && 2 * XCH <= P),
                   "clusters are for the plain ResBlock");
-    static constexpr int SMEM_BYTES = 2 * XBYTES + NSTAGE * CHUNK + 2 * C * 4 + (2 * NSTAGE + (CS > 1 ? 2 : 0) + 1) * 8;
+    // per-CTA constants, copied into shared memory before griddepcontrol.wait: the six conv biases [conv][C] (c1[0..2],
+    // c2[0..2]: layers l0 .. l0 + 5), then the front ConvT's bias (C), the tail ConvT's bias (C / 2), conv_post's weights
+    // [ci][8] and bias
+    static constexpr int CB_UPF = 6 * C, CB_UPT = CB_UPF + (UPF_ ? C : 0), CB_POST = CB_UPT + (UPT_ ? C / 2 : 0);
+    static constexpr int NCONST = CB_POST + (POST_ ? 32 * 8 + 4 : 0);
+    static_assert(CB_POST % 4 == 0 && NCONST % 2 == 0, "conv_post weights are read as float4, the mbarriers follow");
+    static constexpr int SMEM_BYTES = 2 * XBYTES + NSTAGE * CHUNK + (2 * C + NCONST) * 4 + (2 * NSTAGE + (CS > 1 ? 2 : 0) + 1) * 8;
     static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "shared memory budget");
     static_assert(XPITCH / 16 < 16384, "LBO field");
     static_assert(NRB % RPW == 0 && C % NCP == 0 && NCW % 32 == 0, "warpgroup split");
@@ -112,8 +118,9 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *Xh = smem, *Xl = smem + XBYTES, *ring = smem + 2 * XBYTES;
     float *pend = reinterpret_cast<float *>(ring + NSTAGE * CHUNK);  // sum of the c2 biases folded so far
-    float *b1s = pend + C;                                            // bias of the c1 in flight
-    uint64_t *full = reinterpret_cast<uint64_t *>(b1s + C);
+    float *b1s = pend + C;                                            // (tail ConvT: lrelu(x[L-1]) for its fix-up)
+    float *cst = b1s + C;                                             // [NCONST]: the per-CTA constants (RbCfg)
+    uint64_t *full = reinterpret_cast<uint64_t *>(cst + Cfg::NCONST);
     uint64_t *empty = full + NSTAGE;
     // clusters: hfull completes once every cluster neighbour's border rows have landed in this CTA's slack rows (one phase
     // per X hand-off), hfree once every neighbour's MMAs have finished reading its X (one phase per conv): then the copies
@@ -165,6 +172,21 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         *reinterpret_cast<uint4 *>((hl ? Xl : Xh) + kp * XPITCH + row * 16) = make_uint4(0, 0, 0, 0);
     }
     for (int i = tid; i < C; i += Cfg::NT) pend[i] = 0.f;
+    // the constants come from the packed blob, not from the previous kernel: read before pdl_wait(), like the weight stream,
+    // so that no global load sits between a hand-off and the next conv
+    for (int i = tid; i < Cfg::NCONST; i += Cfg::NT) {
+        float v = 0.f;
+        if (i < Cfg::CB_UPF) v = __ldg(packed + bias_offset(l0) + i);  // layers l0 .. l0 + 5 have C biases each
+        else if (i < Cfg::CB_UPT) v = __ldg(packed + bias_offset(1 + stage) + (i - Cfg::CB_UPF));
+        else if (i < Cfg::CB_POST) v = __ldg(packed + bias_offset(1 + stage + 1) + (i - Cfg::CB_UPT));
+        else if (i < Cfg::CB_POST + 32 * 8) {
+            const int j = i - Cfg::CB_POST;
+            if ((j & 7) < kPostK) v = __ldg(packed + weight_offset(29) + (j >> 3) * kPostK + (j & 7));
+        } else if (i == Cfg::CB_POST + 32 * 8) {
+            v = __ldg(packed + bias_offset(29));
+        }
+        cst[i] = v;
+    }
     fence_proxy_async();
     __syncthreads();
     if constexpr (CS > 1) cluster_sync();  // every CTA's barriers are initialised before any remote access
@@ -405,7 +427,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         drain();
         sync_cons();  // every ConvT MMA has read the operand: the region becomes the fp32 staging buffer [c][p]
         float *stg = reinterpret_cast<float *>(Xh);
-        const float *ubias = packed + bias_offset(1 + stage);
+        const float *ubias = cst + Cfg::CB_UPF;
         if (mine) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -414,7 +436,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                 for (int j = 0; j < NA; ++j) {
                     const int col = frag_col(q, (j & ~3) | (j & 1));
                     if ((j & 2) == 2 * h) {
-                        const float bj = __ldg(ubias + col);
+                        const float bj = ubias[col];
                         *reinterpret_cast<float2 *>(stg + (size_t)col * SPITCH + 2 * m) = make_float2(R[0][j] + bj, D[0][j] + bj);
                     }
                 }
@@ -458,17 +480,14 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
 #pragma unroll 1
     for (int pr = 0; pr < 3; ++pr) {
         // ---- c1 (dilation 1, 3, 9) into D, then X <- split(lrelu(D + b1))
-        const float *bias1 = packed + bias_offset(l0 + pr);
-        for (int c = tid; c < C; c += NCONS) b1s[c] = __ldg(bias1 + c);
         MG_TR(2 + 6 * pr);
         conv_mma(D, pr == 0 ? 1 : pr == 1 ? 3 : 9, true, 2 * pr);
         MG_TR(3 + 6 * pr);
-        x_read();  // (and b1s is complete)
-        hand_off(D, b1s, false);
+        x_read();
+        hand_off(D, cst + pr * C, false);
         MG_TR(4 + 6 * pr);
         // ---- c2 (dilation 1) accumulating onto R, then X <- split(lrelu(R + pend)) for the next c1 (or the tail ConvT)
-        const float *bias2 = packed + bias_offset(l0 + 3 + pr);
-        for (int c = tid; c < C; c += NCONS) pend[c] += __ldg(bias2 + c);
+        for (int c = tid; c < C; c += NCONS) pend[c] += cst[(3 + pr) * C + c];
         MG_TR(5 + 6 * pr);
         conv_mma(R, 1, false, 2 * pr + 1);
         MG_TR(6 + 6 * pr);
@@ -484,10 +503,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         // now), then audio[p] = tanh(b + sum_k q_k[p + k - 3]).
         pdl_trigger();
         float *Q = reinterpret_cast<float *>(Xh);      // [7][P]
-        float *wpost = reinterpret_cast<float *>(Xl);  // [32][8]
-        for (int i = tid; i < 32 * 8; i += NCONS)
-            wpost[i] = (i & 7) < kPostK ? __ldg(packed + weight_offset(29) + (i >> 3) * kPostK + (i & 7)) : 0.f;
-        sync_cons();
+        const float *wpost = cst + Cfg::CB_POST;        // [32][8]
 #pragma unroll
         for (int r = 0; r < RPW; ++r)
 #pragma unroll
@@ -521,7 +537,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
             }
         sync_cons();
         const int b = item(), L = len();
-        const float bpost = __ldg(packed + bias_offset(29));
+        const float bpost = cst[Cfg::CB_POST + 32 * 8];
 #pragma unroll 1
         for (int p = tid; p < P; p += NCONS) {
             const int tp = o + p;
@@ -542,7 +558,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         constexpr int S = Cfg::UPT, TNG = Cfg::TNG, TN = Cfg::TN, PADT = S / 2, COT = C / 2;
         const int b = item(), L = len();
         const int Lout = S * Ls;  // output positions between items
-        const float *tbias = packed + bias_offset(1 + stage + 1);
+        const float *tbias = cst + Cfg::CB_UPT;
         // ---- fix-up first (it only needs b1s[]): out[co][S L - pad + j] = bias + sum_ci lrelu(x[ci][L-1]) * W[ci][co][j + S],
         // j < pad (the outputs position L would own: x[L] = 0 leaves only the x[L-1] tap), by the CTA whose owned rows include
         // position L - 1.  fp32 FFMA on the fp32 copy of the ConvT weights ([Cin][Cout][S][2], mg_layout.h).
@@ -567,7 +583,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                             acc3 = fmaf(b1s[cc + k + 3], wv[k + 3], acc3);
                         }
                     }
-                    y[((size_t)b * COT + co) * Lout + (size_t)S * L - PADT + j] = (acc0 + acc1) + (acc2 + acc3) + __ldg(tbias + co);
+                    y[((size_t)b * COT + co) * Lout + (size_t)S * L - PADT + j] = (acc0 + acc1) + (acc2 + acc3) + tbias[co];
                 }
             }
         }
@@ -615,7 +631,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int co = 8 * c + 2 * q + e;
-                                const float bj = __ldg(tbias + cg * TNG + co);
+                                const float bj = tbias[cg * TNG + co];
                                 if (ok8)
                                     *reinterpret_cast<float4 *>(yb + (size_t)co * Lout) =
                                         make_float4(D[r][4 * c + 2 * h + e] + bj, D[r][4 * (4 + c) + 2 * h + e] + bj,
@@ -628,7 +644,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int col = c0 + frag_col(q, 4 * k + e), phi = col / TNG, co = col % TNG;
-                                if (phi == 0 ? lo_ok : hi_ok) yb[(size_t)co * Lout + phi] = D[r][4 * k + 2 * h + e] + __ldg(tbias + co);
+                                if (phi == 0 ? lo_ok : hi_ok) yb[(size_t)co * Lout + phi] = D[r][4 * k + 2 * h + e] + tbias[co];
                             }
                     }
                 }

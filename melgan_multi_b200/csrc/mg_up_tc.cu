@@ -24,6 +24,11 @@
 // Warp roles: converter warpgroup, NMW MMA warpgroups (one per 64-row block; accumulators in registers, they also run
 // the epilogue), TMA producer warp.  An N = 256 tile is 128 accumulator registers per thread, so the stride-8 stages run
 // one MMA warpgroup per CTA.
+//
+// The stride-2 stages (2, 3) move 4 bytes of input and 4 of output per 8 multiply-adds (x 3 passes): they are bound by
+// memory, not by the tensor cores, so they run as a streaming kernel of their own (convt_stream_tc_kernel below): persistent
+// CTAs, the weights resident in shared memory, each tile's input brought in by bulk copies several slots ahead of the
+// converter, and an epilogue that stores pairs of neighbouring output samples.
 #include "mg_common.cuh"
 #include "mg_tc.cuh"
 
@@ -45,7 +50,7 @@ struct UpCfg {
     static constexpr int APITCH = AROWS * 16;             // bytes between k-panels
     static constexpr int ASLOT = 2 * (KCA / 8) * APITCH;  // [half: hi, lo][k-panel][AROWS][16 B]
     static constexpr int BSLOT = up_slot_bytes(STAGE);    // [tap][half][k-panel: 2][N][16 B]
-    static constexpr int NSA = (CIN == KCA) ? 1 : 2, NSB = (S == 8) ? 4 : (CIN >= 128 ? 2 : 3);
+    static constexpr int NSA = (CIN == KCA) ? 1 : 2, NSB = 4;  // (convt_tc_kernel: stride 8)
     static constexpr int NCHUNK = CIN / 16;               // B slots per tile
     static constexpr int NCONV = 128;                     // converter threads
     static constexpr int NT = NCONV + 128 * NMW + 32;
@@ -60,7 +65,8 @@ struct UpCfg {
 template <class Cfg, class Row>
 __device__ __forceinline__ void convt_store(const float *acc, float *__restrict__ y, const float *__restrict__ bias, int mw, int t,
                                             int cg, int Lout, Row row) {
-    constexpr int S = Cfg::S, NG = Cfg::NG, N = Cfg::N, COUT = Cfg::COUT, PAD = Cfg::PAD;
+    constexpr int S = Cfg::S, NG = Cfg::NG, COUT = Cfg::COUT, PAD = Cfg::PAD;
+    static_assert(S == 8, "the stride-2 stages store through convt_stream_store");
     const int q = t & 3;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -73,34 +79,23 @@ __device__ __forceinline__ void convt_store(const float *acc, float *__restrict_
         const bool row_ok = p.item >= 0;
         const bool lo_ok = row_ok && s >= 1, hi_ok = row_ok && s <= p.len - 1;
         float *yb = y + ((size_t)(row_ok ? p.item : 0) * COUT + cg * NG) * Lout + (S * s - PAD);
-        if constexpr (S == 8) {
-            // column 8k + 2q + e = phi * 32 + co: block k holds phase k / 4 of channels 8 (k % 4) + 2q + e
+        // column 8k + 2q + e = phi * 32 + co: block k holds phase k / 4 of channels 8 (k % 4) + 2q + e
 #pragma unroll
-            for (int c = 0; c < 4; ++c)
+        for (int c = 0; c < 4; ++c)
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int co = 8 * c + 2 * q + e;
-                    const float bj = __ldg(bias + co);
-                    float *yp = yb + (size_t)co * Lout;
-                    if (lo_ok)
-                        *reinterpret_cast<float4 *>(yp) =
-                            make_float4(acc[4 * (0 + c) + 2 * h + e] + bj, acc[4 * (4 + c) + 2 * h + e] + bj,
-                                        acc[4 * (8 + c) + 2 * h + e] + bj, acc[4 * (12 + c) + 2 * h + e] + bj);
-                    if (hi_ok)
-                        *reinterpret_cast<float4 *>(yp + 4) =
-                            make_float4(acc[4 * (16 + c) + 2 * h + e] + bj, acc[4 * (20 + c) + 2 * h + e] + bj,
-                                        acc[4 * (24 + c) + 2 * h + e] + bj, acc[4 * (28 + c) + 2 * h + e] + bj);
-                }
-        } else {  // S == 2: out[2s - 1] (phase 0) and out[2s] (phase 1)
-#pragma unroll
-            for (int k = 0; k < N / 8; ++k)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int col = frag_col(q, 4 * k + e), phi = col / NG, co = col % NG;
-                    const float o = acc[4 * k + 2 * h + e] + __ldg(bias + co);
-                    if (phi == 0 ? lo_ok : hi_ok) yb[(size_t)co * Lout + phi] = o;
-                }
-        }
+            for (int e = 0; e < 2; ++e) {
+                const int co = 8 * c + 2 * q + e;
+                const float bj = __ldg(bias + co);
+                float *yp = yb + (size_t)co * Lout;
+                if (lo_ok)
+                    *reinterpret_cast<float4 *>(yp) =
+                        make_float4(acc[4 * (0 + c) + 2 * h + e] + bj, acc[4 * (4 + c) + 2 * h + e] + bj,
+                                    acc[4 * (8 + c) + 2 * h + e] + bj, acc[4 * (12 + c) + 2 * h + e] + bj);
+                if (hi_ok)
+                    *reinterpret_cast<float4 *>(yp + 4) =
+                        make_float4(acc[4 * (16 + c) + 2 * h + e] + bj, acc[4 * (20 + c) + 2 * h + e] + bj,
+                                    acc[4 * (24 + c) + 2 * h + e] + bj, acc[4 * (28 + c) + 2 * h + e] + bj);
+            }
     }
 }
 
@@ -243,6 +238,300 @@ static int launch_convt(const float *x, float *y, const float *packed, const Run
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// Streaming kernel of the stride-2 stages.  Per output element it computes exactly what convt_tc_kernel would (the same
+// A and B operands, MMA order, 3 passes and bias add); only the data movement differs:
+//  - persistent CTAs, one per SM (grid = min(tiles, SMs)), walk the row tiles blockIdx.x, + gridDim.x, ...  The layer's
+//    whole B operand (NCHUNK slots: 128 KB at stage 2, one channel group) is loaded once per CTA and stays resident;
+//  - a tile's input arrives by 1-D bulk copies, one per (channel, item segment) of the 16-byte-aligned superset of the
+//    segment, into a ring of NSX fp32 staging slots of KCA channels.  The producer warp (lane c: channel c of the slot)
+//    runs up to NSX slots ahead, across tiles, so the next tile's loads are in flight under this tile's MMAs and stores;
+//  - the converter does LeakyReLU + split from the staging slot into the A ring (rows of items too short to be staged,
+//    past the MAXSEG-th segment of a tile, it reads from global memory);
+//  - the MMA warpgroups add the bias (registers, loaded once) and store, per channel, out[2s] (phase 1 of row s) and
+//    out[2s + 1] (phase 0 of row s + 1, from the lane 4 up by shuffle) as one float2; meanwhile the converter already fills
+//    the A ring with the next tile.
+template <class Cfg>
+struct StreamCfg {
+    static_assert(Cfg::S == 2 && Cfg::NCG == 1 && Cfg::NMW == 2, "streaming ConvT: stride 2, one channel group");
+    static constexpr int MAXSEG = 3;                          // staged item segments per tile: 3 when items have >= 64 positions
+    static constexpr int AR = Cfg::ROWS + 1;                  // A rows of a tile (virtual rows r0 - 1 .. r0 + ROWS - 1)
+    static constexpr int XPITCH = (AR + 6 * MAXSEG + 3) & ~3;  // floats per channel of a staging slot: each segment's
+                                                               // aligned superset is at most 6 floats longer than it
+    static constexpr int XSLOT = Cfg::KCA * XPITCH * 4;
+    static constexpr int BRES = Cfg::NCHUNK * Cfg::BSLOT;     // resident B
+    static constexpr int NSA = 2;
+    static constexpr int FIXED = BRES + NSA * Cfg::ASLOT + 256;  // (+ the mbarriers)
+    static constexpr int NSX = (227 * 1024 - 1024 - FIXED) / XSLOT < 4 ? (227 * 1024 - 1024 - FIXED) / XSLOT : 4;
+    static constexpr int NT = Cfg::NCONV + 128 * Cfg::NMW + 32;
+    static constexpr int SMEM_BYTES = BRES + NSA * Cfg::ASLOT + NSX * XSLOT + (1 + 2 * NSA + 2 * NSX) * 8;
+    static_assert(NSX >= 2 && SMEM_BYTES + 1024 <= 227 * 1024, "shared memory budget");
+    static_assert(XPITCH % 4 == 0 && Cfg::KCA == 32, "staging slot: 16-byte channel rows, one channel per producer lane");
+};
+
+// A rows [i0, i0 + n) of a tile are input positions [u0, u0 + n) of `item`, staged from float dst (+ the channel's
+// alignment offset) of each channel's staging row
+struct XSeg {
+    int i0, n, item, u0, dst;
+};
+// The staged segments of the tile at virtual row r0 (A row i = virtual row r0 - 1 + i); producer and converter both call
+// it.  Rows below `covered` outside every segment are zero rows (row -1, an item's zero row); rows from `covered` on
+// (only with items shorter than 64 positions) are not staged.
+template <class SC>
+__device__ __forceinline__ void tile_segments(const RunTable &rows, int r0, XSeg (&seg)[SC::MAXSEG], int &covered) {
+    int i = r0 == 0 ? 1 : 0, dst = 0;
+#pragma unroll
+    for (int k = 0; k < SC::MAXSEG; ++k) {
+        RunPos p = rows.find(r0 - 1 + i);
+        if (i < SC::AR && p.item >= 0 && p.unit == p.len) p = rows.find(r0 - 1 + ++i);  // skip an item's zero row
+        const int n = (i < SC::AR && p.item >= 0) ? min(p.len - p.unit, SC::AR - i) : 0;
+        seg[k] = {i, n, p.item, p.unit, dst};
+        dst += (n + 6) & ~3;
+        i += n;
+    }
+    covered = i;
+}
+
+// D[s, phi*NG + co] + bias -> out[co][2s - 1 + phi] for the two accumulator rows of this thread (stride 2, pad 1).  Row s
+// with s < len owns the pair out[2s], out[2s + 1] = (its phase 1, row s + 1's phase 0); the last row of each warp (its
+// successor is in the next warp) stores only out[2s], the first row of each warp also its own out[2s - 1].
+template <class Cfg>
+__device__ __forceinline__ void convt_stream_store(const float *acc, const float (&bj)[Cfg::NG / 8][2], float *__restrict__ y, int mw,
+                                                   int t, int r0, const RunTable &rows) {
+    constexpr int KB = Cfg::NG / 8, COUT = Cfg::COUT;
+    const int lane = t & 31, q = t & 3, g = lane >> 2;
+    const int Lout = 2 * rows.stride;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        int m = 64 * mw + frag_row(t, h);
+        asm volatile("" : "+r"(m) : : "memory");  // one row's lookup at a time (see convt_store)
+        const RunPos p = rows.find(r0 + m);
+        const int s = p.unit;
+        const bool pair_ok = p.item >= 0 && s < p.len, lo_ok = p.item >= 0 && s >= 1;
+        float *yb = y + (size_t)(p.item >= 0 ? p.item : 0) * COUT * Lout + 2 * s;
+#pragma unroll
+        for (int k = 0; k < KB; ++k)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int co = 8 * k + 2 * q + e;
+                const float p0 = acc[4 * k + 2 * h + e] + bj[k][e];         // phase 0: out[2s - 1]
+                const float p1 = acc[4 * (KB + k) + 2 * h + e] + bj[k][e];  // phase 1: out[2s]
+                // phase 0 of row m + 1: lane + 4, same h; for h = 0 and g = 7 it is lane - 28's h = 1 row
+                const float nx = h == 0 ? __shfl_sync(0xffffffffu, g == 0 ? acc[4 * k + 2 + e] + bj[k][e] : p0, (lane + 4) & 31)
+                                        : __shfl_down_sync(0xffffffffu, p0, 4);
+                float *yp = yb + (size_t)co * Lout;
+                if (h == 1 && g == 7) {
+                    if (pair_ok) yp[0] = p1;
+                } else if (pair_ok) {
+                    *reinterpret_cast<float2 *>(yp) = make_float2(p1, nx);
+                }
+                if (h == 0 && g == 0 && lo_ok) yp[-1] = p0;
+            }
+    }
+}
+
+template <class Cfg>
+__global__ void __launch_bounds__(StreamCfg<Cfg>::NT, 1)
+convt_stream_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed,
+                       const __grid_constant__ RunTable rows, int ntiles, int *__restrict__ status) {
+    using SC = StreamCfg<Cfg>;
+    constexpr int CIN = Cfg::CIN, N = Cfg::N, NG = Cfg::NG, KCA = Cfg::KCA, NCONV = Cfg::NCONV, NMW = Cfg::NMW;
+    constexpr int ROWS = Cfg::ROWS, APITCH = Cfg::APITCH, ASLOT = Cfg::ASLOT, BSLOT = Cfg::BSLOT, NCHUNK = Cfg::NCHUNK;
+    constexpr int AR = SC::AR, XPITCH = SC::XPITCH, XSLOT = SC::XSLOT, NSA = SC::NSA, NSX = SC::NSX, MAXSEG = SC::MAXSEG;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint8_t *bres = smem, *aring = smem + SC::BRES, *xring = aring + NSA * ASLOT;
+    uint64_t *fullW = reinterpret_cast<uint64_t *>(xring + NSX * XSLOT);
+    uint64_t *fullA = fullW + 1, *emptyA = fullA + NSA, *fullX = emptyA + NSA, *emptyX = fullX + NSX;
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int Lin = rows.stride;  // input positions between items
+
+    if (tid == 0) {
+        mbar_init(fullW, 1);
+        for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NMW); }
+        for (int s = 0; s < NSX; ++s) { mbar_init(&fullX[s], 1); mbar_init(&emptyX[s], NCONV); }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp == (NCONV + 128 * NMW) / 32) {
+        // ================= producer warp: resident B (lane 0), then the input tiles (lane c: channel c of a slot) =========
+        if (lane == 0) {
+            const uint8_t *src = reinterpret_cast<const uint8_t *>(packed) + tc_region_start() + tc_up_offset(Cfg::STAGE);
+            mbar_arrive_expect_tx(fullW, SC::BRES);
+            for (int i = 0; i < NCHUNK; ++i) bulk_g2s(bres + i * BSLOT, src + (size_t)i * BSLOT, BSLOT, fullW);
+        }
+        pdl_wait();  // x: the previous kernel's output
+        int sx = 0, phx = 0;
+        bool ok = true;
+#pragma unroll 1
+        for (int tile = blockIdx.x; tile < ntiles && ok; tile += gridDim.x) {
+            const int r0 = tile * ROWS;
+            XSeg seg[MAXSEG];
+            int covered;
+            tile_segments<SC>(rows, r0, seg, covered);
+#pragma unroll 1
+            for (int ca = 0; ca < CIN / KCA; ++ca) {
+                ok = __shfl_sync(0xffffffffu, lane == 0 ? mbar_wait(&emptyX[sx], phx ^ 1) : false, 0);
+                if (!ok) break;
+                float *slot = reinterpret_cast<float *>(xring + sx * XSLOT) + lane * XPITCH;
+                size_t g0[MAXSEG];
+                uint32_t bytes = 0;
+#pragma unroll
+                for (int k = 0; k < MAXSEG; ++k) {
+                    g0[k] = ((size_t)seg[k].item * CIN + ca * KCA + lane) * Lin + seg[k].u0;
+                    if (seg[k].n > 0) bytes += (uint32_t)((((g0[k] + seg[k].n + 3) & ~(size_t)3) - (g0[k] & ~(size_t)3)) * 4);
+                }
+                const uint32_t total = __reduce_add_sync(0xffffffffu, bytes);
+                if (lane == 0) mbar_arrive_expect_tx(&fullX[sx], total);
+                __syncwarp();
+#pragma unroll
+                for (int k = 0; k < MAXSEG; ++k)
+                    if (seg[k].n > 0) {
+                        const size_t a = g0[k] & ~(size_t)3, e = (g0[k] + seg[k].n + 3) & ~(size_t)3;
+                        bulk_g2s(slot + seg[k].dst, x + a, (uint32_t)((e - a) * 4), &fullX[sx]);
+                    }
+                if (++sx == NSX) { sx = 0; phx ^= 1; }
+            }
+        }
+        if (!ok && lane == 0) atomicExch(status, 12);
+    } else if (warp >= NCONV / 32) {
+        // ================= MMA warpgroup mw: rows [64 mw, 64 mw + 64) of every tile =================
+        const int mw = warp / 4 - NCONV / 128, t = tid & 127;
+        const uint64_t adesc_t = desc_template(APITCH, 128), bdesc_t = desc_template(N * 16, 128);
+        const uint32_t aring_addr = smem_u32(aring) + mw * 64 * 16, bres_addr = smem_u32(bres);
+        float bj[NG / 8][2];  // bias of this thread's channels 8k + 2q + e
+#pragma unroll
+        for (int k = 0; k < NG / 8; ++k)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) bj[k][e] = __ldg(packed + bias_offset(1 + Cfg::STAGE) + 8 * k + 2 * (t & 3) + e);
+        float acc[N / 2];
+        int sa = 0, pha = 0;
+        bool ok = mbar_wait(fullW, 0);  // a timed-out wait only raises the status word: control flow stays uniform
+#pragma unroll 1
+        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+            int psa = -1;
+#pragma unroll 1
+            for (int ca = 0; ca < CIN / KCA; ++ca) {
+                ok &= mbar_wait(&fullA[sa], pha);
+                const uint64_t abase = desc_at(adesc_t, aring_addr + sa * ASLOT);
+#pragma unroll 1
+                for (int j = 0; j < KCA / 16; ++j) {
+                    const uint64_t bbase = desc_at(bdesc_t, bres_addr + (ca * (KCA / 16) + j) * BSLOT);
+                    wgmma_fence();
+#pragma unroll
+                    for (int tap = 0; tap < 2; ++tap)
+#pragma unroll
+                        for (int pass = 0; pass < 3; ++pass) {
+                            const int ahalf = (pass == 1), bhalf = (pass == 2);
+                            const uint64_t bdesc = bbase + (uint64_t)((((tap * 2 + bhalf) * 2) * N * 16) >> 4);
+                            const uint64_t adesc = abase + (uint64_t)((ahalf * (KCA / 8) * APITCH + (1 - tap) * 16) >> 4) +
+                                                   (uint64_t)(2 * j * (APITCH >> 4));
+                            wgmma_bf16<N>(acc, adesc, bdesc, (ca | j | tap | pass) != 0);
+                        }
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    if (t == 0 && psa >= 0) mbar_arrive(&emptyA[psa]);
+                    psa = (j == KCA / 16 - 1) ? sa : -1;
+                }
+                if (++sa == NSA) { sa = 0; pha ^= 1; }
+            }
+            wgmma_wait<0>();
+            acc_fence<N / 2>(acc);
+            if (t == 0) mbar_arrive(&emptyA[psa]);
+            if (tile + (int)gridDim.x >= ntiles) pdl_trigger();  // last tile's MMAs done: the next kernel may be scheduled
+            pdl_wait();
+            convt_stream_store<Cfg>(acc, bj, y, mw, t, tile * ROWS, rows);
+        }
+        if (!ok && t == 0) atomicExch(status, 13);
+    } else {
+        // ================= converter warps: A slots = split(lrelu(x)) from the staging slots =================
+        pdl_wait();  // (rows that are not staged are read from x)
+        int sx = 0, phx = 0, sa = 0, pha = 0;
+        bool ok = true;
+#pragma unroll 1
+        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+            const int r0 = tile * ROWS;
+            XSeg seg[MAXSEG];
+            int covered;
+            tile_segments<SC>(rows, r0, seg, covered);
+#pragma unroll 1
+            for (int ca = 0; ca < CIN / KCA; ++ca) {
+                if (ok && !(mbar_wait(&fullX[sx], phx) && mbar_wait(&emptyA[sa], pha ^ 1))) {
+                    ok = false;
+                    atomicExch(status, 14);
+                }
+                const float *xs = reinterpret_cast<const float *>(xring + sx * XSLOT);
+                uint8_t *slot = aring + sa * ASLOT;
+#pragma unroll 1
+                for (int u = tid; u < AR * (KCA / 8); u += NCONV) {
+                    const int i = u % AR, kp = u / AR;
+                    int off = -1;
+                    uint32_t gb = 0;  // low bits of the global float index of channel 8 kp's row: the staging alignment
+#pragma unroll
+                    for (int k = 0; k < MAXSEG; ++k)
+                        if (i >= seg[k].i0 && i < seg[k].i0 + seg[k].n) {
+                            off = seg[k].dst + i - seg[k].i0;
+                            gb = ((uint32_t)seg[k].item * CIN + ca * KCA + 8 * kp) * (uint32_t)Lin + seg[k].u0;
+                        }
+                    float f[8];
+                    if (off >= 0) {
+#pragma unroll
+                        for (int e = 0; e < 8; ++e) f[e] = xs[(8 * kp + e) * XPITCH + off + ((gb + e * Lin) & 3)];
+                    } else {
+                        const RunPos p = i >= covered ? rows.find(r0 - 1 + i) : RunPos{-1, 0, 0};
+                        const bool inr = p.item >= 0 && p.unit < p.len;
+                        const float *xp = x + ((size_t)(inr ? p.item : 0) * CIN + ca * KCA + 8 * kp) * Lin + (inr ? p.unit : 0);
+#pragma unroll
+                        for (int e = 0; e < 8; ++e) f[e] = inr ? __ldg(xp + (size_t)e * Lin) : 0.f;
+                    }
+                    uint32_t h[4], l[4];
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) split2_bf16(lrelu(f[2 * e]), lrelu(f[2 * e + 1]), h[e], l[e]);
+                    *reinterpret_cast<uint4 *>(slot + kp * APITCH + i * 16) = make_uint4(h[0], h[1], h[2], h[3]);
+                    *reinterpret_cast<uint4 *>(slot + (KCA / 8 + kp) * APITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
+                }
+                fence_proxy_async();
+                mbar_arrive(&fullA[sa]);
+                mbar_arrive(&emptyX[sx]);
+                if (++sa == NSA) { sa = 0; pha ^= 1; }
+                if (++sx == NSX) { sx = 0; phx ^= 1; }
+            }
+        }
+    }
+}
+
+template <class Cfg>
+static int launch_convt_stream(const float *x, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s) {
+    using SC = StreamCfg<Cfg>;
+    static bool configured = false;
+    if (!configured) {
+        MG_CUDA_TRY(cudaFuncSetAttribute(convt_stream_tc_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, SC::SMEM_BYTES));
+        configured = true;
+    }
+    if (reinterpret_cast<uintptr_t>(x) % 16 != 0)  // the bulk copies read 16-byte-aligned supersets of x's rows
+        return set_error(MG_ERR_INVALID_ARGUMENT, "launch_convt_tc: stage %d input not 16-byte aligned", Cfg::STAGE);
+    int dev = 0, sms = 0;
+    MG_CUDA_TRY(cudaGetDevice(&dev));
+    MG_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const RunTable rows = convt_rows(batch);
+    const int ntiles = (rows.first[rows.n] + Cfg::ROWS - 1) / Cfg::ROWS;
+    const unsigned grid = (unsigned)(ntiles < sms ? ntiles : sms);
+    MG_CUDA_TRY(launch_ex(convt_stream_tc_kernel<Cfg>, dim3(grid), dim3(SC::NT), SC::SMEM_BYTES, s, true, 1, x, y, packed, rows, ntiles,
+                          status));
+    return MG_OK;
+}
+
+// the tile geometry of the streaming stride-2 ConvT (stage 2 or 3): rows per tile, staged item segments per tile, staging
+// slots; its grid is min(tiles, SMs)
+template <class Cfg>
+static const char *stream_cfg_name() {
+    static char buf[80];
+    snprintf(buf, sizeof(buf), "convt_stream_tc_kernel<StreamCfg<%d,%d,%d,%d>>", Cfg::STAGE, Cfg::ROWS, StreamCfg<Cfg>::MAXSEG,
+             StreamCfg<Cfg>::NSX);
+    return buf;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // Variant for a stage whose whole activation tile fits in shared memory (stage 1: 65 rows x 256 channels, hi+lo =
 // 72 KB): the A operand is converted ONCE per row tile and stays resident, and the CTA loops over the NCG output-channel
 // groups, so no activation is loaded or converted twice.  One MMA warpgroup (64 rows, N = 256) per CTA.  The converter
@@ -378,10 +667,19 @@ int launch_convt_tc(const float *x, float *y, const float *packed, int stage, co
     switch (stage) {
         case 0: return launch_convt<UpCfg<0>>(x, y, packed, batch, status, s);
         case 1: return launch_convt_resident<UpCfg<1>>(x, y, packed, batch, status, s);
-        case 2: return launch_convt<UpCfg<2>>(x, y, packed, batch, status, s);
-        case 3: return launch_convt<UpCfg<3>>(x, y, packed, batch, status, s);
+        case 2: return launch_convt_stream<UpCfg<2>>(x, y, packed, batch, status, s);
+        case 3: return launch_convt_stream<UpCfg<3>>(x, y, packed, batch, status, s);
     }
     return set_error(MG_ERR_INVALID_ARGUMENT, "launch_convt_tc: stage %d", stage);
+}
+
+// the configuration launch_convt_tc runs for the stride-2 stages ("" for the others)
+const char *convt_config_name(int stage) {
+    switch (stage) {
+        case 2: return stream_cfg_name<UpCfg<2>>();
+        case 3: return stream_cfg_name<UpCfg<3>>();
+    }
+    return "";
 }
 
 }  // namespace mg

@@ -62,6 +62,8 @@ def lib():
         L.mg_gen_upres_post.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
         L.mg_gen_resblock_config.restype = ctypes.c_char_p
         L.mg_gen_resblock_config.argtypes = [ctypes.c_int]
+        L.mg_gen_convt_config.restype = ctypes.c_char_p
+        L.mg_gen_convt_config.argtypes = [ctypes.c_int]
         L.mg_gen_conv_pre.restype = ctypes.c_int
         L.mg_gen_conv_pre.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
         L.mg_gen_resblock_post.restype = ctypes.c_int
