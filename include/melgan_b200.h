@@ -92,6 +92,27 @@ int mg_gen_forward(const void *packed, const float *mel, float *audio, int B, in
 int mg_gen_forward_ragged(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
                           void *workspace, size_t workspace_bytes, void *stream);
 
+/* Inference precision of a generator forward.
+ *   MG_GEN_PRECISION_FP32: what mg_gen_forward computes -- every tensor-core product as three bf16 passes on a hi + lo
+ *     split of both operands, fp32-equivalent audio (~1e-5 from a float64 forward).
+ *   MG_GEN_PRECISION_BF16: one bf16 pass per product, fp32 accumulation, in the ConvTranspose of stages 0, 1 and 3 and in
+ *     all 24 ResBlock convs: LeakyReLU(x) and the folded weights are each rounded to bf16 (round to nearest even) before
+ *     they are multiplied.  conv_pre and the stride-2 ConvTranspose of stage 2 keep their three passes; the residual
+ *     stream, the biases and LeakyReLU -> conv_post -> tanh stay fp32.  Same packed weights, same workspace, no extra
+ *     memory.  Measured with the seeded random weights of the tests at B = 64, T = 32 (tests/test_bf16_inference_gpu.py):
+ *     relative L2 from float64 9.8e-4 / 1.6e-3, SNR 60 / 56 dB, max |d| 1.8e-4 / 3.1e-4 for N(0,1) / log-mel-like input,
+ *     within 1.12x of a float64 emulation of the same rounding.  Trained weights may behave differently.
+ * Only the default chain has bf16 kernels: after mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected another one,
+ * a bf16 forward returns MG_ERR_INVALID_ARGUMENT. */
+#define MG_GEN_PRECISION_FP32 0
+#define MG_GEN_PRECISION_BF16 1
+/* mg_gen_forward (lengths NULL: every item T_max frames) or mg_gen_forward_ragged (lengths as there) with a precision;
+ * MG_GEN_PRECISION_FP32 gives exactly their audio.  Ragged batches, batch slices, mg_gen_check_status and
+ * mg_gen_stage_output work as after those calls.  Every argument is checked before any CUDA call; an unknown precision is
+ * MG_ERR_INVALID_ARGUMENT. */
+int mg_gen_forward_precision(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
+                             int precision, void *workspace, size_t workspace_bytes, void *stream);
+
 /* Same as mg_gen_forward, but brackets each of the mg_gen_forward_launches() kernels with CUDA
  * events on `stream`, waits for the last one and returns the per-kernel device times in
  * kernel_ms[0 .. mg_gen_forward_launches()-1] (names: mg_gen_kernel_name(i)).  Used by bench.py for the
@@ -218,6 +239,10 @@ int mg_gen_engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_
  * valid prefix and the zero tail). */
 int mg_gen_engine_forward_ragged(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max,
                                  const int *lengths);
+/* mg_gen_engine_forward (lengths NULL) / mg_gen_engine_forward_ragged with a precision (MG_GEN_PRECISION_*, contract at
+ * mg_gen_forward_precision). */
+int mg_gen_engine_forward_precision(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max,
+                                    const int *lengths, int precision);
 /* Device time of the last forward in milliseconds (CUDA events on the engine's stream around the sliced
  * upload -> kernels -> download sequence). */
 int mg_gen_engine_last_kernel_ms(mg_gen_engine *e, float *ms);

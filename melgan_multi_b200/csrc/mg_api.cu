@@ -17,10 +17,24 @@ static int *status_ptr(void *workspace, int B, int T) {
 // batch: mel lengths (stride T); mel_host / audio_host: optional pinned host buffers (the engine entry point); the copies
 // ride on the batch slices' streams
 static int run_generator(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, cudaStream_t s,
-                         cudaEvent_t *ev, const float *mel_host = nullptr, float *audio_host = nullptr) {
+                         cudaEvent_t *ev, const float *mel_host = nullptr, float *audio_host = nullptr,
+                         int precision = MG_GEN_PRECISION_FP32) {
     int *st = status_ptr(ws, batch.items(), batch.stride);
     MG_CUDA_TRY(cudaMemsetAsync(st, 0, sizeof(int), s));
-    return launch_generator_tc(packed, mel, audio, batch, ws, st, s, ev, mel_host, audio_host);
+    return launch_generator_tc(packed, mel, audio, batch, ws, st, s, ev, mel_host, audio_host, precision);
+}
+
+// a known precision, and bf16 only on the default chain (the only one with single-pass kernels)
+static int check_precision(const char *fn, int precision) {
+    if (precision != MG_GEN_PRECISION_FP32 && precision != MG_GEN_PRECISION_BF16)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: unknown precision %d (MG_GEN_PRECISION_FP32 = 0, MG_GEN_PRECISION_BF16 = 1)", fn,
+                         precision);
+    if (precision == MG_GEN_PRECISION_BF16 && !generator_tc_default_chain())
+        return set_error(MG_ERR_INVALID_ARGUMENT,
+                         "%s: bf16 runs on the default chain only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected "
+                         "another (tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
+                         fn, generator_tc_tail(), generator_tc_fused_up());
+    return MG_OK;
 }
 
 static int check_shape(const char *fn, int B, int T) {
@@ -120,6 +134,17 @@ int mg_gen_forward_ragged(const void *packed, const float *mel, float *audio, in
     if (rc) return rc;
     return run_generator((const float *)packed, mel, audio, RunTable::ragged(lengths, B, T_max), (float *)workspace,
                          (cudaStream_t)stream, nullptr);
+}
+
+int mg_gen_forward_precision(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
+                             int precision, void *workspace, size_t workspace_bytes, void *stream) {
+    const char *fn = "mg_gen_forward_precision";
+    int rc = check_precision(fn, precision);
+    if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
+    if (!rc) rc = check_forward(fn, packed, mel, audio, B, T_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    return run_generator((const float *)packed, mel, audio, lengths ? RunTable::ragged(lengths, B, T_max) : RunTable::uniform(B, T_max),
+                         (float *)workspace, (cudaStream_t)stream, nullptr, nullptr, nullptr, precision);
 }
 
 int mg_gen_forward_timed(const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
@@ -519,7 +544,8 @@ static int engine_check(const char *fn, mg_gen_engine *e, const float *mel_host,
     return MG_OK;
 }
 
-static int engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, const RunTable &batch) {
+static int engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, const RunTable &batch,
+                          int precision = MG_GEN_PRECISION_FP32) {
     const int B = batch.items(), T = batch.stride;
     const size_t frames = (size_t)B * T;
     int rc = engine_reserve(e, frames);
@@ -534,7 +560,8 @@ static int engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_
     if (!e->pin_status) MG_CUDA_TRY(cudaMallocHost(&e->pin_status, sizeof(int)));
     MG_CUDA_TRY(cudaEventRecord(e->ev0, e->stream));
     // upload, kernels and download are enqueued per batch slice (launch_generator_tc); one synchronisation at the end
-    rc = run_generator(e->packed, e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : e->pin_out);
+    rc = run_generator(e->packed, e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : e->pin_out,
+                       precision);
     if (rc) return rc;
     MG_CUDA_TRY(cudaEventRecord(e->ev1, e->stream));
     *e->pin_status = 0;
@@ -557,6 +584,17 @@ int mg_gen_engine_forward_ragged(mg_gen_engine *e, const float *mel_host, float 
     int rc = check_lengths("mg_gen_engine_forward_ragged", B, T_max, lengths);
     if (!rc) rc = engine_check("mg_gen_engine_forward_ragged", e, mel_host, audio_host);
     return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::ragged(lengths, B, T_max));
+}
+
+int mg_gen_engine_forward_precision(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max,
+                                    const int *lengths, int precision) {
+    const char *fn = "mg_gen_engine_forward_precision";
+    int rc = check_precision(fn, precision);
+    if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
+    if (!rc) rc = engine_check(fn, e, mel_host, audio_host);
+    if (rc) return rc;
+    return engine_forward(e, mel_host, audio_host, lengths ? RunTable::ragged(lengths, B, T_max) : RunTable::uniform(B, T_max),
+                          precision);
 }
 
 int mg_gen_engine_last_kernel_ms(mg_gen_engine *e, float *ms) {

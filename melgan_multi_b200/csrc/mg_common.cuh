@@ -161,13 +161,15 @@ int generator_tc_num_launches();
 int generator_tc_fused_up();  // bit 0: stage 2, bit 1: stage 3 run their stride-2 ConvT at the FRONT of the ResBlock kernel
 int generator_tc_tail();      // bit i: stage i's ConvT runs at the TAIL of ResBlock i-1's kernel
 void generator_tc_set_tail(int mask);
+bool generator_tc_default_chain();  // no tail fusion, stage 3's ConvT (only) at the front of the last kernel
 const char *generator_tc_kernel_name(int i);
 const char *generator_tc_kernel_config(int i, int T);
 const char *resblock_config_name(int stage, int L);
 int generator_tc_slices(int B, long long frames);  // batch slices (concurrent kernel chains) one forward is cut into
 // batch: the items' mel lengths, stride T_max (the layout of mel, audio and every workspace buffer)
 int launch_generator_tc(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
-                        cudaStream_t s, cudaEvent_t *ev = nullptr, const float *mel_host = nullptr, float *audio_host = nullptr);
+                        cudaStream_t s, cudaEvent_t *ev = nullptr, const float *mel_host = nullptr, float *audio_host = nullptr,
+                        int precision = MG_GEN_PRECISION_FP32);
 int launch_gen_pre_tc(const float *mel, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s);
 int launch_disc_post1_tc(const float *x, float *y, const uint8_t *wtc, const float *bias, int Bt, int L, int *status,
                          cudaStream_t s);
@@ -208,9 +210,11 @@ int mel_frames(int L);
 int launch_mel(const void *tables, const float *audio, float *mel, int B, int L, cudaStream_t s);
 int launch_msd_forward(const void *packed, const float *y, int Bt, int L, float *const *fmaps, int *status, cudaStream_t s);
 // batch: lengths and stride of the kernel's input (ConvT) / of the ResBlock itself (the output length for codes 12..14)
-int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s);
+// precision: MG_GEN_PRECISION_FP32 (3-pass split bf16) or MG_GEN_PRECISION_BF16 (one pass; only the default chain's kernels)
+int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
+                    int precision = MG_GEN_PRECISION_FP32);
 const char *convt_config_name(int stage);
 int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
-                       long long *trace = nullptr);
+                       long long *trace = nullptr, int precision = MG_GEN_PRECISION_FP32);
 
 }  // namespace mg

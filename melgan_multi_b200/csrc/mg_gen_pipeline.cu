@@ -26,6 +26,7 @@ int generator_tc_tail() {
     }();
     return g_tail_override >= 0 ? (g_tail_override & 0b1110) : env_mask;
 }
+bool generator_tc_default_chain() { return generator_tc_tail() == 0 && generator_tc_fused_up() == 2; }
 int generator_tc_fused_up() {
     static const int mask = [] {
         const char *e = getenv("MG_GEN_FUSE_UP");
@@ -89,9 +90,10 @@ const char *generator_tc_kernel_config(int i, int T) {
 
 // Tensor-core pipeline of one contiguous slice of the batch (mel lengths, stride T_max).  a0: conv_pre output; a[0]:
 // ResBlock-0 output (unfused chains); a[1], a[2], u: three buffers of 8192 T_max floats per item that the stages rotate
-// through (a kernel never writes its input).  Every kernel gets the batch at its own scale.
+// through (a kernel never writes its input).  Every kernel gets the batch at its own scale.  precision goes to the ConvT
+// and ResBlock kernels (conv_pre always runs its three passes).
 static int generator_tc_chain(const float *packed, const float *mel, float *audio, const RunTable &batch, float *a0,
-                              float *const *a, float *u, int *status, cudaStream_t s, cudaEvent_t *ev) {
+                              float *const *a, float *u, int *status, cudaStream_t s, cudaEvent_t *ev, int precision) {
     ChainStep st[12];
     const int n = build_chain(st);
     int rc;
@@ -111,7 +113,7 @@ static int generator_tc_chain(const float *packed, const float *mel, float *audi
             cur = a0;
         } else if (k.kind == 1) {
             float *out = cur != u ? u : other(cur, nullptr);  // (unfused chain: ConvT outputs live in u, ResBlock i's in a[i])
-            if ((rc = launch_convt_tc(cur, out, packed, k.arg, batch.scaled(len), status, s))) return rc;
+            if ((rc = launch_convt_tc(cur, out, packed, k.arg, batch.scaled(len), status, s, precision))) return rc;
             cur = out;
             len *= stage_stride(k.arg);
         } else {
@@ -120,7 +122,7 @@ static int generator_tc_chain(const float *packed, const float *mel, float *audi
             const bool front = k.arg >= 12 && k.arg <= 14, tailf = k.arg >= 20;
             float *out = last ? audio : (k.arg <= 2 && cur != a[k.arg]) ? a[k.arg] : other(cur, nullptr);
             const int Lk = front ? 2 * len : len;  // the ResBlock's own length
-            if ((rc = launch_resblock_tc(cur, out, packed, k.arg, batch.scaled(Lk), status, s))) return rc;
+            if ((rc = launch_resblock_tc(cur, out, packed, k.arg, batch.scaled(Lk), status, s, nullptr, precision))) return rc;
             cur = out;
             len = tailf ? Lk * stage_stride(k.arg - 20 + 1) : Lk;
         }
@@ -169,9 +171,10 @@ int generator_tc_slices(int B, long long frames) {
 
 // mel_host / audio_host (both or neither; pinned): the host-buffer entry point's copies, cut the same way -- each slice's
 // stream uploads its items' valid mel prefixes before its chain and downloads its audio rows (valid prefix and zero tail)
-// after it, so all but the last download overlap the other chains' kernels.
+// after it, so all but the last download overlap the other chains' kernels.  precision: MG_GEN_PRECISION_*; the caller
+// has checked that a bf16 forward runs the default chain.
 int launch_generator_tc(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
-                        cudaStream_t s, cudaEvent_t *ev, const float *mel_host, float *audio_host) {
+                        cudaStream_t s, cudaEvent_t *ev, const float *mel_host, float *audio_host, int precision) {
     const int B = batch.items(), T = batch.stride;
     long long frames = 0;
     for (int r = 0; r < batch.n; ++r) frames += (long long)(batch.item0[r + 1] - batch.item0[r]) * batch.len[r];
@@ -226,7 +229,7 @@ int launch_generator_tc(const float *packed, const float *mel, float *audio, con
             }
             float *a[3] = {base[1] + b0 * per_item[1], base[2] + b0 * per_item[2], base[3] + b0 * per_item[3]};
             int r = generator_tc_chain(packed, mel + b0 * mel_item, audio + b0 * audio_item, part, base[0] + b0 * per_item[0], a,
-                                       base[5] + b0 * per_item[5], status, q, ev);
+                                       base[5] + b0 * per_item[5], status, q, ev, precision);
             if (r) return r;
             if (audio_host)
                 MG_CUDA_TRY(cudaMemcpyAsync(audio_host + b0 * audio_item, audio + b0 * audio_item, nb * audio_item * sizeof(float),

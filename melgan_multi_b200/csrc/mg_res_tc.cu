@@ -37,6 +37,10 @@
 // disappears.  An input position s owns the outputs [S s - pad, S s - pad + S) and needs x[s - 1]: tiles overlap by one
 // more row on the left (HL = HALO + 1).  Position L (x[L] = 0) would own the last `pad` outputs; those pad * C/2 outputs --
 // dot products of x[L-1] with the tap-1 weights -- are computed in fp32 by the CTA that owns position L - 1.
+// Bf16<Cfg> (mg_tc.cuh; the default chain's Rb0, Rb1, Rb2 and Up3Rb3Post): the same kernel with one pass (xh, wh) per
+// product -- in the convs and the front ConvT's taps --, X and the front ConvT operand written as hi only, the weight
+// ring filled with the hi half of each chunk and the cluster halo exchange sending the hi k-panels only.  The fp32 parts
+// (residual stream, biases, conv_post epilogue) are unchanged.
 #include <stdlib.h>
 #include <string.h>
 
@@ -54,6 +58,7 @@ struct RbCfg {
     static constexpr int C = C_, NRB = NRB_, RPW = RPW_, NCP = NCP_, NSTAGE = NSTAGE_, UPT = UPT_, CS = CS_;
     static constexpr bool POST = POST_;  // fuse LeakyReLU -> conv_post -> tanh into the final epilogue (last stage)
     static constexpr bool UPF = UPF_;
+    static constexpr bool ONEPASS = false;  // Bf16<RbCfg<..>>: one bf16 pass per product (mg_tc.cuh)
     static constexpr int P = 64 * NRB;
     static constexpr int NWG = NRB / RPW * NCP;  // consumer warpgroups
     static constexpr int NCONS = 128 * NWG;
@@ -115,6 +120,12 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     constexpr int XPITCH = Cfg::XPITCH, XBYTES = Cfg::XBYTES, KC = Cfg::KC, CHUNK = Cfg::CHUNK, NSTAGE = Cfg::NSTAGE;
     constexpr int NCONS = Cfg::NCONS, NCP = Cfg::NCP, NCW = Cfg::NCW, RPW = Cfg::RPW, KSL = Cfg::KSL, NA = NCW / 2;
     constexpr int CS = Cfg::CS, XCH = Cfg::XCH;
+    // passes per product: (xh, wh), (xl, wh), (xh, wl), or (xh, wh) alone in the single-pass variant, which then never
+    // writes or reads Xl nor the lo half of a weight chunk
+    constexpr bool ONE = Cfg::ONEPASS;
+    constexpr int NPASS = ONE ? 1 : 3;
+    constexpr uint32_t WBYTES = ONE ? Cfg::HALF : CHUNK;  // bytes of a ResBlock / front-ConvT weight chunk brought in
+    static_assert(!ONE || Cfg::UPT == 0, "the single-pass variant has no tail ConvT");
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *Xh = smem, *Xl = smem + XBYTES, *ring = smem + 2 * XBYTES;
     float *pend = reinterpret_cast<float *>(ring + NSTAGE * CHUNK);  // sum of the c2 biases folded so far
@@ -198,7 +209,8 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     if (warp == NCONS / 32) {
         // ================= TMA producer: streams the weight chunks through the ring in consumption order =================
         // (clusters: chunk j is read from L2 once, by rank j % CS, and multicast into the same slot of every CTA; each
-        // producer still posts its own CTA's expected bytes, after its empty[s] has seen every consumer of the cluster)
+        // producer still posts its own CTA's expected bytes, after its empty[s] has seen every consumer of the cluster.
+        // Single pass: only the first WBYTES = HALF bytes of a chunk, its hi half, are sent and expected.)
         if (lane == 0) {
             int s = 0, ph = 0, j = 0;
             bool ok = true;
@@ -212,11 +224,11 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
             };
             if constexpr (Cfg::UPF) {  // the fused ConvT's 4 taps x UKSL K-slices, in blob order
                 const uint8_t *src = tc_base + tc_upf_offset(stage);
-                for (int i = 0; i < Cfg::NUPCH; ++i) put(src + (size_t)i * CHUNK, CHUNK);
+                for (int i = 0; i < Cfg::NUPCH; ++i) put(src + (size_t)i * CHUNK, WBYTES);
             }
             for (int conv = 0; conv < 6; ++conv) {  // chunk (tap, K-slice) sits at blob index tap * KSL + ks: consumption order
                 const uint8_t *src = tc_base + tc_res_offset(l0 + (conv >> 1) + 3 * (conv & 1));
-                for (int i = 0; i < Cfg::NCHUNK; ++i) put(src + (size_t)i * CHUNK, CHUNK);
+                for (int i = 0; i < Cfg::NCHUNK; ++i) put(src + (size_t)i * CHUNK, WBYTES);
             }
             if constexpr (Cfg::UPT != 0) {  // the tail ConvT's B slots, in blob order [group][16-channel chunk][tap]
                 const uint8_t *src = tc_base + tc_up_offset(stage + 1);
@@ -298,14 +310,15 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                     uint32_t hi, lo;
                     split2_bf16(f0, f1, hi, lo);
                     *reinterpret_cast<uint32_t *>(xh + k * XPITCH) = hi;
-                    *reinterpret_cast<uint32_t *>(xl + k * XPITCH) = lo;
+                    if constexpr (!ONE) *reinterpret_cast<uint32_t *>(xl + k * XPITCH) = lo;
                     if (keep_last && tp == L - 1) *reinterpret_cast<float2 *>(b1s + col) = make_float2(f0, f1);
                 }
             }
     };
-    // clusters: the XCH rows next to a cluster-internal border (all k-panels of hi and lo) are bulk-copied into the
-    // neighbour's slack rows after every hand-off.  A thread that writes such a row first waits until the neighbours'
-    // MMAs of the previous conv are done, which also means the previous copies out of this X have landed.
+    // clusters: the XCH rows next to a cluster-internal border (all k-panels of hi and lo; of hi only in the single-pass
+    // variant) are bulk-copied into the neighbour's slack rows after every hand-off.  A thread that writes such a row first
+    // waits until the neighbours' MMAs of the previous conv are done, which also means the previous copies out of this X
+    // have landed.
     bool border = false;
 #pragma unroll
     for (int r = 0; r < RPW; ++r)
@@ -314,7 +327,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
             const int p = (rb0 + r) * 64 + frag_row(t, h);
             border |= (crank > 0 && p < XCH) || (crank < CS - 1 && p >= P - XCH);
         }
-    constexpr int NXC = 2 * Cfg::KP;        // copies per border: one per k-panel of hi and lo
+    constexpr int NXC = (ONE ? 1 : 2) * Cfg::KP;  // copies per border: one per k-panel of hi and lo (hi: single pass)
     constexpr uint32_t XCB = XCH * 16;      // bytes per copy
     // (a warp issues bulk copies one lane at a time: they are spread over every consumer warp, copy i by warp i % NW)
     constexpr int NW = NCONS / 32;
@@ -344,7 +357,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         if constexpr (CS > 1) send_halo();
         ++hand;
     };
-    // one conv: every chunk (tap, K-slice) x 3 passes x KC/16 k-steps x RPW row blocks
+    // one conv: every chunk (tap, K-slice) x NPASS passes x KC/16 k-steps x RPW row blocks
     auto conv_mma = [&](float (&A)[RPW][NA], int dil, bool fresh, int conv) {
         if constexpr (CS > 1) {  // the neighbours' border rows of this conv's input are in the slack rows
             MG_TR(88 + 2 * conv);
@@ -359,7 +372,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
             if (ch == 0) MG_TR(65 + 3 * conv);
             const uint32_t arow = (SLACK + rb0 * 64 + (tap - 1) * dil) * 16 + ks * (KC / 8) * XPITCH;
 #pragma unroll
-            for (int pass = 0; pass < 3; ++pass)
+            for (int pass = 0; pass < NPASS; ++pass)
 #pragma unroll
                 for (int k16 = 0; k16 < KC / 16; ++k16) {
                     const uint64_t bdesc = bbase + (uint64_t)(((pass == 2 ? Cfg::HALF : 0) + 2 * k16 * (C * 16)) >> 4);
@@ -394,7 +407,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
 #pragma unroll
             for (int e = 0; e < 4; ++e) split2_bf16(f[2 * e], f[2 * e + 1], h[e], l[e]);
             *reinterpret_cast<uint4 *>(Xh + kp * UPITCH + i * 16) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4 *>(Xl + kp * UPITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
+            if constexpr (!ONE) *reinterpret_cast<uint4 *>(Xl + kp * UPITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
         }
         fence_proxy_async();
         sync_cons();
@@ -410,7 +423,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                 const uint64_t bbase = desc_at(bdesc_t, chunk_begin());
                 const uint32_t arow = (rowoff + pb * 64) * 16 + ks * (KC / 8) * UPITCH;
 #pragma unroll
-                for (int pass = 0; pass < 3; ++pass)
+                for (int pass = 0; pass < NPASS; ++pass)
 #pragma unroll
                     for (int k16 = 0; k16 < KC / 16; ++k16) {
                         const uint64_t bdesc = bbase + (uint64_t)(((pass == 2 ? Cfg::HALF : 0) + 2 * k16 * (C * 16)) >> 4);
@@ -739,9 +752,21 @@ using Rb1Up2 = RbCfg<128, 2, 1, 1, 4, false, false, 2>;
 using Rb2Up3 = RbCfg<64, 4, 1, 1, 3, false, false, 2>;
 
 // x, y: [B][C][L] fp32 NCL with C = 256 >> stage, L = batch.stride, item i's first len_i positions its own; status: device
-// int, set non-zero if a pipeline wait timed out.
+// int, set non-zero if a pipeline wait timed out.  precision MG_GEN_PRECISION_BF16: the single-pass variant, which exists
+// for the default chain's stage codes 0, 1, 2 and 14.
 int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
-                       long long *trace) {
+                       long long *trace, int precision) {
+    if (precision == MG_GEN_PRECISION_BF16) {
+        switch (stage) {
+            case 0: return launch_resblock<Bf16<Rb0>>(x, y, packed, 0, batch, status, trace, s);
+            case 1: return launch_resblock<Bf16<Rb1>>(x, y, packed, 1, batch, status, trace, s);
+            case 2: return launch_resblock<Bf16<Rb2>>(x, y, packed, 2, batch, status, trace, s);
+            case 14: return launch_resblock<Bf16<Up3Rb3Post>>(x, y, packed, 3, batch, status, trace, s);
+        }
+        return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: stage code %d has no bf16 variant", stage);
+    }
+    if (precision != MG_GEN_PRECISION_FP32)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: precision %d", precision);
     switch (stage) {
         case 0: return launch_resblock<Rb0>(x, y, packed, 0, batch, status, trace, s);
         case 1: return launch_resblock<Rb1>(x, y, packed, 1, batch, status, trace, s);

@@ -198,5 +198,15 @@ __device__ __forceinline__ void split2_bf16(float x0, float x1, uint32_t &hi, ui
     lo = *reinterpret_cast<uint32_t *>(&l);
 }
 
+// ---- single-pass bf16 variant of a kernel configuration (mg_gen_forward_precision, MG_GEN_PRECISION_BF16) ----------
+// The same tiles, shared-memory layout and packed blob as Cfg, but one pass (xh, wh) per product with fp32 accumulation:
+// the converters store only the hi operand, and only the hi half of each weight chunk / slot is brought in (the lo half
+// of the blob and the Xl / lo regions of shared memory are left unused).  A distinct type, so the instantiations have
+// kernel symbols of their own ("resblock_tc_kernel<mg::tc::Bf16<mg::RbCfg<...>>>") in a profiler trace.
+template <class Cfg>
+struct Bf16 : Cfg {
+    static constexpr bool ONEPASS = true;
+};
+
 }  // namespace tc
 }  // namespace mg

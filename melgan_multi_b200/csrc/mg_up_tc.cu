@@ -29,6 +29,10 @@
 // memory, not by the tensor cores, so they run as a streaming kernel of their own (convt_stream_tc_kernel below): persistent
 // CTAs, the weights resident in shared memory, each tile's input brought in by bulk copies several slots ahead of the
 // converter, and an epilogue that stores pairs of neighbouring output samples.
+//
+// Bf16<UpCfg<0>> / Bf16<UpCfg<1>> (mg_tc.cuh): the stride-8 kernels with one pass (xh, wh) per product.  The converter
+// writes the hi operand only, and each B slot is filled by two bulk copies, tap 0 hi and tap 1 hi (half the slot's bytes),
+// at their usual offsets.  The streaming stride-2 kernel has no such variant: it is bound by memory, not by its MMAs.
 #include "mg_common.cuh"
 #include "mg_tc.cuh"
 
@@ -41,6 +45,7 @@ struct UpCfg {
     static constexpr int CIN = stage_cin(STAGE), COUT = stage_cout(STAGE), S = stage_stride(STAGE), PAD = stage_pad(STAGE);
     static constexpr int NG = up_ng(STAGE);
     static constexpr int NCG = COUT / NG;
+    static constexpr bool ONEPASS = false;                // Bf16<UpCfg<..>>: one bf16 pass per product (mg_tc.cuh)
     static constexpr int N = S * NG;                      // MMA N: every phase of the channel group
     static constexpr int NMW = (N > 128) ? 1 : 2;         // MMA warpgroups = 64-row blocks per CTA
     // channels per A slot = channels fetched per memory round trip of a converter thread
@@ -99,6 +104,21 @@ __device__ __forceinline__ void convt_store(const float *acc, float *__restrict_
     }
 }
 
+// B slot i of the blob ([tap][half: hi, lo][k-panel: 2][N][16 B]) into shared memory, completing on `bar`: the whole slot,
+// or (single pass) its tap-0 hi and tap-1 hi quarters, at the same offsets
+template <class Cfg>
+__device__ __forceinline__ void load_bslot(uint8_t *dst, const uint8_t *src, uint64_t *bar) {
+    constexpr uint32_t BSLOT = Cfg::BSLOT;
+    if constexpr (Cfg::ONEPASS) {
+        mbar_arrive_expect_tx(bar, BSLOT / 2);
+        bulk_g2s(dst, src, BSLOT / 4, bar);
+        bulk_g2s(dst + BSLOT / 2, src + BSLOT / 2, BSLOT / 4, bar);
+    } else {
+        mbar_arrive_expect_tx(bar, BSLOT);
+        bulk_g2s(dst, src, BSLOT, bar);
+    }
+}
+
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NT, 1)
 convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed,
@@ -106,6 +126,7 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
     constexpr int CIN = Cfg::CIN, N = Cfg::N, NG = Cfg::NG;
     constexpr int ROWS = Cfg::ROWS, APITCH = Cfg::APITCH, ASLOT = Cfg::ASLOT, BSLOT = Cfg::BSLOT, KCA = Cfg::KCA;
     constexpr int NSA = Cfg::NSA, NSB = Cfg::NSB, NCHUNK = Cfg::NCHUNK, NCONV = Cfg::NCONV, NMW = Cfg::NMW;
+    constexpr int NPASS = Cfg::ONEPASS ? 1 : 3;  // (xh, wh), (xl, wh), (xh, wl), or the first alone
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *aring = smem, *bring = smem + NSA * ASLOT;
     uint64_t *fullA = reinterpret_cast<uint64_t *>(bring + NSB * BSLOT);
@@ -132,8 +153,7 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
             bool ok = true;
             for (int i = 0; i < NCHUNK && ok; ++i) {
                 if (!mbar_wait(&emptyB[s], ph ^ 1)) { ok = false; break; }
-                mbar_arrive_expect_tx(&fullB[s], BSLOT);
-                bulk_g2s(bring + s * BSLOT, src + (size_t)i * BSLOT, BSLOT, &fullB[s]);
+                load_bslot<Cfg>(bring + s * BSLOT, src + (size_t)i * BSLOT, &fullB[s]);
                 if (++s == NSB) { s = 0; ph ^= 1; }
             }
             if (!ok) atomicExch(status, 12);
@@ -158,7 +178,7 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
 #pragma unroll
                 for (int tap = 0; tap < 2; ++tap)
 #pragma unroll
-                    for (int pass = 0; pass < 3; ++pass) {
+                    for (int pass = 0; pass < NPASS; ++pass) {
                         const int ahalf = (pass == 1), bhalf = (pass == 2);
                         const uint64_t bdesc = bbase + (uint64_t)((((tap * 2 + bhalf) * 2) * N * 16) >> 4);
                         const uint64_t adesc =
@@ -207,7 +227,8 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
 #pragma unroll
                     for (int e = 0; e < 4; ++e) split2_bf16(lrelu(f[8 * kp + 2 * e]), lrelu(f[8 * kp + 2 * e + 1]), h[e], l[e]);
                     *reinterpret_cast<uint4 *>(slot + kp * APITCH + i * 16) = make_uint4(h[0], h[1], h[2], h[3]);
-                    *reinterpret_cast<uint4 *>(slot + (KCA / 8 + kp) * APITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
+                    if constexpr (!Cfg::ONEPASS)
+                        *reinterpret_cast<uint4 *>(slot + (KCA / 8 + kp) * APITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
                 }
             }
             fence_proxy_async();
@@ -545,6 +566,7 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
     constexpr int KPT = CIN / 8;                    // k-panels of the resident A
     constexpr int AHALF = KPT * APITCH;             // bytes of one of {hi, lo}
     constexpr int NSB = 4, NCONV = Cfg::NCONV;
+    constexpr int NPASS = Cfg::ONEPASS ? 1 : 3;  // (xh, wh), (xl, wh), (xh, wl), or the first alone
     static_assert(Cfg::S == 8 && N == 256 && Cfg::NMW == 1 && 2 * AHALF + NSB * BSLOT + 256 + ROWS * 12 <= 227 * 1024,
                   "resident ConvT shape");
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -572,8 +594,7 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
             bool ok = true;
             for (int i = 0; i < NCG * NCHUNK && ok; ++i) {  // blob order is [cg][chunk]: exactly this loop
                 if (!mbar_wait(&emptyB[s], ph ^ 1)) { ok = false; break; }
-                mbar_arrive_expect_tx(&fullB[s], BSLOT);
-                bulk_g2s(bring + s * BSLOT, src + (size_t)i * BSLOT, BSLOT, &fullB[s]);
+                load_bslot<Cfg>(bring + s * BSLOT, src + (size_t)i * BSLOT, &fullB[s]);
                 if (++s == NSB) { s = 0; ph ^= 1; }
             }
             if (!ok) atomicExch(status, 32);
@@ -598,7 +619,7 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
 #pragma unroll
                 for (int tap = 0; tap < 2; ++tap)
 #pragma unroll
-                    for (int pass = 0; pass < 3; ++pass) {
+                    for (int pass = 0; pass < NPASS; ++pass) {
                         const uint64_t bdesc = bbase + (uint64_t)((((tap * 2 + (pass == 2)) * 2) * N * 16) >> 4);
                         const uint64_t adesc = abase + (uint64_t)((((pass == 1) ? AHALF : 0) + (1 - tap) * 16) >> 4);
                         wgmma_bf16<N>(acc, adesc, bdesc, (ch | tap | pass) != 0);
@@ -638,7 +659,8 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
 #pragma unroll
                     for (int e = 0; e < 4; ++e) split2_bf16(lrelu(f[8 * kp + 2 * e]), lrelu(f[8 * kp + 2 * e + 1]), h[e], l[e]);
                     *reinterpret_cast<uint4 *>(abuf + (ca * 8 + kp) * APITCH + i * 16) = make_uint4(h[0], h[1], h[2], h[3]);
-                    *reinterpret_cast<uint4 *>(abuf + AHALF + (ca * 8 + kp) * APITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
+                    if constexpr (!Cfg::ONEPASS)
+                        *reinterpret_cast<uint4 *>(abuf + AHALF + (ca * 8 + kp) * APITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
                 }
             }
             fence_proxy_async();
@@ -662,8 +684,14 @@ static int launch_convt_resident(const float *x, float *y, const float *packed, 
 }
 
 // x [B][Cin][Lin] -> y [B][Cout][S*Lin], fp32 NCL, (Cin, Cout, S) of generator stage `stage`; Lin = batch.stride, item i's
-// first len_i input positions (and S len_i output positions) are its own.
-int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s) {
+// first len_i input positions (and S len_i output positions) are its own.  precision MG_GEN_PRECISION_BF16: stages 0 and 1
+// run their single-pass variants; stages 2 and 3 keep the streaming kernel's three passes (it is bound by memory).
+int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
+                    int precision) {
+    if (precision != MG_GEN_PRECISION_FP32 && precision != MG_GEN_PRECISION_BF16)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "launch_convt_tc: precision %d", precision);
+    if (precision == MG_GEN_PRECISION_BF16 && stage == 0) return launch_convt<Bf16<UpCfg<0>>>(x, y, packed, batch, status, s);
+    if (precision == MG_GEN_PRECISION_BF16 && stage == 1) return launch_convt_resident<Bf16<UpCfg<1>>>(x, y, packed, batch, status, s);
     switch (stage) {
         case 0: return launch_convt<UpCfg<0>>(x, y, packed, batch, status, s);
         case 1: return launch_convt_resident<UpCfg<1>>(x, y, packed, batch, status, s);

@@ -45,6 +45,9 @@ def lib():
         L.mg_gen_forward_ragged.restype = ctypes.c_int
         L.mg_gen_forward_ragged.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+        L.mg_gen_forward_precision.restype = ctypes.c_int
+        L.mg_gen_forward_precision.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                               ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
         L.mg_gen_forward_timed.restype = ctypes.c_int
         L.mg_gen_forward_timed.argtypes = L.mg_gen_forward.argtypes + [ctypes.POINTER(ctypes.c_float)]
         L.mg_gen_check_status.restype = ctypes.c_int
@@ -143,6 +146,9 @@ def lib():
         L.mg_gen_engine_forward_ragged.restype = ctypes.c_int
         L.mg_gen_engine_forward_ragged.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                                    ctypes.c_void_p]
+        L.mg_gen_engine_forward_precision.restype = ctypes.c_int
+        L.mg_gen_engine_forward_precision.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                                      ctypes.c_void_p, ctypes.c_int]
         L.mg_gen_engine_last_kernel_ms.restype = ctypes.c_int
         L.mg_gen_engine_last_kernel_ms.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float)]
         L.mg_gen_engine_destroy.restype = None
@@ -176,6 +182,17 @@ def _lengths(lengths, B, T_max):
     if bad:
         raise EngineError("lengths must lie in [1, T_max = %d] (got %d)" % (T_max, bad[0]))
     return (ctypes.c_int * B)(*lengths)
+
+
+PRECISIONS = {"fp32": 0, "bf16": 1}  # MG_GEN_PRECISION_FP32 / _BF16, include/melgan_b200.h
+
+
+def _precision(precision):
+    """The C code of an inference precision: "fp32" (three bf16 passes per product, fp32-equivalent audio) or "bf16"
+    (one pass; the accuracy contract is at mg_gen_forward_precision in include/melgan_b200.h)."""
+    if not isinstance(precision, str) or precision not in PRECISIONS:
+        raise EngineError("precision must be one of %s (got %r)" % (", ".join(map(repr, PRECISIONS)), precision))
+    return PRECISIONS[precision]
 
 
 class _StatusWatch:
@@ -273,8 +290,11 @@ class GeneratorDevice:
             self._ws = self.torch.empty((need + 3) // 4, dtype=self.torch.float32, device=self.device)
         return self._ws
 
-    def forward(self, mel, out=None):
+    def forward(self, mel, out=None, precision="fp32"):
+        """mel [B, 80, T] -> audio [B, 1, 256 T].  precision "fp32" (the default) or "bf16" (one bf16 pass per tensor-core
+        product: inference only, contract at mg_gen_forward_precision in include/melgan_b200.h)."""
         torch = self.torch
+        code = _precision(precision)
         if mel.dim() != 3 or mel.shape[1] != 80:
             raise EngineError("mel must be [B, 80, T], got %s" % (tuple(mel.shape),))
         if mel.device != self.device or mel.dtype != torch.float32:
@@ -287,17 +307,22 @@ class GeneratorDevice:
         ws = self.workspace(B, T)
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            check(lib().mg_gen_forward(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T,
-                                       ws.data_ptr(), ws.numel() * 4, stream))
+            if code == 0:
+                check(lib().mg_gen_forward(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T,
+                                           ws.data_ptr(), ws.numel() * 4, stream))
+            else:
+                check(lib().mg_gen_forward_precision(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, None, code,
+                                                     ws.data_ptr(), ws.numel() * 4, stream))
             off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4  # the status word sits after the activation buffers
             self._watch.arm(ws.view(torch.int32)[off:off + 1])
         return out
 
-    def forward_ragged(self, mel, lengths, out=None):
+    def forward_ragged(self, mel, lengths, out=None, precision="fp32"):
         """Ragged batch (inference): mel [B, 80, T_max] with item i's frames [0, lengths[i]) valid (the rest is never read)
-        -> audio [B, 1, 256 T_max]; item i's first 256 lengths[i] samples equal its own forward bit for bit, the rest are 0.
-        lengths: a list, a tuple or a CPU integer tensor.  Asynchronous, like forward."""
+        -> audio [B, 1, 256 T_max]; item i's first 256 lengths[i] samples equal its own forward (at the same precision) bit
+        for bit, the rest are 0.  lengths: a list, a tuple or a CPU integer tensor.  Asynchronous, like forward."""
         torch = self.torch
+        code = _precision(precision)
         if mel.dim() != 3 or mel.shape[1] != 80:
             raise EngineError("mel must be [B, 80, T_max], got %s" % (tuple(mel.shape),))
         if mel.device != self.device or mel.dtype != torch.float32:
@@ -311,8 +336,12 @@ class GeneratorDevice:
         ws = self.workspace(B, T)
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            check(lib().mg_gen_forward_ragged(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens,
-                                              ws.data_ptr(), ws.numel() * 4, stream))
+            if code == 0:
+                check(lib().mg_gen_forward_ragged(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens,
+                                                  ws.data_ptr(), ws.numel() * 4, stream))
+            else:
+                check(lib().mg_gen_forward_precision(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens, code,
+                                                     ws.data_ptr(), ws.numel() * 4, stream))
             off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4
             self._watch.arm(ws.view(torch.int32)[off:off + 1])
         return out
@@ -730,19 +759,25 @@ class GeneratorHost:
                 lst.append(a.ctypes.data)
         check(lib().mg_gen_engine_load_state(self._h, _ptr_array(vs), _ptr_array(gs), _ptr_array(bs)))
 
-    def forward(self, mel, out=None):
+    def forward(self, mel, out=None, precision="fp32"):
+        """mel [B, 80, T] -> audio [B, 1, 256 T]; precision as for GeneratorDevice.forward."""
+        code = _precision(precision)
         mel = np.ascontiguousarray(mel, dtype=np.float32)
         B, C, T = mel.shape
         if C != 80:
             raise EngineError("mel must be [B, 80, T]")
         if out is None:
             out = np.empty((B, 1, 256 * T), np.float32)
-        check(lib().mg_gen_engine_forward(self._h, mel.ctypes.data, out.ctypes.data, B, T))
+        if code == 0:
+            check(lib().mg_gen_engine_forward(self._h, mel.ctypes.data, out.ctypes.data, B, T))
+        else:
+            check(lib().mg_gen_engine_forward_precision(self._h, mel.ctypes.data, out.ctypes.data, B, T, None, code))
         return out
 
-    def forward_ragged(self, mel, lengths, out=None):
-        """Ragged batch from host memory (mg_gen_engine_forward_ragged): mel [B, 80, T_max], lengths as for
+    def forward_ragged(self, mel, lengths, out=None, precision="fp32"):
+        """Ragged batch from host memory (mg_gen_engine_forward_ragged): mel [B, 80, T_max], lengths and precision as for
         GeneratorDevice.forward_ragged -> audio [B, 1, 256 T_max]."""
+        code = _precision(precision)
         mel = np.ascontiguousarray(mel, dtype=np.float32)
         if mel.ndim != 3 or mel.shape[1] != 80:
             raise EngineError("mel must be [B, 80, T_max]")
@@ -750,7 +785,10 @@ class GeneratorHost:
         lens = _lengths(lengths, B, T)
         if out is None:
             out = np.empty((B, 1, 256 * T), np.float32)
-        check(lib().mg_gen_engine_forward_ragged(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens))
+        if code == 0:
+            check(lib().mg_gen_engine_forward_ragged(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens))
+        else:
+            check(lib().mg_gen_engine_forward_precision(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens, code))
         return out
 
     def forward_ptr(self, mel_ptr, out_ptr, B, T):
@@ -759,11 +797,12 @@ class GeneratorHost:
 
     HALO_FRAMES = 8  # the generator's receptive field is +-7 mel frames (SURVEY section 5); 8 for slack
 
-    def stream(self, mel, chunk_frames=128):
+    def stream(self, mel, chunk_frames=128, precision="fp32"):
         """Long-utterance streaming (BASELINE config 5): yields the audio of `mel` [1, 80, T] chunk by chunk, each chunk
         computed from its frames plus an 8-frame halo either side, so latency and memory are bounded by the chunk and the
         concatenation equals the whole-utterance result (every conv of the fused stages re-applies its zero padding only
-        at the true ends, which a chunk touching an end reproduces exactly)."""
+        at the true ends, which a chunk touching an end reproduces exactly).  precision as for forward."""
+        _precision(precision)  # (a bad value is refused before any chunk is computed)
         mel = np.ascontiguousarray(mel, dtype=np.float32)
         if mel.ndim != 3 or mel.shape[0] != 1 or mel.shape[1] != 80:
             raise EngineError("stream() takes one utterance [1, 80, T]")
@@ -771,7 +810,7 @@ class GeneratorHost:
         for lo in range(0, T, chunk_frames):
             hi = min(T, lo + chunk_frames)
             a, b = max(0, lo - h), min(T, hi + h)
-            audio = self.forward(mel[:, :, a:b])
+            audio = self.forward(mel[:, :, a:b], precision=precision)
             yield audio[:, :, (lo - a) * 256:(lo - a + hi - lo) * 256]
 
     def last_kernel_ms(self):

@@ -140,15 +140,21 @@ class Generator(nn.Module):
     def _engine_forward(self, mel):
         return self._ensure_packed().forward(mel)
 
-    def generate(self, x, lengths):
-        """Vocodes a batch of utterances of different lengths in one forward (inference only: no autograd graph is built).
-        x [B, 80, T_max] fp32 CUDA, lengths: B mel lengths in [1, T_max] as a list, a tuple or a CPU integer tensor; the
-        frames past each length are never read.  Returns audio [B, 1, 256 T_max] whose item i starts with exactly the
-        256 lengths[i] samples of self(x[i:i+1, :, :lengths[i]]) and is 0 after them."""
+    def generate(self, x, lengths=None, precision="fp32"):
+        """Vocodes a batch in one forward (inference only: no autograd graph is built).  x [B, 80, T_max] fp32 CUDA.
+        lengths None: every item has T_max frames.  Otherwise B mel lengths in [1, T_max] as a list, a tuple or a CPU integer
+        tensor; the frames past each length are never read, and the audio [B, 1, 256 T_max] of item i starts with exactly
+        the 256 lengths[i] samples of generate(x[i:i+1, :, :lengths[i]], precision=precision) and is 0 after them.
+        precision "fp32" computes what self(x) computes; "bf16" runs one bf16 pass per tensor-core product (faster, audio
+        about 1e-3 from float64 in relative L2: the contract is at mg_gen_forward_precision, include/melgan_b200.h)."""
+        _engine._precision(precision)
         if not x.is_cuda:
             raise _engine.EngineError("melgan_multi_b200.Generator.generate needs a CUDA tensor (no CPU fallback)")
         with torch.no_grad():
-            return self._ensure_packed().forward_ragged(x.detach().float(), lengths)
+            dev = self._ensure_packed()
+            if lengths is None:
+                return dev.forward(x.detach().float(), precision=precision)
+            return dev.forward_ragged(x.detach().float(), lengths, precision=precision)
 
     def _graphed_recompute(self, mel, params):
         """(graphed stock-op forward+backward, mel_requires_grad) for this input shape, or None.  Cached per shape / dtype

@@ -39,6 +39,12 @@ with torch.no_grad():
     mr[2, :, 17:] = float("nan")
     yr = g.generate(mr, [5, 40, 17])
     g._dev.check_status(3, 40)
+    # the single-pass bf16 kernels (hi-only weight stream, multicast and halo exchange of the clustered stages): a uniform
+    # batch with several tiles per item, and the ragged batch
+    yb = g.generate(torch.from_numpy(synth.mel_input(1, 40, 9)).cuda(), precision="bf16")
+    g._dev.check_status(1, 40)
+    yrb = g.generate(mr, [5, 40, 17], precision="bf16")
+    g._dev.check_status(3, 40)
     m = meldataset.mel_spectrogram(y3[0, 0].clamp(-1, 1), 1024, 80, 22050, 256, 1024, 55, 9000)
 # one train.py:108-129 step on a 512-sample segment
 g.train(); d.train()
