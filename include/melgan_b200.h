@@ -210,7 +210,8 @@ int mg_disc_forward(const void *packed, const float *x, int Bt, int L, float *co
  *     norm: 0 none, 1 Slaney area normalisation (= librosa 0.6/0.7 `norm=1`, today's `norm="slaney"`), 2 L1.  The caller
  *     copies it to device memory (16-byte aligned) once.
  *   mg_mel_spectrogram: audio [B][L] device fp32 in [-1, 1] -> mel [B][n_mels][T] device fp32, T = mg_mel_frames(L)
- *     (= L / 256 when L is a multiple of 256).  Asynchronous on `stream`.
+ *     (= L / 256 when L is a multiple of 256).  Asynchronous on `stream`.  One CTA per item and pair of frames, all on
+ *     grid.x: any B works as long as B * ceil(T / 2) <= 2^31 - 1; beyond that MG_ERR_INVALID_ARGUMENT, before any launch.
  */
 size_t mg_mel_tables_bytes(void);
 int mg_mel_tables_build(int sampling_rate, int n_mels, float fmin, float fmax, int norm, void *tables_host);

@@ -8,7 +8,7 @@
 // here and in oracle/mel_oracle.py (its header says which API version the reference's call site implies, and that this row's
 // parity is UNPINNED by any reference fixture).
 //
-// One CTA = 2 frames of one batch item, 128 threads each:
+// One CTA = 2 frames of one batch item, 128 threads each (CTA c: item c / ceil(T/2), frames 2 (c mod ceil(T/2)) + {0, 1}):
 //   z[n] = w[2n] x[2n] + i w[2n+1] x[2n+1]  ->  512-point complex Stockham FFT in shared memory (fp32, table twiddles)
 //   ->  split into the 513 bins of the real 1024-point transform, magnitudes  ->  80 short dot products with the
 //   triangular mel weights (stored sparse: each filter is a contiguous run of bins)  ->  log(max(., 1e-5)).
@@ -90,7 +90,8 @@ __global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ 
     float2 *buf = reinterpret_cast<float2 *>(smem_raw + ((sizeof(MelTables) + 15) / 16) * 16);  // [2 frames][2 buffers][512]
     float *mag = reinterpret_cast<float *>(buf + 2 * 2 * 512);                                     // [2 frames][513 (+3)]
     const int tid = threadIdx.x, fr = tid >> 7, lt = tid & 127;
-    const int b = blockIdx.y, t = 2 * (int)blockIdx.x + fr;
+    const int pairs = (T + 1) >> 1;  // grid.x = items x frame pairs: a batch is not limited by grid.y's 65535
+    const int b = (int)blockIdx.x / pairs, t = 2 * ((int)blockIdx.x - b * pairs) + fr;
     for (int i = tid; i < (int)(sizeof(MelTables) / 4); i += 256) reinterpret_cast<uint32_t *>(st)[i] = reinterpret_cast<const uint32_t *>(tab)[i];
     __syncthreads();
     const bool live = t < T;
@@ -145,13 +146,16 @@ int mel_frames(int L) { return L + 2 * kMelPad < kMelNfft ? 0 : 1 + (L + 2 * kMe
 int launch_mel(const void *tables, const float *audio, float *mel, int B, int L, cudaStream_t s) {
     const int T = mel_frames(L);
     if (T < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_mel_spectrogram: %d samples are fewer than one frame", L);
+    const long long ctas = (long long)B * ((T + 1) / 2);
+    if (ctas > 0x7fffffffll)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "mg_mel_spectrogram: B=%d x %d frame pairs exceed 2^31 - 1 CTAs", B, (T + 1) / 2);
     constexpr int smem = ((sizeof(MelTables) + 15) / 16) * 16 + 2 * 2 * 512 * 8 + 2 * 516 * 4;
     static bool configured = false;
     if (!configured) {
         MG_CUDA_TRY(cudaFuncSetAttribute(mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         configured = true;
     }
-    mel_kernel<<<dim3((T + 1) / 2, B), 256, smem, s>>>(reinterpret_cast<const MelTables *>(tables), audio, mel, L, T);
+    mel_kernel<<<(unsigned)ctas, 256, smem, s>>>(reinterpret_cast<const MelTables *>(tables), audio, mel, L, T);
     MG_CUDA_TRY(cudaGetLastError());
     return MG_OK;
 }

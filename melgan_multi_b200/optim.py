@@ -63,16 +63,25 @@ class Adam(torch.optim.Optimizer):
                        p=col([p.data_ptr() for p in ps]), m=col([self.state[p]["exp_avg"].data_ptr() for p in ps]),
                        v=col([self.state[p]["exp_avg_sq"].data_ptr() for p in ps]),
                        g=torch.empty(len(ps), dtype=torch.int64, device=dev),
-                       pin=[torch.empty(len(ps), dtype=torch.int64).pin_memory() for _ in range(2)], flip=0, grads=None)
+                       pin=[torch.empty(len(ps), dtype=torch.int64).pin_memory() for _ in range(2)], uploaded=[None, None],
+                       flip=0, grads=None)
             self._tables[gi] = tab
         if tab.get("t") is None:
             tab["t"] = self._group_step(ps)  # (re)read the step count from state for a new table
         ptrs = [p.grad.data_ptr() for p in ps]  # (holding the grad tensors to compare identities would keep them alive)
         if ptrs != tab["grads"]:
-            pin = tab["pin"][tab["flip"]]
+            # The upload is asynchronous: a pinned buffer may be rewritten only once the copy that read it has run, or a
+            # host running steps ahead of the GPU would hand an earlier step's kernel a later step's gradient pointers.
+            # Each buffer keeps the event recorded after its last upload; a loop that syncs every step finds it complete.
+            i = tab["flip"]
             tab["flip"] ^= 1
+            if tab["uploaded"][i] is not None:
+                tab["uploaded"][i].synchronize()
+            pin = tab["pin"][i]
             pin.copy_(torch.tensor(ptrs, dtype=torch.int64))
             tab["g"].copy_(pin, non_blocking=True)
+            ev = tab["uploaded"][i] = tab["uploaded"][i] or torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(tab["g"].device))
             tab["grads"] = ptrs
         return tab
 

@@ -10,7 +10,8 @@ image: **librosa, unpinned** in /root/reference/requirements.txt:3.  The call si
 means *Slaney area normalisation* (each triangle scaled by 2 / (f[m+2] - f[m]); spelled `norm='slaney'` since 0.8, where
 the integer 1 became an L1 normalisation instead).  This file restates the published algorithm of that API:
   stft            librosa.core.spectrum.stft: periodic Hann (scipy.signal.get_window('hann', win_length, fftbins=True)),
-                  zero-padded/centred to n_fft, frames y[t*hop : t*hop + n_fft], rfft, complex64 result
+                  zero-padded/centred to n_fft, frames y[t*hop : t*hop + n_fft], the float64 window times the
+                  frames and rfft in float64, complex64 result
   melspectrogram  |stft| ** power, then `filters.mel(...) @ S`
   filters.mel     Slaney mel scale (htk=False): linear below 1 kHz (200/3 Hz per mel), logarithmic above (step ln(6.4)/27);
                   n_mels + 2 band edges from fmin to fmax, triangular weights on the rfft bin frequencies
@@ -41,6 +42,11 @@ def mel_to_hz(m):
 def mel_filterbank(sr, n_fft, n_mels, fmin, fmax, norm=1):
     """librosa.filters.mel of the 0.6/0.7 API.  norm: None, 1 (Slaney area normalisation), or "l1" (what the integer 1 means
     from librosa 0.8 on: every filter divided by its L1 norm)."""
+    return mel_filterbank64(sr, n_fft, n_mels, fmin, fmax, norm).astype(np.float32)
+
+
+def mel_filterbank64(sr, n_fft, n_mels, fmin, fmax, norm=1):
+    """mel_filterbank before its float32 cast: [n_mels, 1 + n_fft/2] float64."""
     fftfreqs = np.linspace(0, float(sr) / 2, 1 + n_fft // 2, endpoint=True)
     mel_f = mel_to_hz(np.linspace(hz_to_mel(fmin), hz_to_mel(fmax), n_mels + 2))
     fdiff = np.diff(mel_f)
@@ -54,21 +60,21 @@ def mel_filterbank(sr, n_fft, n_mels, fmin, fmax, norm=1):
         w *= (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None]
     elif norm == "l1":
         w /= np.maximum(np.abs(w).sum(axis=1, keepdims=True), 1e-30)
-    return w.astype(np.float32)
+    return w
 
 
 def stft_magnitude(y, n_fft, hop, win_length):
-    """|librosa.stft(y, n_fft, hop, win_length, window='hann', center=False)|: [1 + n_fft/2, frames] float32."""
+    """|librosa.stft(y, n_fft, hop, win_length, window='hann', center=False)|: [1 + n_fft/2, frames] float32.
+    As librosa does it: the float64 window times the float32 frames, the FFT in float64, the result stored as complex64."""
     n = np.arange(win_length)
-    win = 0.5 - 0.5 * np.cos(2 * np.pi * n / win_length)  # periodic Hann
+    win = 0.5 - 0.5 * np.cos(2 * np.pi * n / win_length)  # periodic Hann, float64
     if win_length < n_fft:
         lpad = (n_fft - win_length) // 2
         win = np.pad(win, (lpad, n_fft - win_length - lpad))
-    win = win.astype(np.float32)
     y = np.asarray(y, np.float32)
     frames = 1 + (len(y) - n_fft) // hop
     idx = np.arange(n_fft)[:, None] + hop * np.arange(frames)[None, :]
-    spec = np.fft.rfft(win[:, None] * y[idx], axis=0).astype(np.complex64)
+    spec = np.fft.rfft(win[:, None] * y[idx].astype(np.float64), axis=0).astype(np.complex64)
     return np.abs(spec).astype(np.float32)
 
 

@@ -313,6 +313,24 @@ def test_mel_tables_match_the_oracle_filterbank():
         ref = mo.mel_filterbank(22050, 1024, 80, 55, 9000, norm=onorm)
         assert np.abs(dense - ref).max() <= 2e-7 * max(ref.max(), 1e-30) + 1e-9, (norm, np.abs(dense - ref).max())
     assert L.mg_mel_tables_build(22050, 200, ctypes.c_float(55), ctypes.c_float(9000), 1, buf.ctypes.data_as(ctypes.c_void_p)) == -1
+    # every setting of the GPU option sweep (tests/test_mel_isolation_gpu.py) against the float64 filter bank: the sparse
+    # runs hold exactly the positive bins, and each weight is its float64 value to fp32 rounding
+    from test_mel_isolation_gpu import _option_cases, NORMS
+    for sr, n_mels, fmin, fmax, norm in _option_cases():
+        assert L.mg_mel_tables_build(sr, n_mels, ctypes.c_float(fmin), ctypes.c_float(fmax), norm, buf.ctypes.data_as(ctypes.c_void_p)) == 0
+        ib = buf.view(np.int32)
+        assert ib[2048] == n_mels
+        ks, kc, wo = ib[2049:2049 + 128], ib[2049 + 128:2049 + 256], ib[2049 + 256:2049 + 384]
+        wts = buf[2049 + 384:2049 + 384 + 1026]
+        ref = mo.mel_filterbank64(sr, 1024, n_mels, fmin, fmax, NORMS[norm])
+        dense = np.zeros((n_mels, 513))
+        for m in range(n_mels):
+            assert (kc[m] == 0) == (ref[m].max() == 0), (sr, n_mels, norm, m)   # filters that cover no bin
+            dense[m, ks[m]:ks[m] + kc[m]] = wts[wo[m]:wo[m] + kc[m]]
+        # 2 ulps of each weight (L1: rounded once to float, divided, rounded again); a bin whose float64 weight is a
+        # rounding residue (the last filter's top bin at fmax = sr/2) may differ by that residue
+        tol = 2 * 2.0 ** -24 * ref + 1e-12 * ref.max(axis=1, keepdims=True)
+        assert (np.abs(dense - ref) <= tol).all(), (sr, n_mels, fmin, fmax, norm, float((np.abs(dense - ref) / tol).max()))
     assert L.mg_mel_frames(8192) == 32 and L.mg_mel_frames(255) == 0 and L.mg_mel_frames(256) == 1 and L.mg_mel_frames(1000) == 3
     from melgan_multi_b200 import meldataset
     with pytest.raises(engine.EngineError):

@@ -1,7 +1,9 @@
 """GPU parity of the mel-spectrogram front end (csrc/mg_mel.cu through melgan_multi_b200.meldataset.mel_spectrogram, the
 drop-in for /root/reference/meldataset.py:44-55) against oracle/mel_oracle.py on the same seeded waveforms.  Tolerance: the
-reference's own pipeline is fp32 after a double-precision FFT; the kernel is fp32 throughout (table twiddles), so linear mel
-energies agree to ~1e-6 of the frame's largest band and log-mels to 1e-4 wherever they are above the clip floor."""
+oracle computes as librosa does -- the float64 window times the float32 frames, the FFT in float64, magnitudes stored as
+complex64 / float32, then a float32 filter bank; the kernel is fp32 throughout (table twiddles), so linear mel energies agree
+to ~1e-6 of the frame's largest band and log-mels to 1e-4 wherever they are above the clip floor.  The element-wise float64
+bound of every option, length and batch layout is tests/test_mel_isolation_gpu.py."""
 import numpy as np
 import pytest
 import torch
