@@ -186,6 +186,8 @@ int mg_gen_stage_output(const void *workspace, int which, float *out, int B, int
  *   maps [Bt, C_l, len] with len = lens[scale*7 + l] from mg_msd_lengths(L, lens); the first six of a scale are
  *   post-LeakyReLU, the seventh is conv_post2's raw output, i.e. the flattened logits [Bt, len].
  * status_word: >= 4 bytes of device memory; check it with mg_msd_check_status after the call (bounded waits).
+ * Bt <= 65535 (conv_pre, conv_post2 and the SIMT grouped convs put the items on grid.y / grid.z); a larger batch returns
+ *   MG_ERR_INVALID_ARGUMENT before any CUDA call: split it into calls of at most 65535 items.
  */
 size_t mg_msd_packed_bytes(void);
 int mg_msd_pack(const float *const *v, const float *const *g, const float *const *bias, void *packed, void *stream);
@@ -196,7 +198,8 @@ int mg_msd_check_status(const void *status_word, void *stream);
 /* One stand-alone Discriminator (models.py:74-103: Discriminator() called on its own, outside MultiScaleDiscriminator):
  * v, g, bias: HOST arrays of 7 DEVICE pointers (conv_pre, grouped_convs.0-3, conv_post1, conv_post2); packed: device buffer of
  * mg_disc_packed_bytes() bytes, 256-byte aligned.  x [Bt,1,L] -> fmaps: HOST array of 7 DEVICE pointers, lengths
- * lens[0..6] of mg_msd_lengths(L, lens) (the scale-0 row); fmaps[6] is the flattened logits.  status_word as above. */
+ * lens[0..6] of mg_msd_lengths(L, lens) (the scale-0 row); fmaps[6] is the flattened logits.  status_word and the
+ * Bt <= 65535 limit as above. */
 size_t mg_disc_packed_bytes(void);
 int mg_disc_pack(const float *const *v, const float *const *g, const float *const *bias, void *packed, void *stream);
 int mg_disc_forward(const void *packed, const float *x, int Bt, int L, float *const *fmaps, void *status_word, void *stream);

@@ -414,6 +414,8 @@ int mg_msd_lengths(int L, int *lens) {
 int mg_msd_forward(const void *packed, const float *y, int Bt, int L, float *const *fmaps, void *status_word, void *stream) {
     if (!packed || !y || !fmaps || !status_word || Bt < 1 || L < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_msd_forward: bad argument");
+    if (Bt > 65535)  // conv_pre, conv_post2 and the SIMT grouped convs put the items on grid.y / grid.z
+        return set_error(MG_ERR_INVALID_ARGUMENT, "mg_msd_forward: batch %d exceeds 65535 items", Bt);
     int lens[21];
     int rc = mg_msd_lengths(L, lens);
     if (rc) return rc;
@@ -434,6 +436,7 @@ int mg_disc_pack(const float *const *v, const float *const *g, const float *cons
 int mg_disc_forward(const void *packed, const float *x, int Bt, int L, float *const *fmaps, void *status_word, void *stream) {
     if (!packed || !x || !fmaps || !status_word || Bt < 1 || L < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_disc_forward: bad argument");
+    if (Bt > 65535) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_disc_forward: batch %d exceeds 65535 items", Bt);
     int lens[21];
     msd_lengths(L, lens);
     for (int i = 0; i < 7; ++i) {

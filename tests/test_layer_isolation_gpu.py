@@ -79,14 +79,14 @@ class Gen64:
         return torch.tanh(F.conv1d(F.leaky_relu(x), w, b, padding=3))
 
 
-def conv_bound_ratio(got, x64, w64, b64, stride=1, padding=0, groups=1, lrelu=False):
-    """Worst |y - y64| / (TAU A2 + 2^-20 |y64 before the activation|) of one conv (<= 1: within the bound)."""
+def conv_bound_ratio(got, x64, w64, b64, stride=1, padding=0, groups=1, lrelu=False, tau=TAU):
+    """Worst |y - y64| / (tau A2 + 2^-20 |y64 before the activation|) of one conv (<= 1: within the bound)."""
     pre = F.conv1d(x64, w64, b64, stride=stride, padding=padding, groups=groups)
     a2 = F.conv1d(x64 * x64, w64 * w64, None, stride=stride, padding=padding, groups=groups).sqrt()
     ref = F.leaky_relu(pre) if lrelu else pre
     assert got.shape == ref.shape, (tuple(got.shape), tuple(ref.shape))
     d = (got.double() - ref).abs()
-    return float((d / (TAU * a2 + REL * pre.abs()).clamp_min(1e-300)).max())
+    return float((d / (tau * a2 + REL * pre.abs()).clamp_min(1e-300)).max())
 
 
 def row_errors(got, ref):
