@@ -145,6 +145,11 @@ int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, i
  * front, 20 / 21 / 22 next ConvT fused at the tail), "resblock_tc_kernel<RbCfg<C,NRB,RPW,NCP,NSTAGE,POST,UPF,UPT,CS>>";
  * "" for an unknown code.  Tests derive the tile and cluster borders from it. */
 const char *mg_gen_resblock_config(int code);
+/* Where the packed blob keeps the split-bf16 copy of one ResBlock weight (front = 0: layer 5..28, w[co][ci][tap], tap 0..2) or
+ * of one weight of the stride-2 ConvT fused in front of stage 2 / 3 (front = 1: layer = stage, W[ci][co][tap], tap 0..3):
+ * the byte offset of half h (0 hi, 1 lo) from the start of the blob, or (size_t)-1 for an argument out of range.  Tests
+ * restate the layout the tensor-core descriptors expect against it. */
+size_t mg_gen_tc_weight_offset(int front, int layer, int co, int ci, int tap, int h);
 /* Tile geometry of the streaming ConvT kernel of stage 2 or 3, "convt_stream_tc_kernel<StreamCfg<STAGE,ROWS,MAXSEG,NSX>>":
  * ROWS input positions per tile (the batch's items concatenated with one zero row after each), at most MAXSEG item
  * segments of a tile staged by bulk copy, NSX staging slots; persistent grid of min(tiles, SMs) CTAs.  "" for stages

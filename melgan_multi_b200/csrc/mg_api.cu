@@ -391,6 +391,19 @@ int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, i
 }
 
 const char *mg_gen_resblock_config(int code) { return resblock_config_name(code, 0); }
+size_t mg_gen_tc_weight_offset(int front, int layer, int co, int ci, int tap, int h) {
+    if (h < 0 || h > 1 || co < 0 || ci < 0 || tap < 0) return (size_t)-1;
+    if (front) {
+        if (layer < 2 || layer > 3 || tap > 3) return (size_t)-1;
+        const int C = stage_cout(layer);
+        if (co >= C || ci >= 2 * C) return (size_t)-1;
+        return tc_region_start() + tc_upf_offset(layer) + 2 * upf_weight_index(C, ci, co, tap, h);
+    }
+    if (layer < 5 || layer > 28 || tap > 2) return (size_t)-1;
+    const int C = layer_shape(layer).cout;
+    if (co >= C || ci >= C) return (size_t)-1;
+    return tc_region_start() + tc_res_offset(layer) + 2 * tc_weight_index(C, co, ci, tap, h);
+}
 const char *mg_gen_convt_config(int stage) { return convt_config_name(stage); }
 
 /* ------------------------------- multi-scale discriminator ------------------------------- */

@@ -79,7 +79,19 @@ static_assert(packed_float_count() == 4524290 - 4353, "packed blob = all G param
 //   [tap][kslice = ci/KC][half: hi, lo][k-panel = (ci%KC)/8][co][ci%8]   (bf16)
 // so one (tap, kslice) chunk -- hi and lo halves back to back -- is one contiguous bulk copy, and inside a
 // half the layout is the "row-linear K-major" operand layout of mg_tc.cuh with rows = output channels.
+// C <= 64 (tc_stacked; stages 2 and 3 and their fused front ConvT below): the halves are interleaved per k-panel,
+//   [tap][kslice][k-panel][half: hi, lo][co][ci%8]
+// so the 2 C rows of a k-panel -- hi rows [0, C), lo rows [C, 2 C) -- are one operand of N = 2 C with a panel pitch
+// (LBO) of 2 C * 16 bytes: one MMA multiplies the activations by [wh | wl], and the same descriptor at N = C reads wh
+// alone.  Chunk size, chunk order and every offset below are the same for both layouts.
 MG_HD constexpr int tc_kc(int C) { return C >= 128 ? 4096 / C : C; }          // 256:16, 128:32, 64:64, 32:32
+MG_HD constexpr bool tc_stacked(int C) { return C <= 64; }
+// bf16 element index inside a chunk of KC input channels x C output rows
+MG_HD constexpr size_t tc_in_chunk_index(int C, int co, int cik, int h) {  // cik = ci % KC
+    const int KC = tc_kc(C);
+    return tc_stacked(C) ? (((size_t)(cik / 8) * 2 + h) * C + co) * 8 + (cik % 8)
+                         : (((size_t)h * (KC / 8) + cik / 8) * C + co) * 8 + (cik % 8);
+}
 MG_HD constexpr int tc_chunk_bytes(int C) { return 4 * C * tc_kc(C); }          // hi + lo halves
 MG_HD constexpr int tc_chunks_per_conv(int C) { return 3 * C / tc_kc(C); }
 MG_HD constexpr size_t tc_conv_bytes(int C) { return (size_t)12 * C * C; }
@@ -123,7 +135,8 @@ MG_HD constexpr size_t tc_pre_offset() { return tc_up_offset(4); }
 MG_HD constexpr size_t tc_pre_bytes() { return (size_t)kMelBins * kPreCout * kPreK * 4; }
 // ---- stride-2 ConvT fused into the ResBlock kernel (stages 2, 3; mg_res_tc.cu, UPF): the four taps W_k[co][ci] are four
 // "conv taps" over the 2C input channels, chunked exactly like a ResBlock conv of C output channels:
-//   [tap k][kslice = ci/KC][half: hi, lo][k-panel = (ci%KC)/8][co][ci%8]   (bf16), chunk = tc_chunk_bytes(C)
+//   [tap k][kslice = ci/KC][k-panel = (ci%KC)/8][half: hi, lo][co][ci%8]   (bf16), chunk = tc_chunk_bytes(C)
+// (C = 64 and 32: the stacked in-chunk order of tc_in_chunk_index)
 MG_HD constexpr int upf_chunks(int C) { return 4 * (2 * C / tc_kc(C)); }
 MG_HD constexpr size_t upf_bytes(int stage) { return (size_t)upf_chunks(stage_cout(stage)) * tc_chunk_bytes(stage_cout(stage)); }
 MG_HD constexpr size_t tc_upf_offset(int stage) {  // stage 2 or 3; bytes from the start of the TC region
@@ -131,7 +144,7 @@ MG_HD constexpr size_t tc_upf_offset(int stage) {  // stage 2 or 3; bytes from t
 }
 MG_HD constexpr size_t upf_weight_index(int C, int ci, int co, int k, int h) {  // bf16 element index in the stage's block
     const int KC = tc_kc(C);
-    return ((((size_t)(k * (2 * C / KC) + ci / KC) * 2 + h) * (KC / 8) + (ci % KC) / 8) * C + co) * 8 + (ci % 8);
+    return (size_t)(k * (2 * C / KC) + ci / KC) * (2 * KC * C) + tc_in_chunk_index(C, co, ci % KC, h);
 }
 MG_HD constexpr size_t tc_region_bytes() { return tc_upf_offset(3) + upf_bytes(3); }
 MG_HD constexpr size_t packed_total_bytes() { return ((packed_float_count() * 4 + 255) / 256) * 256 + tc_region_bytes(); }
@@ -139,7 +152,7 @@ MG_HD constexpr size_t tc_region_start() { return ((packed_float_count() * 4 + 2
 // element (bf16) index of w[co][ci][tap] (half h) inside its conv's TC block
 MG_HD constexpr size_t tc_weight_index(int C, int co, int ci, int tap, int h) {
     const int KC = tc_kc(C);
-    return ((((size_t)(tap * (C / KC) + ci / KC) * 2 + h) * (KC / 8) + (ci % KC) / 8) * C + co) * 8 + (ci % 8);
+    return (size_t)(tap * (C / KC) + ci / KC) * (2 * KC * C) + tc_in_chunk_index(C, co, ci % KC, h);
 }
 
 // =========================================================================================================

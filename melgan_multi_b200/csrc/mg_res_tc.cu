@@ -15,7 +15,9 @@
 //   smem   ring of weight chunks (one (tap, K-slice) of [Cout x KC] hi+lo per chunk), filled by 1-D bulk TMA
 //               copies from the pre-packed blob (mg_layout.h), released by the consumers once their MMAs have read it.
 // GEMM view of one conv: D[pos, co] (+)= sum_tap sum_pass X_pass[pos + (tap-1)*d, :] * W_pass[tap][co, :]^T with
-// M = 64 positions per instruction, N = NCW, K = 16; passes (xh,wh), (xl,wh), (xh,wl).
+// M = 64 positions per instruction, N = NCW, K = 16; passes (xh,wh), (xl,wh), (xh,wl).  At C <= 64 an instruction of
+// N = NCW reads more operand bytes per clock than shared memory delivers, so there the weights are stacked [wh | wl]
+// along N: xh * [wh | wl] is one MMA of N = 2 NCW and the activations are read twice per k-step, not three times.
 // c2 accumulates straight onto R, so the residual add costs nothing; conv biases are added when the accumulator
 // is read back (b2 is carried in `pend`).  Positions outside [0, L) are written as zeros into X after every conv,
 // which is the per-layer zero padding of the reference.
@@ -39,7 +41,7 @@
 // dot products of x[L-1] with the tap-1 weights -- are computed in fp32 by the CTA that owns position L - 1.
 // Bf16<Cfg> (mg_tc.cuh; the default chain's Rb0, Rb1, Rb2 and Up3Rb3Post): the same kernel with one pass (xh, wh) per
 // product -- in the convs and the front ConvT's taps --, X and the front ConvT operand written as hi only, the weight
-// ring filled with the hi half of each chunk and the cluster halo exchange sending the hi k-panels only.  The fp32 parts
+// ring filled with the hi half of each chunk (C <= 64: the whole stacked chunk, of which only the hi rows are read) and the cluster halo exchange sending the hi k-panels only.  The fp32 parts
 // (residual stream, biases, conv_post epilogue) are unchanged.
 #include <stdlib.h>
 #include <string.h>
@@ -124,7 +126,19 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     // writes or reads Xl nor the lo half of a weight chunk
     constexpr bool ONE = Cfg::ONEPASS;
     constexpr int NPASS = ONE ? 1 : 3;
-    constexpr uint32_t WBYTES = ONE ? Cfg::HALF : CHUNK;  // bytes of a ResBlock / front-ConvT weight chunk brought in
+    // C <= 64: a weight chunk holds [hi | lo] rows per k-panel (mg_layout.h, tc_stacked).  Where a second accumulator is
+    // free the three passes become two MMAs per k-step -- xh * [wh | wl] as one instruction of N = 2 NCW into an
+    // accumulator pair (main, lo), then xl * wh of N = NCW onto main -- so the A operand is read from shared memory twice
+    // instead of three times; the pair is added when the accumulator is read back.  That is every c2 (lo = D, dead between
+    // its hand-off and the next c1) and the front ConvT's taps at RPW >= 2 (lo = row block 1 of R / D).  A c1 has R and D
+    // live and would need a third accumulator: 3 * RPW * NA = 96 registers, which is all a thread of these 17-warp CTAs
+    // can have (ptxas spills 1.6 - 2.8 KB per thread), so the c1 convs keep three passes, on the same chunks.
+    // WLO: bytes from a k-panel's hi rows to its lo rows, WKP: k-panel pitch.
+    constexpr bool STK = tc_stacked(C), PAIR = STK && !ONE;
+    constexpr uint32_t WLO = STK ? C * 16 : Cfg::HALF, WKP = STK ? 2 * C * 16 : C * 16;
+    static_assert(!STK || NCP == 1, "stacked weights: one column part");
+    // bytes of a ResBlock / front-ConvT weight chunk brought in (single pass: the hi half where it is contiguous)
+    constexpr uint32_t WBYTES = ONE && !STK ? Cfg::HALF : CHUNK;
     static_assert(!ONE || Cfg::UPT == 0, "the single-pass variant has no tail ConvT");
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *Xh = smem, *Xl = smem + XBYTES, *ring = smem + 2 * XBYTES;
@@ -202,7 +216,9 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     __syncthreads();
     if constexpr (CS > 1) cluster_sync();  // every CTA's barriers are initialised before any remote access
     // optional timeline of one interior CTA (clock64 stamps of thread 0; see mg_gen_resblock_trace); per conv c = 0..5 the
-    // slots 2 + 3c (X handed over), 3 + 3c (accumulator ready), 4 + 3c (next X written) are 2 + 6j .. 7 + 6j of conv pair j
+    // slots 2 + 3c (X handed over), 3 + 3c (accumulator ready), 4 + 3c (next X written) are 2 + 6j .. 7 + 6j of conv pair j;
+    // front ConvT: 21 (operand in shared memory), 22 (its MMAs done), 23 (R read back from the staging buffer); conv_post
+    // epilogue: 24 (start), 26 (per-tap sums parked), 25 (audio stored)
     const bool tr = trace && blockIdx.x == (gridDim.x > 1 ? 1u : 0u) && tid == 0;
 #define MG_TR(slot) do { if (tr) trace[slot] = clock64(); } while (0)
 
@@ -210,7 +226,8 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         // ================= TMA producer: streams the weight chunks through the ring in consumption order =================
         // (clusters: chunk j is read from L2 once, by rank j % CS, and multicast into the same slot of every CTA; each
         // producer still posts its own CTA's expected bytes, after its empty[s] has seen every consumer of the cluster.
-        // Single pass: only the first WBYTES = HALF bytes of a chunk, its hi half, are sent and expected.)
+        // Single pass: only the first WBYTES = HALF bytes of a chunk, its hi half, are sent and expected; of a stacked chunk,
+        // whose hi rows are not contiguous, all of it.)
         if (lane == 0) {
             int s = 0, ph = 0, j = 0;
             bool ok = true;
@@ -243,7 +260,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     // ================= consumer warpgroups: rows of blocks [rb0, rb0 + RPW), columns [c0, c0 + NCW) =================
     const int wgi = warp >> 2, t = tid & 127, q = lane & 3;
     const int rb0 = (wgi / NCP) * RPW, c0 = (wgi % NCP) * NCW;
-    const uint64_t adesc_t = desc_template(XPITCH, 128), bdesc_t = desc_template(C * 16, 128);
+    const uint64_t adesc_t = desc_template(XPITCH, 128), bdesc_t = desc_template(WKP, 128);
     const uint32_t xh_addr = smem_u32(Xh), xl_addr = smem_u32(Xl), ring_addr = smem_u32(ring);
     float R[RPW][NA], D[RPW][NA];
     int s = 0, ph = 0, ps = -1;
@@ -357,34 +374,67 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         if constexpr (CS > 1) send_halo();
         ++hand;
     };
-    // one conv: every chunk (tap, K-slice) x NPASS passes x KC/16 k-steps x RPW row blocks
+    // one conv: every chunk (tap, K-slice) x NPASS passes x KC/16 k-steps x RPW row blocks.  Stacked weights, c2
+    // (!fresh; a literal at both call sites): the accumulator pair is (D, R) -- D, started from zero, takes the wh
+    // products and R, on top of the residual, the xh * wl^T ones -- and D is added to R once the MMAs are done.  D comes
+    // first in the pair because a c1 and the xl * wh pass use it alone: ptxas keeps MMAs asynchronous only if such an
+    // accumulator is the leading part of every wider one it belongs to.
     auto conv_mma = [&](float (&A)[RPW][NA], int dil, bool fresh, int conv) {
+        float (&Hi)[RPW][NA] = D;
+        const bool pair = PAIR && !fresh;
         if constexpr (CS > 1) {  // the neighbours' border rows of this conv's input are in the slack rows
             MG_TR(88 + 2 * conv);
             ok &= mbar_wait(hfull, conv & 1);
             MG_TR(89 + 2 * conv);
         }
         MG_TR(64 + 3 * conv);
+        if (pair) {
+#pragma unroll
+            for (int r = 0; r < RPW; ++r)
+#pragma unroll
+                for (int j = 0; j < NA; ++j) Hi[r][j] = 0.f;
+        }
 #pragma unroll 1
         for (int ch = 0; ch < Cfg::NCHUNK; ++ch) {
             const int tap = ch / KSL, ks = ch % KSL;
             const uint64_t bbase = desc_at(bdesc_t, chunk_begin() + c0 * 16);
             if (ch == 0) MG_TR(65 + 3 * conv);
             const uint32_t arow = (SLACK + rb0 * 64 + (tap - 1) * dil) * 16 + ks * (KC / 8) * XPITCH;
-#pragma unroll
-            for (int pass = 0; pass < NPASS; ++pass)
+            if (pair) {
 #pragma unroll
                 for (int k16 = 0; k16 < KC / 16; ++k16) {
-                    const uint64_t bdesc = bbase + (uint64_t)(((pass == 2 ? Cfg::HALF : 0) + 2 * k16 * (C * 16)) >> 4);
-                    const uint64_t adesc = desc_at(adesc_t, (pass == 1 ? xl_addr : xh_addr) + arow + 2 * k16 * XPITCH);
+                    const uint64_t bdesc = bbase + (uint64_t)((2 * k16 * WKP) >> 4);
+                    const uint64_t ah = desc_at(adesc_t, xh_addr + arow + 2 * k16 * XPITCH);
+                    const uint64_t al = desc_at(adesc_t, xl_addr + arow + 2 * k16 * XPITCH);
 #pragma unroll
                     for (int r = 0; r < RPW; ++r)
-                        wgmma_bf16<NCW>(A[r], adesc + (uint64_t)(r * 64), bdesc, !(fresh && ch == 0 && pass == 0 && k16 == 0));
+                        wgmma_bf16_pair<PAIR ? 2 * NCW : 64>(Hi[r], A[r], ah + (uint64_t)(r * 64), bdesc, 1);
+#pragma unroll
+                    for (int r = 0; r < RPW; ++r) wgmma_bf16<NCW>(Hi[r], al + (uint64_t)(r * 64), bdesc, 1);
                 }
+            } else {
+#pragma unroll
+                for (int pass = 0; pass < NPASS; ++pass)
+#pragma unroll
+                    for (int k16 = 0; k16 < KC / 16; ++k16) {
+                        const uint64_t bdesc = bbase + (uint64_t)(((pass == 2 ? WLO : 0) + 2 * k16 * WKP) >> 4);
+                        const uint64_t adesc = desc_at(adesc_t, (pass == 1 ? xl_addr : xh_addr) + arow + 2 * k16 * XPITCH);
+#pragma unroll
+                        for (int r = 0; r < RPW; ++r)
+                            wgmma_bf16<NCW>(A[r], adesc + (uint64_t)(r * 64), bdesc, !(fresh && ch == 0 && pass == 0 && k16 == 0));
+                    }
+            }
             chunk_end();
         }
         MG_TR(66 + 3 * conv);
         drain();
+        if (pair) {
+#pragma unroll
+            for (int r = 0; r < RPW; ++r)
+#pragma unroll
+                for (int j = 0; j < NA; ++j) A[r][j] += Hi[r][j];
+            acc_fence2(A);  // folded here: D is free again from this point on
+        }
     };
 
     pdl_wait();  // x is the previous kernel's output (and y may still be read by it): every global access of this kernel is below
@@ -394,23 +444,34 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         const int b = item(), L = len();
         const int Lin = L >> 1, Lins = Ls >> 1, s0 = (o >> 1) - 1;  // A row i <-> input position s0 + i (o is even)
         // ---- ConvT operand: A <- split(lrelu(x_in)), 2C channels of UROWS input positions; consecutive threads take
-        // consecutive positions of one 8-channel k-panel
-#pragma unroll 1
-        for (int idx = tid; idx < UROWS * 2 * Cfg::KP; idx += NCONS) {
-            const int i = idx % UROWS, kp = idx / UROWS, sp = s0 + i;
-            const bool inr = (sp >= 0 && sp < Lin);
-            const float *xp = x + ((size_t)b * 2 * C + 8 * kp) * Lins + (inr ? sp : 0);
-            float f[8];
+        // consecutive positions of one 8-channel k-panel.  A thread's UNR rounds of 8 loads are all issued before the
+        // first is split and stored (no accumulator is live yet, so the registers are there): the loop pays one memory
+        // latency, not one per round
+        constexpr int UNIT = UROWS * 2 * Cfg::KP, UNR = (UNIT + NCONS - 1) / NCONS;
+        static_assert(UNR * 8 <= 48, "front ConvT operand: rounds held in registers");
+        float f[UNR][8];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] = inr ? lrelu(__ldg(xp + (size_t)j * Lins)) : 0.f;
+        for (int rd = 0; rd < UNR; ++rd) {
+            const int idx = tid + rd * NCONS, i = idx % UROWS, kp = idx / UROWS, sp = s0 + i;
+            const bool inr = (idx < UNIT && sp >= 0 && sp < Lin);
+            const float *xp = x + ((size_t)b * 2 * C + 8 * kp) * Lins + (inr ? sp : 0);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[rd][j] = inr ? __ldg(xp + (size_t)j * Lins) : 0.f;
+        }
+#pragma unroll
+        for (int rd = 0; rd < UNR; ++rd) {
+            const int idx = tid + rd * NCONS, i = idx % UROWS, kp = idx / UROWS;
             uint32_t h[4], l[4];
 #pragma unroll
-            for (int e = 0; e < 4; ++e) split2_bf16(f[2 * e], f[2 * e + 1], h[e], l[e]);
-            *reinterpret_cast<uint4 *>(Xh + kp * UPITCH + i * 16) = make_uint4(h[0], h[1], h[2], h[3]);
-            if constexpr (!ONE) *reinterpret_cast<uint4 *>(Xl + kp * UPITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
+            for (int e = 0; e < 4; ++e) split2_bf16(lrelu(f[rd][2 * e]), lrelu(f[rd][2 * e + 1]), h[e], l[e]);
+            if (idx < UNIT) {
+                *reinterpret_cast<uint4 *>(Xh + kp * UPITCH + i * 16) = make_uint4(h[0], h[1], h[2], h[3]);
+                if constexpr (!ONE) *reinterpret_cast<uint4 *>(Xl + kp * UPITCH + i * 16) = make_uint4(l[0], l[1], l[2], l[3]);
+            }
         }
         fence_proxy_async();
         sync_cons();
+        MG_TR(21);
         // ---- ConvT MMAs: pair block wgi % NPB (warpgroups beyond NPB repeat a block and discard it: the MMA stream stays
         // free of divergent branches); odd taps feed the even outputs (R), even taps the odd ones (D)
         const uint64_t udesc_t = desc_template(UPITCH, 128);
@@ -426,7 +487,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                 for (int pass = 0; pass < NPASS; ++pass)
 #pragma unroll
                     for (int k16 = 0; k16 < KC / 16; ++k16) {
-                        const uint64_t bdesc = bbase + (uint64_t)(((pass == 2 ? Cfg::HALF : 0) + 2 * k16 * (C * 16)) >> 4);
+                        const uint64_t bdesc = bbase + (uint64_t)(((pass == 2 ? WLO : 0) + 2 * k16 * WKP) >> 4);
                         const uint64_t adesc = desc_at(udesc_t, (pass == 1 ? xl_addr : xh_addr) + arow + 2 * k16 * UPITCH);
                         wgmma_bf16<NCW>(A[0], adesc, bdesc, !(k < 2 && ks == 0 && pass == 0 && k16 == 0));
                     }
@@ -438,6 +499,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         upf_tap(D, 2);
         upf_tap(R, 3);
         drain();
+        MG_TR(22);
         sync_cons();  // every ConvT MMA has read the operand: the region becomes the fp32 staging buffer [c][p]
         float *stg = reinterpret_cast<float *>(Xh);
         const float *ubias = cst + Cfg::CB_UPF;
@@ -465,6 +527,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
                 R[r][j] = stg[(size_t)frag_col(q, (j & ~3) | (j & 1)) * SPITCH + p];
             }
         sync_cons();  // every staging read is done: the region becomes X
+        MG_TR(23);
         for (int i = tid; i < 2 * Cfg::KP * 2 * SLACK; i += NCONS) {  // zero the slack rows of Xh and Xl
             const int r = i % (2 * SLACK), kp = (i / (2 * SLACK)) % Cfg::KP, hl = i / (2 * SLACK * Cfg::KP);
             const int row = r < SLACK ? r : P + r;
@@ -515,39 +578,65 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         // (the four threads that share a row add their columns' parts), parks them in shared memory (the X buffer is dead
         // now), then audio[p] = tanh(b + sum_k q_k[p + k - 3]).
         pdl_trigger();
+        MG_TR(24);
         float *Q = reinterpret_cast<float *>(Xh);      // [7][P]
         const float *wpost = cst + Cfg::CB_POST;        // [32][8]
+        // A thread holds 8 channels of NR = 4 rows.  Channel outermost: its 7 weights and its bias are read once and
+        // applied to the four rows (per row the sum runs over the channels in the same order as row by row).
+        constexpr int NR = 2 * RPW;
+        static_assert(NR == 4, "conv_post epilogue: four rows per thread, one per lane of a quad after the reduction");
+        float qk[NR][kPostK];
+        bool inr[NR];
+        {
+            const int L = len();
 #pragma unroll
-        for (int r = 0; r < RPW; ++r)
+            for (int i = 0; i < NR; ++i) {
+                const int tp = o + (rb0 + (i >> 1)) * 64 + frag_row(t, i & 1);
+                inr[i] = (tp >= 0 && tp < L);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int p = (rb0 + r) * 64 + frag_row(t, h), tp = o + p;
-                const bool inr = (tp >= 0 && tp < len());
-                float qk[kPostK];
+                for (int k = 0; k < kPostK; ++k) qk[i][k] = 0.f;
+            }
+        }
 #pragma unroll
-                for (int k = 0; k < kPostK; ++k) qk[k] = 0.f;
+        for (int k = 0; k < NCW / 8; ++k)
 #pragma unroll
-                for (int k = 0; k < NCW / 8; ++k)
+            for (int e = 0; e < 2; ++e) {
+                const int ci = frag_col(q, 4 * k + e);
+                const float pe = pend[ci];
+                const float4 w0 = *reinterpret_cast<const float4 *>(wpost + ci * 8);
+                const float4 w1 = *reinterpret_cast<const float4 *>(wpost + ci * 8 + 4);
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int ci = frag_col(q, 4 * k + e);
-                        const float a = inr ? lrelu(R[r][4 * k + 2 * h + e] + pend[ci]) : 0.f;
-                        const float4 w0 = *reinterpret_cast<const float4 *>(wpost + ci * 8);
-                        const float4 w1 = *reinterpret_cast<const float4 *>(wpost + ci * 8 + 4);
-                        qk[0] = fmaf(w0.x, a, qk[0]); qk[1] = fmaf(w0.y, a, qk[1]); qk[2] = fmaf(w0.z, a, qk[2]);
-                        qk[3] = fmaf(w0.w, a, qk[3]); qk[4] = fmaf(w1.x, a, qk[4]); qk[5] = fmaf(w1.y, a, qk[5]);
-                        qk[6] = fmaf(w1.z, a, qk[6]);
-                    }
-#pragma unroll
-                for (int k = 0; k < kPostK; ++k) {
-                    qk[k] += __shfl_xor_sync(0xffffffffu, qk[k], 1);
-                    qk[k] += __shfl_xor_sync(0xffffffffu, qk[k], 2);
-                }
-                if (q == 0) {
-#pragma unroll
-                    for (int k = 0; k < kPostK; ++k) Q[k * P + p] = qk[k];
+                for (int i = 0; i < NR; ++i) {
+                    const float a = inr[i] ? lrelu(R[i >> 1][4 * k + 2 * (i & 1) + e] + pe) : 0.f;
+                    qk[i][0] = fmaf(w0.x, a, qk[i][0]); qk[i][1] = fmaf(w0.y, a, qk[i][1]); qk[i][2] = fmaf(w0.z, a, qk[i][2]);
+                    qk[i][3] = fmaf(w0.w, a, qk[i][3]); qk[i][4] = fmaf(w1.x, a, qk[i][4]); qk[i][5] = fmaf(w1.y, a, qk[i][5]);
+                    qk[i][6] = fmaf(w1.z, a, qk[i][6]);
                 }
             }
+        // The four lanes of a quad add their parts, (q0 + q1) + (q2 + q3) per row and tap.  Each step hands half of the
+        // values to the partner lane instead of exchanging all of them: after lane ^ 1 the odd lanes keep rows 2, 3 and
+        // the even ones rows 0, 1; after lane ^ 2 lane q holds the finished sums of row 2 (q & 1) + (q >> 1) -- 21
+        // shuffles per thread instead of 56, and every lane stores one row.
+        const bool odd = q & 1, up = q & 2;
+        float s1[2][kPostK], s2[kPostK];
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int k = 0; k < kPostK; ++k) {
+                const float keep = odd ? qk[j + 2][k] : qk[j][k], send = odd ? qk[j][k] : qk[j + 2][k];
+                s1[j][k] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
+            }
+#pragma unroll
+        for (int k = 0; k < kPostK; ++k) {
+            const float keep = up ? s1[1][k] : s1[0][k], send = up ? s1[0][k] : s1[1][k];
+            s2[k] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+        }
+        {
+            const int i = 2 * (q & 1) + (q >> 1), p = (rb0 + (i >> 1)) * 64 + frag_row(t, i & 1);
+#pragma unroll
+            for (int k = 0; k < kPostK; ++k) Q[k * P + p] = s2[k];
+        }
+        MG_TR(26);
         sync_cons();
         const int b = item(), L = len();
         const float bpost = cst[Cfg::CB_POST + 32 * 8];
@@ -566,6 +655,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         }
         if (oc + P >= L)  // the item's last CTA: the audio past the item's end reads 0 (ragged batches)
             for (int p = L + tid; p < Ls; p += NCONS) y[(size_t)b * Ls + p] = 0.f;
+        MG_TR(25);
     } else if constexpr (Cfg::UPT != 0) {
         // ---- tail ConvT: D[s, phi*TNG + co] (+)= X[s - tap, :] * Wstack_tap^T over the C channels of X = split(lrelu(x_out))
         constexpr int S = Cfg::UPT, TNG = Cfg::TNG, TN = Cfg::TN, PADT = S / 2, COT = C / 2;

@@ -179,6 +179,27 @@ template <> __device__ __forceinline__ void wgmma_bf16<256>(float *d, uint64_t a
                  : MG_D8(0), MG_D8(8), MG_D8(16), MG_D8(24), MG_D8(32), MG_D8(40), MG_D8(48), MG_D8(56), MG_D8(64), MG_D8(72), MG_D8(80), MG_D8(88), MG_D8(96), MG_D8(104), MG_D8(112), MG_D8(120)
                  : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
+// The same instruction with its accumulator in two register arrays: columns [0, N/2) in d0[0 .. N/4), columns [N/2, N) in
+// d1[0 .. N/4).  With B = [wh | wl] stacked along N (mg_layout.h, tc_stacked) one MMA leaves x * wh^T in d0 and x * wl^T
+// in d1; scale_d applies to both.
+template <int N>
+__device__ __forceinline__ void wgmma_bf16_pair(float *d0, float *d1, uint64_t adesc, uint64_t bdesc, uint32_t scale_d);
+#define MG_E8(i) "+f"(d1[i]), "+f"(d1[i + 1]), "+f"(d1[i + 2]), "+f"(d1[i + 3]), "+f"(d1[i + 4]), "+f"(d1[i + 5]), "+f"(d1[i + 6]), "+f"(d1[i + 7])
+template <> __device__ __forceinline__ void wgmma_bf16_pair<64>(float *d0, float *d1, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    float *d = d0;
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : MG_D8(0), MG_D8(8), MG_E8(0), MG_E8(8)
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16_pair<128>(float *d0, float *d1, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    float *d = d0;
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : MG_D8(0), MG_D8(8), MG_D8(16), MG_D8(24), MG_E8(0), MG_E8(8), MG_E8(16), MG_E8(24)
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+#undef MG_E8
 #undef MG_D8
 
 // ---- bf16 hi/lo split ----------------------------------------------------------------------------
@@ -201,7 +222,8 @@ __device__ __forceinline__ void split2_bf16(float x0, float x1, uint32_t &hi, ui
 // ---- single-pass bf16 variant of a kernel configuration (mg_gen_forward_precision, MG_GEN_PRECISION_BF16) ----------
 // The same tiles, shared-memory layout and packed blob as Cfg, but one pass (xh, wh) per product with fp32 accumulation:
 // the converters store only the hi operand, and only the hi half of each weight chunk / slot is brought in (the lo half
-// of the blob and the Xl / lo regions of shared memory are left unused).  A distinct type, so the instantiations have
+// of the blob and the Xl / lo regions of shared memory are left unused; a stacked chunk, mg_layout.h tc_stacked, comes in
+// whole and its lo rows are skipped by the descriptor).  A distinct type, so the instantiations have
 // kernel symbols of their own ("resblock_tc_kernel<mg::tc::Bf16<mg::RbCfg<...>>>") in a profiler trace.
 template <class Cfg>
 struct Bf16 : Cfg {
