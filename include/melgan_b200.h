@@ -113,6 +113,52 @@ int mg_gen_forward_ragged(const void *packed, const float *mel, float *audio, in
 int mg_gen_forward_precision(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
                              int precision, void *workspace, size_t workspace_bytes, void *stream);
 
+/* Streaming vocoder: many live sessions, mel frames pushed a few at a time, each audio sample emitted once it is final.
+ * A handle serves up to max_sessions (<= MG_GEN_RAGGED_MAX_B) slots at one precision.  Each mg_gen_stream_step gives slot i
+ * (i < n) a push of frames[i] in [0, max_push_frames] new mel frames and flags[i] (flags NULL: all 0):
+ *   MG_GEN_STREAM_RESET  drop the slot's unfinished utterance before these frames;
+ *   MG_GEN_STREAM_END    the utterance ends after these frames (END on a slot with no frames is MG_ERR_INVALID_ARGUMENT).
+ * and writes the slot's newly final audio samples to audio[i][0 .. out_samples[i]):
+ *   - open utterance of t frames in total: exactly max(0, 256 t - mg_gen_stream_lookahead()) samples have been emitted
+ *     over all its steps (the look-ahead, 1542 samples = 70 ms at 22.05 kHz, is the default chain's right-hand receptive
+ *     field; sample j depends on no frame past (j + 1542) / 256);
+ *   - after the END step all 256 t samples have been emitted; the slot is then free and its next push starts a new
+ *     utterance;
+ *   - the concatenation of an utterance's outputs is bit-identical to mg_gen_forward_precision of its whole mel (T = t,
+ *     same precision, default chain) for any push schedule, 0- and 1-frame pushes included.
+ * out_samples is a HOST array filled before the call returns: the step derives every count and launch shape from frame
+ * counts alone, enqueues its work asynchronously on `stream` and never synchronises or reads the device.
+ * Arguments:
+ *   mel   [n][80][max_push_frames] device fp32; slot i's frames are mel[i][:][0 .. frames[i]) (the rest is never read);
+ *         may be NULL when every frames[i] is 0
+ *   audio [n][mg_gen_stream_max_out(max_push_frames)] device fp32; only audio[i][0 .. out_samples[i]) is written
+ *   packed: the weights of mg_gen_pack (may be re-packed between steps: each step reads them anew)
+ *   state: caller-owned device memory of mg_gen_stream_state_bytes(max_sessions, max_push_frames) bytes, 256-byte aligned,
+ *          for the lifetime of the handle and not shared with another handle.  It holds each session's cached left context
+ *          at every kernel boundary, the kernels' windows and the status word.  No step lets a byte that an earlier step
+ *          has not written reach an output, so its initial contents do not matter.
+ * Every argument is checked before any CUDA call.  On a chain other than the default one (mg_gen_set_pipeline,
+ * MG_GEN_TAIL, MG_GEN_FUSE_UP) create and step return MG_ERR_INVALID_ARGUMENT.  One thread drives a handle at a time;
+ * steps of one handle must be enqueued on one stream (or otherwise ordered).  mg_gen_stream_check_status waits for `stream`
+ * and reports a timed-out tensor-core pipeline wait of any step so far. */
+#define MG_GEN_STREAM_END 1
+#define MG_GEN_STREAM_RESET 2
+typedef struct mg_gen_stream mg_gen_stream; /* host-side counters only */
+int mg_gen_stream_lookahead(void);
+size_t mg_gen_stream_state_bytes(int max_sessions, int max_push_frames);
+int mg_gen_stream_max_out(int max_push_frames); /* 256 max_push_frames + mg_gen_stream_lookahead() */
+int mg_gen_stream_create(mg_gen_stream **out, int max_sessions, int max_push_frames, int precision, void *state, size_t state_bytes);
+void mg_gen_stream_destroy(mg_gen_stream *s);
+int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, const int *frames, const int *flags, int n, float *audio,
+                       int *out_samples, void *stream);
+int mg_gen_stream_check_status(mg_gen_stream *s, void *stream);
+/* Planning without a device: advances the handle's counters exactly as mg_gen_stream_step would and reports out_samples,
+ * the items each of the 8 chain kernels would run (kernel_items[8], may be NULL) and the bytes the window-assembly and
+ * audio copies would read and write (copy_bytes, may be NULL).  No CUDA call.  A handle advanced this way refuses later
+ * real steps. */
+int mg_gen_stream_dry_step(mg_gen_stream *s, const int *frames, const int *flags, int n, int *out_samples, int *kernel_items,
+                           long long *copy_bytes);
+
 /* Same as mg_gen_forward, but brackets each of the mg_gen_forward_launches() kernels with CUDA
  * events on `stream`, waits for the last one and returns the per-kernel device times in
  * kernel_ms[0 .. mg_gen_forward_launches()-1] (names: mg_gen_kernel_name(i)).  Used by bench.py for the

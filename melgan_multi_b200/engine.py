@@ -153,6 +153,22 @@ def lib():
         L.mg_gen_engine_last_kernel_ms.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_float)]
         L.mg_gen_engine_destroy.restype = None
         L.mg_gen_engine_destroy.argtypes = [ctypes.c_void_p]
+        L.mg_gen_stream_lookahead.restype = ctypes.c_int
+        L.mg_gen_stream_state_bytes.restype = ctypes.c_size_t
+        L.mg_gen_stream_state_bytes.argtypes = [ctypes.c_int, ctypes.c_int]
+        L.mg_gen_stream_max_out.restype = ctypes.c_int
+        L.mg_gen_stream_max_out.argtypes = [ctypes.c_int]
+        L.mg_gen_stream_create.restype = ctypes.c_int
+        L.mg_gen_stream_create.argtypes = [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                           ctypes.c_size_t]
+        L.mg_gen_stream_destroy.restype = None
+        L.mg_gen_stream_destroy.argtypes = [ctypes.c_void_p]
+        L.mg_gen_stream_step.restype = ctypes.c_int
+        L.mg_gen_stream_step.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_int] + [ctypes.c_void_p] * 3
+        L.mg_gen_stream_check_status.restype = ctypes.c_int
+        L.mg_gen_stream_check_status.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+        L.mg_gen_stream_dry_step.restype = ctypes.c_int
+        L.mg_gen_stream_dry_step.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int] + [ctypes.c_void_p] * 3
         _lib = L
     return _lib
 
@@ -468,6 +484,105 @@ class GeneratorDevice:
             stream = torch.cuda.current_stream().cuda_stream
             check(lib().mg_gen_stage_output(self._ws.data_ptr(), which, out.data_ptr(), B, T, stream))
         return out
+
+
+STREAM_END, STREAM_RESET = 1, 2  # MG_GEN_STREAM_END / _RESET, include/melgan_b200.h
+
+
+class GeneratorStream:
+    """Incremental vocoding of up to ``max_sessions`` live mel streams (mg_gen_stream_*, contract in
+    include/melgan_b200.h).  Each step pushes a few new frames per session and returns the audio samples that became final:
+    256 t - lookahead_samples of them after t frames, all 256 t after the step that ends the utterance, and their
+    concatenation equals Generator.generate of the whole mel bit for bit.
+
+    packed_fn: a callable returning the GeneratorDevice whose packed weights a step reads (Generator._ensure_packed, so
+    weights changed between steps are re-packed).  state: optional caller-provided uint8 CUDA tensor of at least
+    mg_gen_stream_state_bytes bytes (the stream never lets a byte it has not written reach an output)."""
+
+    def __init__(self, packed_fn, device, max_sessions=1, max_push_frames=32, precision="fp32", state=None):
+        import torch
+        self.torch = torch
+        self._packed_fn = packed_fn
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise EngineError("stream: the native engine runs on CUDA devices only (got %s)" % (device,))
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.precision = precision
+        code = _precision(precision)
+        self.max_sessions, self.max_push_frames = int(max_sessions), int(max_push_frames)
+        nbytes = lib().mg_gen_stream_state_bytes(self.max_sessions, self.max_push_frames)
+        if nbytes == 0:
+            raise EngineError("stream: max_sessions must lie in [1, 256] and max_push_frames in [1, 65536]")
+        if state is None:
+            state = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        if state.device != self.device or state.numel() * state.element_size() < nbytes or not state.is_contiguous():
+            raise EngineError("stream: state must be a contiguous CUDA tensor of at least %d bytes on %s" % (nbytes, self.device))
+        self.state = state
+        self.lookahead_samples = lib().mg_gen_stream_lookahead()
+        self.max_out = lib().mg_gen_stream_max_out(self.max_push_frames)
+        self._h = ctypes.c_void_p()
+        check(lib().mg_gen_stream_create(ctypes.byref(self._h), self.max_sessions, self.max_push_frames, code, state.data_ptr(),
+                                         state.numel() * state.element_size()))
+        self._mel = torch.zeros((self.max_sessions, 80, self.max_push_frames), dtype=torch.float32, device=self.device)
+
+    def step_packed(self, mel, frames, flags=None, audio=None):
+        """The C step on a packed buffer: mel [n, 80, max_push_frames] fp32 CUDA (slot i's frames first), frames / flags: n
+        ints.  Returns (audio [n, max_out], per-slot sample counts as a list of ints)."""
+        torch = self.torch
+        n = len(frames)
+        dev = self._packed_fn()
+        if audio is None:
+            audio = torch.empty((n, self.max_out), dtype=torch.float32, device=self.device)
+        fr = (ctypes.c_int * max(n, 1))(*[int(v) for v in frames])
+        fl = (ctypes.c_int * max(n, 1))(*[int(v) for v in flags]) if flags is not None else None
+        cnt = (ctypes.c_int * max(n, 1))()
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream().cuda_stream
+            check(lib().mg_gen_stream_step(self._h, dev.packed.data_ptr(), mel.data_ptr() if mel is not None else None, fr, fl, n,
+                                           audio.data_ptr(), cnt, stream))
+        return audio, [cnt[i] for i in range(n)]
+
+    def step(self, chunks, end=None, reset=None):
+        """chunks: one entry per slot 0 .. n-1, each a [80, n_i] fp32 CUDA tensor (0 <= n_i <= max_push_frames) or None;
+        end / reset: None or n booleans (end: the utterance ends after this chunk; reset: drop the slot's unfinished
+        utterance first).  Returns n [1, m_i] CUDA tensors of newly final audio, owned by the caller.  Asynchronous on the
+        current stream: the lengths are known on return, the values once the stream gets there."""
+        n = len(chunks)
+        if n > self.max_sessions:
+            raise EngineError("stream: %d chunks for %d sessions" % (n, self.max_sessions))
+        frames = []
+        for i, c in enumerate(chunks):
+            if c is None:
+                frames.append(0)
+                continue
+            if c.dim() != 2 or c.shape[0] != 80 or c.shape[1] > self.max_push_frames:
+                raise EngineError("stream: chunk %d must be [80, n] with n <= %d, got %s" % (i, self.max_push_frames, tuple(c.shape)))
+            if c.device != self.device or c.dtype != self.torch.float32:
+                raise EngineError("stream: chunks must be fp32 tensors on %s" % (self.device,))
+            frames.append(int(c.shape[1]))
+            if c.shape[1]:
+                self._mel[i, :, :c.shape[1]].copy_(c)
+        flags = [(STREAM_END if end is not None and end[i] else 0) | (STREAM_RESET if reset is not None and reset[i] else 0)
+                 for i in range(n)]
+        audio, counts = self.step_packed(self._mel, frames, flags)
+        return [audio[i:i + 1, :m] for i, m in enumerate(counts)]
+
+    def check_status(self):
+        """Synchronises and raises if a tensor-core pipeline wait of any step so far timed out."""
+        with self.torch.cuda.device(self.device):
+            check(lib().mg_gen_stream_check_status(self._h, self.torch.cuda.current_stream().cuda_stream))
+
+    def close(self):
+        if self._h:
+            lib().mg_gen_stream_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 D_CHANNELS = (16, 64, 256, 1024, 1024, 1024, 1)  # channels of the seven feature maps of one Discriminator

@@ -156,6 +156,17 @@ class Generator(nn.Module):
                 return dev.forward(x.detach().float(), precision=precision)
             return dev.forward_ragged(x.detach().float(), lengths, precision=precision)
 
+    def stream(self, max_sessions=1, max_push_frames=32, precision="fp32"):
+        """A streaming vocoder over this generator's weights (inference only): up to max_sessions live mel streams, each
+        step pushing at most max_push_frames new frames per session and returning the audio samples that became final
+        (engine.GeneratorStream; the concatenation of a session's outputs equals generate() of its whole mel bit for bit).
+        Weights changed between steps are re-packed, as in generate."""
+        vs, _, _ = self._param_triplets()
+        if vs[0].device.type != "cuda":
+            raise _engine.EngineError("melgan_multi_b200.Generator.stream needs the module on CUDA (no CPU fallback)")
+        self._ensure_packed()
+        return _engine.GeneratorStream(self._ensure_packed, vs[0].device, max_sessions, max_push_frames, precision)
+
     def _graphed_recompute(self, mel, params):
         """(graphed stock-op forward+backward, mel_requires_grad) for this input shape, or None.  Cached per shape / dtype
         policy; the graphs own static copies of nothing but activations -- parameters are call arguments."""
