@@ -191,16 +191,37 @@ int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, i
  * front, 20 / 21 / 22 next ConvT fused at the tail), "resblock_tc_kernel<RbCfg<C,NRB,RPW,NCP,NSTAGE,POST,UPF,UPT,CS>>";
  * "" for an unknown code.  Tests derive the tile and cluster borders from it. */
 const char *mg_gen_resblock_config(int code);
-/* Where the packed blob keeps the split-bf16 copy of one ResBlock weight (front = 0: layer 5..28, w[co][ci][tap], tap 0..2) or
- * of one weight of the stride-2 ConvT fused in front of stage 2 / 3 (front = 1: layer = stage, W[ci][co][tap], tap 0..3):
- * the byte offset of half h (0 hi, 1 lo) from the start of the blob, or (size_t)-1 for an argument out of range.  Tests
- * restate the layout the tensor-core descriptors expect against it. */
+/* Where the packed blob keeps the split-bf16 copy of one tensor-core weight: the byte offset of half h (0 hi, 1 lo) from the
+ * start of the blob, or (size_t)-1 for an argument out of range.
+ *   front = 0, layer 0: conv_pre, w[co][ci][tap], tap 0..6;
+ *   front = 0, layer 1..4: ups[layer - 1], W[ci][co][tap] (the ConvTranspose1d layout), tap 0 .. 2 S - 1;
+ *   front = 0, layer 5..28: a ResBlock conv, w[co][ci][tap], tap 0..2;
+ *   front = 1, layer = stage 2 / 3: the stride-2 ConvT fused in front of that stage's ResBlock, W[ci][co][tap], tap 0..3.
+ * Tests restate the layout the tensor-core descriptors expect against it. */
 size_t mg_gen_tc_weight_offset(int front, int layer, int co, int ci, int tap, int h);
-/* Tile geometry of the streaming ConvT kernel of stage 2 or 3, "convt_stream_tc_kernel<StreamCfg<STAGE,ROWS,MAXSEG,NSX>>":
- * ROWS input positions per tile (the batch's items concatenated with one zero row after each), at most MAXSEG item
- * segments of a tile staged by bulk copy, NSX staging slots; persistent grid of min(tiles, SMs) CTAs.  "" for stages
- * 0 and 1.  Tests derive tile borders from it. */
+/* Tile geometry of the ConvT kernel launch_convt_tc runs for `stage`; tests derive tile borders from it.  A tile is ROWS
+ * input positions of the batch's items concatenated with one zero row after each.
+ *   stage 0: "convt_tc_kernel<UpCfg<0,ROWS,NG>>", one CTA per (tile, group of NG output channels);
+ *   stage 1: "convt_resident_tc_kernel<UpCfg<1,ROWS,NG>>", one CTA per tile, looping over the groups of NG channels;
+ *   stage 2 / 3: "convt_stream_tc_kernel<StreamCfg<STAGE,ROWS,MAXSEG,NSX>>": at most MAXSEG item segments of a tile staged
+ *   by bulk copy, NSX staging slots; persistent grid of min(tiles, SMs) CTAs.
+ * "" for any other stage. */
 const char *mg_gen_convt_config(int stage);
+/* conv_pre's tile geometry, "conv_rows_tc_kernel<ConvCfg<80,512,7,ROWS,N>>": ROWS virtual rows per CTA (each item's
+ * positions followed by 3 zero rows), N output channels per CTA. */
+const char *mg_gen_conv_pre_config(void);
+/* Kernel k (0..7) of the default chain alone -- 0 conv_pre, 1 up0, 2 res0, 3 up1, 4 res1, 5 up2, 6 res2, 7 up3+res3+post --
+ * as mg_gen_forward_precision and mg_gen_stream_step launch it, on a batch of B <= MG_GEN_RAGGED_MAX_B items:
+ *   x [B][Cin][L_max] -> y [B][Cout][R L_max], device fp32, 16-byte aligned, x != y, where (Cin, Cout, R) is
+ *   (80, 512, 1), (512, 256, 8), (256, 256, 1), (256, 128, 8), (128, 128, 1), (128, 64, 2), (64, 64, 1), (64, 1, 2) for k = 0..7;
+ *   lengths: NULL (every item L_max positions) or a HOST array of B lengths in [1, L_max], in kernel k's input units.
+ * Item i reads only x[i][:][0 .. lengths[i]) (the rest may hold NaN) and writes only y[i][:][0 .. R lengths[i]), except
+ * kernel 7, which also writes 0.0 to y[i][0][R lengths[i] .. R L_max) (the ragged forward's zero audio tail).  precision:
+ * MG_GEN_PRECISION_FP32 or _BF16 (kernels 0 and 5 run three passes at either).  Every argument is checked before any CUDA
+ * call; on a chain other than the default one it returns MG_ERR_INVALID_ARGUMENT.  Synchronous, with its own status word
+ * (a timed-out pipeline wait is MG_ERR_CUDA).  Test entry point: the same launcher the stream steps use. */
+int mg_gen_chain_kernel(const void *packed, int k, const float *x, float *y, int B, int L_max, const int *lengths, int precision,
+                        void *stream);
 
 /* ResBlock `stage` (0..2) with the NEXT stage's LeakyReLU -> ConvTranspose1d fused at its tail, as the default pipeline runs it
  * (models.py:66 followed by :64-65 of the next loop iteration): x [B][C][L] is stage `stage`'s ConvT output, y

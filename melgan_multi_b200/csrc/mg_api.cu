@@ -399,12 +399,52 @@ size_t mg_gen_tc_weight_offset(int front, int layer, int co, int ci, int tap, in
         if (co >= C || ci >= 2 * C) return (size_t)-1;
         return tc_region_start() + tc_upf_offset(layer) + 2 * upf_weight_index(C, ci, co, tap, h);
     }
-    if (layer < 5 || layer > 28 || tap > 2) return (size_t)-1;
+    if (layer < 0) return (size_t)-1;
+    if (layer == 0) {  // conv_pre, w[co][ci][tap]
+        if (co >= kPreCout || ci >= kMelBins || tap >= kPreK) return (size_t)-1;
+        return tc_region_start() + tc_pre_offset() + 2 * conv_tc_weight_index(kMelBins, kPreK, kPreNG, co, ci, tap, h);
+    }
+    if (layer <= 4) {  // ups[layer - 1], W[ci][co][tap], tap < 2 S
+        const int s = layer - 1;
+        if (co >= stage_cout(s) || ci >= stage_cin(s) || tap >= stage_kup(s)) return (size_t)-1;
+        return tc_region_start() + tc_up_offset(s) + 2 * up_weight_index(s, ci, co, tap, h);
+    }
+    if (layer > 28 || tap > 2) return (size_t)-1;
     const int C = layer_shape(layer).cout;
     if (co >= C || ci >= C) return (size_t)-1;
     return tc_region_start() + tc_res_offset(layer) + 2 * tc_weight_index(C, co, ci, tap, h);
 }
 const char *mg_gen_convt_config(int stage) { return convt_config_name(stage); }
+const char *mg_gen_conv_pre_config(void) { return gen_pre_config_name(); }
+
+int mg_gen_chain_kernel(const void *packed, int k, const float *x, float *y, int B, int L_max, const int *lengths, int precision,
+                        void *stream) {
+    const char *fn = "mg_gen_chain_kernel";
+    if (!packed || !x || !y) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
+    if (x == y) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: x and y must differ", fn);
+    if ((uintptr_t)packed % 16 || (uintptr_t)x % 16 || (uintptr_t)y % 16)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed, x and y must be 16-byte aligned", fn);
+    if (k < 0 || k > 7) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: kernel %d is outside [0, 7]", fn, k);
+    if (B < 1 || B > MG_GEN_RAGGED_MAX_B || L_max < 1)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: need 1 <= B <= MG_GEN_RAGGED_MAX_B = %d and L_max >= 1 (got B=%d, L_max=%d)", fn,
+                         MG_GEN_RAGGED_MAX_B, B, L_max);
+    if ((long long)B * L_max > (1ll << 28)) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: B*L_max too large", fn);
+    for (int i = 0; lengths && i < B; ++i)
+        if (lengths[i] < 1 || lengths[i] > L_max)
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: lengths[%d] = %d is outside [1, L_max = %d]", fn, i, lengths[i], L_max);
+    if (precision != MG_GEN_PRECISION_FP32 && precision != MG_GEN_PRECISION_BF16)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: unknown precision %d (MG_GEN_PRECISION_FP32 = 0, MG_GEN_PRECISION_BF16 = 1)", fn,
+                         precision);
+    if (!generator_tc_default_chain())
+        return set_error(MG_ERR_INVALID_ARGUMENT,
+                         "%s: runs the default chain's kernels only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected "
+                         "another (tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
+                         fn, generator_tc_tail(), generator_tc_fused_up());
+    const RunTable t = lengths ? RunTable::ragged(lengths, B, L_max) : RunTable::uniform(B, L_max);
+    return run_one_kernel(fn, (cudaStream_t)stream, [&](int *st) {
+        return launch_chain_kernel(k, x, y, (const float *)packed, t, st, (cudaStream_t)stream, precision);
+    });
+}
 
 /* ------------------------------- multi-scale discriminator ------------------------------- */
 

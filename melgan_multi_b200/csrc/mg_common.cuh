@@ -214,6 +214,10 @@ int launch_msd_forward(const void *packed, const float *y, int Bt, int L, float 
 int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
                     int precision = MG_GEN_PRECISION_FP32);
 const char *convt_config_name(int stage);
+const char *gen_pre_config_name();
+// kernel k (0..7) of the default chain; batch in kernel k's input units (mg_gen_stream.cu)
+int launch_chain_kernel(int k, const float *x, float *y, const float *w, const RunTable &t, int *status, cudaStream_t st,
+                        int precision);
 int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
                        long long *trace = nullptr, int precision = MG_GEN_PRECISION_FP32);
 

@@ -251,6 +251,14 @@ int launch_gen_pre_tc(const float *mel, float *y, const float *packed, const Run
     return launch_conv_rows<PreCfg>(mel, y, wtc, packed + bias_offset(0), rows, rows.first[rows.n], status, s);
 }
 
+// conv_pre's tile geometry: ROWS virtual rows per CTA (each item's positions followed by PAD zero rows), N output channels
+const char *gen_pre_config_name() {
+    static char buf[80];
+    snprintf(buf, sizeof(buf), "conv_rows_tc_kernel<ConvCfg<%d,%d,%d,%d,%d>>", PreCfg::CIN, PreCfg::COUT, PreCfg::NTAP, PreCfg::ROWS,
+             PreCfg::N);
+    return buf;
+}
+
 // x [Bt][1024][L] -> y [Bt][1024][L] = lrelu(conv_post1(x))   (Discriminator.conv_post1)
 int launch_disc_post1_tc(const float *x, float *y, const uint8_t *wtc, const float *bias, int Bt, int L, int *status,
                          cudaStream_t s) {

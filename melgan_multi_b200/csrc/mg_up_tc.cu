@@ -701,9 +701,20 @@ int launch_convt_tc(const float *x, float *y, const float *packed, int stage, co
     return set_error(MG_ERR_INVALID_ARGUMENT, "launch_convt_tc: stage %d", stage);
 }
 
-// the configuration launch_convt_tc runs for the stride-2 stages ("" for the others)
+// the tile geometry of a stride-8 ConvT: ROWS input positions per CTA (the batch's items concatenated with one zero row
+// after each), NG output channels per CTA (grid.y = COUT / NG for convt_tc_kernel; the resident kernel loops over them)
+template <class Cfg>
+static const char *up_cfg_name(const char *kernel) {
+    static char buf[80];
+    snprintf(buf, sizeof(buf), "%s<UpCfg<%d,%d,%d>>", kernel, Cfg::STAGE, Cfg::ROWS, Cfg::NG);
+    return buf;
+}
+
+// the configuration launch_convt_tc runs for `stage` ("" for an unknown stage)
 const char *convt_config_name(int stage) {
     switch (stage) {
+        case 0: return up_cfg_name<UpCfg<0>>("convt_tc_kernel");
+        case 1: return up_cfg_name<UpCfg<1>>("convt_resident_tc_kernel");
         case 2: return stream_cfg_name<UpCfg<2>>();
         case 3: return stream_cfg_name<UpCfg<3>>();
     }

@@ -67,6 +67,11 @@ def lib():
         L.mg_gen_resblock_config.argtypes = [ctypes.c_int]
         L.mg_gen_convt_config.restype = ctypes.c_char_p
         L.mg_gen_convt_config.argtypes = [ctypes.c_int]
+        L.mg_gen_conv_pre_config.restype = ctypes.c_char_p
+        L.mg_gen_conv_pre_config.argtypes = []
+        L.mg_gen_chain_kernel.restype = ctypes.c_int
+        L.mg_gen_chain_kernel.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                          ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
         L.mg_gen_conv_pre.restype = ctypes.c_int
         L.mg_gen_conv_pre.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
         L.mg_gen_resblock_post.restype = ctypes.c_int
@@ -461,6 +466,37 @@ class GeneratorDevice:
             stream = torch.cuda.current_stream().cuda_stream
             check(lib().mg_gen_conv_pre(self.packed.data_ptr(), mel.data_ptr(), y.data_ptr(), B, T, stream))
         return y
+
+    # kernel k of the default chain: (input channels, output channels, output positions per input position)
+    CHAIN_SHAPES = ((80, 512, 1), (512, 256, 8), (256, 256, 1), (256, 128, 8), (128, 128, 1), (128, 64, 2), (64, 64, 1), (64, 1, 2))
+
+    def chain_kernel(self, k, x, lengths=None, precision="fp32", out=None):
+        """Kernel k (0..7) of the default chain alone, as the forward and the stream launch it (mg_gen_chain_kernel):
+        x [B, Cin, L_max] -> [B, Cout, R L_max] (CHAIN_SHAPES[k]); lengths: None (every item L_max) or B lengths in kernel
+        k's input units (list, tuple or CPU tensor).  out: an optional fp32 CUDA tensor whose first B Cout R L_max elements
+        receive the output (a view of them is returned), e.g. a NaN-filled buffer with a guard region after it.
+        Synchronous."""
+        torch = self.torch
+        code = _precision(precision)
+        if not isinstance(k, int) or not 0 <= k < len(self.CHAIN_SHAPES):
+            raise EngineError("chain kernel index must be 0..7 (got %r)" % (k,))
+        cin, cout, R = self.CHAIN_SHAPES[k]
+        if x.dim() != 3 or x.shape[1] != cin:
+            raise EngineError("chain kernel %d expects x [B, %d, L], got %s" % (k, cin, tuple(x.shape)))
+        if x.device != self.device or x.dtype != torch.float32:
+            raise EngineError("x must be an fp32 tensor on %s" % (self.device,))
+        x = x.contiguous()
+        B, _, L = x.shape
+        lens = None if lengths is None else _lengths(lengths, B, L)
+        n = B * cout * R * L
+        if out is None:
+            out = torch.empty(n, dtype=torch.float32, device=self.device)
+        elif out.device != self.device or out.dtype != torch.float32 or not out.is_contiguous() or out.numel() < n:
+            raise EngineError("out must be a contiguous fp32 tensor on %s of at least %d elements" % (self.device, n))
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream().cuda_stream
+            check(lib().mg_gen_chain_kernel(self.packed.data_ptr(), k, x.data_ptr(), out.data_ptr(), B, L, lens, code, stream))
+        return out.view(-1)[:n].view(B, cout, R * L)
 
     def resblock_post(self, x):
         """Last ResBlock + LeakyReLU -> conv_post -> tanh (models.py:66-69) on x [B, 32, L] -> audio [B, 1, L]; synchronous."""

@@ -30,12 +30,13 @@ def geometry(stage):
     return dict(ROWS=rows, MAXSEG=maxseg, NSX=nsx)
 
 
-def test_convt_config_names():
-    """Stages 2 and 3 report their streaming geometry; the stride-8 stages have none."""
+def test_convt_config_names_report_every_stage():
+    """Stages 2 and 3 report their streaming geometry, the stride-8 stages their tiles; unknown stages nothing."""
     for s in (2, 3):
         g = geometry(s)
         assert g["ROWS"] % 64 == 0 and g["MAXSEG"] >= 3 and g["NSX"] >= 2, g
-    assert engine.lib().mg_gen_convt_config(0) == b"" and engine.lib().mg_gen_convt_config(1) == b""
+    assert re.fullmatch(r"convt_tc_kernel<UpCfg<0,\d+,\d+>>", engine.lib().mg_gen_convt_config(0).decode())
+    assert re.fullmatch(r"convt_resident_tc_kernel<UpCfg<1,\d+,\d+>>", engine.lib().mg_gen_convt_config(1).decode())
     assert engine.lib().mg_gen_convt_config(4) == b"" and engine.lib().mg_gen_convt_config(-1) == b""
 
 
