@@ -276,6 +276,24 @@ size_t mg_disc_packed_bytes(void);
 int mg_disc_pack(const float *const *v, const float *const *g, const float *const *bias, void *packed, void *stream);
 int mg_disc_forward(const void *packed, const float *x, int Bt, int L, float *const *fmaps, void *status_word, void *stream);
 
+/* Layer `layer` (1..6: grouped_convs.0-3, conv_post1, conv_post2) of discriminator `scale` (0..2; 0 for a stand-alone
+ * Discriminator's blob) on a caller-given input, through the launcher mg_msd_forward runs for that layer:
+ *   x [Bt][Cin][Lin] -> out [Bt][Cout][Lout] (device fp32, x != out), Lout = (Lin + 2 pad - k) / stride + 1 >= 1; the
+ *   output is post-LeakyReLU except conv_post2's.  Writes out[:, :, 0 .. Lout) and nothing else.
+ * Asynchronous on `stream`; status_word and the 1 <= Bt <= 65535 limit as for mg_msd_forward (the word is not cleared:
+ * check it with mg_msd_check_status).  MG_DISC_GROUP=simt selects the SIMT grouped convs here too.  Every argument is checked
+ * before any CUDA call.  Test entry point: a layer's kernel on inputs the caller chooses. */
+int mg_msd_layer_forward(const void *packed, int scale, int layer, const float *x, float *out, int Bt, int Lin, void *status_word,
+                         void *stream);
+/* Which folded weight a bf16 element of one discriminator's blob holds in the four split-bf16 copies the tensor cores read:
+ * `offset` is the element's byte offset from the start of that discriminator's blob.  Returns the half (0 hi, 1 lo) of weight
+ * w[co][ci][tap] of the layer's torch layout [Cout][Cin / groups][k] (ci < 4 for the grouped convs), 2 for a structural zero
+ * of a Toeplitz copy (co and ci are then the slot's, tap the out-of-range tap it stands for), or -1 for an offset outside
+ * the copies.  *copy: 1..3 the Toeplitz copy of grouped_convs.0-2, 4 that of grouped_convs.3, 5 conv_post1's forward copy,
+ * 6 its transposed, tap-flipped copy (the data gradient's; still reported as the forward weight w[co][ci][tap]).  One
+ * weight sits in several Toeplitz slots, hence the map from slot to weight.  Tests restate the layouts against it. */
+int mg_disc_tc_element(size_t offset, int *copy, int *co, int *ci, int *tap);
+
 /* ---------------------------------------------------------------------------------------
  * Mel-spectrogram front end.   Replaces: mel_spectrogram (meldataset.py:44-55: zero-pad by (n_fft - hop)/2, librosa
  * melspectrogram with power 1 and Slaney-normalised triangles, log(clip(., 1e-5))) for the reference's analysis parameters

@@ -500,6 +500,59 @@ int mg_disc_forward(const void *packed, const float *x, int Bt, int L, float *co
     return launch_disc_forward(packed, x, Bt, L, fmaps, (int *)status_word, (cudaStream_t)stream);
 }
 
+int mg_msd_layer_forward(const void *packed, int scale, int layer, const float *x, float *out, int Bt, int Lin, void *status_word,
+                         void *stream) {
+    const char *fn = "mg_msd_layer_forward";
+    if (!packed || !x || !out || !status_word) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
+    if ((const void *)x == (const void *)out) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: x and out must differ", fn);
+    if (scale < 0 || scale > 2) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: scale %d is outside [0, 2]", fn, scale);
+    if (layer < 1 || layer >= kDiscLayers)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: layer %d is outside [1, %d]", fn, layer, kDiscLayers - 1);
+    if (Bt < 1 || Bt > 65535)  // conv_post2 and the SIMT grouped convs put the items on grid.y / grid.z, as in mg_msd_forward
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: batch %d is outside [1, 65535]", fn, Bt);
+    const DLayer d = d_layer(layer);
+    const int Lout = Lin < 1 ? 0 : (Lin + 2 * d.pad - d.k) / d.stride + 1;
+    if (Lout < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: Lin = %d gives no output at layer %d", fn, Lin, layer);
+    if ((long long)Bt * d.cin * Lin > 0x7fffffffll || (long long)Bt * d.cout * Lout > 0x7fffffffll)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: Bt * C * L exceeds 2^31 - 1 elements", fn);
+    const uint8_t *blob = reinterpret_cast<const uint8_t *>(packed) + (size_t)scale * d_blob_bytes();
+    return launch_disc_layer_forward(blob, layer, x, out, Bt, Lin, Lout, (int *)status_word, (cudaStream_t)stream);
+}
+
+int mg_disc_tc_element(size_t offset, int *copy, int *co, int *ci, int *tap) {
+    if (!copy || !co || !ci || !tap || offset % 2) return -1;
+    int h = 2;
+    if (offset >= d_gtc_start() && offset < d_gtc_start() + d_gtc_bytes()) {  // layers 1..3: d_gtc_index
+        size_t rel = offset - d_gtc_start();
+        int l = 1;
+        while (rel >= d_gtc_offset(l + 1)) ++l;
+        rel -= d_gtc_offset(l);
+        const int grp = (int)(rel / d_gtc_group_bytes()), i = (int)(rel % d_gtc_group_bytes()) / 2;
+        const int c = i & 3, pos = (i >> 2) & 1, n = (i >> 3) & 63, r = ((i >> 9) & 1) | (((i >> 10) & 1) << 1), kp = i >> 11;
+        const int half = n >> 5, e = (n >> 4) & 1, q = 2 * kp + pos - 1 - e, k = 4 * q + r;
+        *copy = l; *co = grp * 16 + (n & 15); *ci = c; *tap = k;
+        if (q >= 0 && k <= 40) h = half;
+    } else if (offset >= d_g4tc_start() && offset < d_g4tc_start() + d_g4tc_bytes()) {  // layer 4: d_g4tc_index
+        const size_t rel = offset - d_g4tc_start();
+        const int grp = (int)(rel / d_g4tc_group_bytes()), i = (int)(rel % d_g4tc_group_bytes()) / 2;
+        const int j = i & 7, n = (i >> 3) & 63, c = ((i >> 9) & 1) | (((i >> 10) & 1) << 1), kp = i >> 11;
+        const int half = n >> 5, e = (n >> 2) & 7, k = 8 * kp + j - e;
+        *copy = 4; *co = grp * 4 + (n & 3); *ci = c; *tap = k;
+        if (k >= 0 && k <= 40) h = half;
+    } else {  // conv_post1: the forward copy (5) and the transposed, tap-flipped copy (6), conv_tc_weight_index
+        const bool fwd = offset >= d_tc_start() && offset < d_tc_start() + d_tc_bytes();
+        if (!fwd && !(offset >= d_tcT_start() && offset < d_tcT_start() + d_tc_bytes())) return -1;
+        const size_t i = (offset - (fwd ? d_tc_start() : d_tcT_start())) / 2;
+        const int c8 = (int)(i % 8), row = (int)((i / 8) % kPost1NG);
+        size_t rest = i / (8 * kPost1NG);
+        const int kh = (int)(rest % 2), half = (int)((rest / 2) % 2), t = (int)((rest / 4) % 5), c16 = (int)((rest / 20) % 64);
+        const int a = (int)(rest / 1280) * kPost1NG + row, b = c16 * 16 + kh * 8 + c8;  // [a][b][t]: W[co][ci][tap] / W'[ci][co][4 - tap]
+        *copy = fwd ? 5 : 6; *co = fwd ? a : b; *ci = fwd ? b : a; *tap = fwd ? t : 4 - t;
+        h = half;
+    }
+    return h;
+}
+
 int mg_msd_check_status(const void *status_word, void *stream) {
     if (!status_word) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_msd_check_status: null argument");
     MG_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)stream));

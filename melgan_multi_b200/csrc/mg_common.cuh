@@ -189,6 +189,8 @@ int launch_disc_group4_tc(const float *x, float *out, const uint8_t *wtc, const 
                           cudaStream_t s);
 int launch_disc_pack(const float *const *v, const float *const *g, const float *const *bias, void *packed, cudaStream_t s, int ndisc = 3);
 int launch_disc_forward(const void *packed, const float *x, int Bt, int L, float *const *fmaps, int *status, cudaStream_t s);
+int launch_disc_layer_forward(const void *blob, int l, const float *x, float *out, int Bt, int Lin, int Lout, int *status,
+                              cudaStream_t s);
 void msd_lengths(int L, int *lens);
 int launch_lrelu_grad(const float *g1, const float *g2, const float *out, float *dz, long long n, cudaStream_t s);
 size_t grouped_bwd_workspace_bytes(int l, int Bt, int Lout);

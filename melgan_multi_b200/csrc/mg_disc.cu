@@ -312,6 +312,27 @@ struct ScaleStreams {
     }
 };
 
+// Layer l (1..6) of one Discriminator: x [Bt][Cin][Lin] -> out [Bt][Cout][Lout], Lout = ln of layer l.  blob: that
+// discriminator's packed weights.  group_tc: the grouped convs on the tensor cores (false: the fp32 SIMT second
+// implementation, MG_DISC_GROUP=simt).  Enqueued on q.
+static int disc_layer(const uint8_t *blob, int l, const float *x, float *out, int Bt, int Lin, int Lout, int *status, bool group_tc,
+                      cudaStream_t q) {
+    const float *fw = reinterpret_cast<const float *>(blob);
+    const DLayer d = d_layer(l);
+    if (l <= 3)
+        return group_tc ? launch_disc_group_tc(x, out, blob + d_gtc_start() + d_gtc_offset(l), fw + d_bias_offset(l), Bt, d.cin,
+                                               d.cout, Lin, Lout, status, q)
+                        : launch_group<16, 4>(x, out, fw + d_weight_offset(l), fw + d_bias_offset(l), Bt, d.cin, d.cout, Lin, Lout, q);
+    if (l == 4)
+        return group_tc ? launch_disc_group4_tc(x, out, blob + d_g4tc_start(), fw + d_bias_offset(4), Bt, Lout, status, q)
+                        : launch_group<4, 1>(x, out, fw + d_weight_offset(4), fw + d_bias_offset(4), Bt, 1024, 1024, Lin, Lout, q);
+    if (l == 5) return launch_disc_post1_tc(x, out, blob + d_tc_start(), fw + d_bias_offset(5), Bt, Lout, status, q);
+    dim3 gp2((Lin + 7) / 8, Bt);
+    disc_post2_kernel<<<gp2, 256, 0, q>>>(x, out, fw + d_weight_offset(6), fw + d_bias_offset(6), Lin);
+    MG_CUDA_TRY(cudaGetLastError());
+    return MG_OK;
+}
+
 // One Discriminator (models.py:87-103) on the input of scale `sc` of y [Bt][1][L] (sc = 0: y itself; 1, 2: the AvgPool1d chain
 // of models.py:114-117, evaluated inside conv_pre).  blob: that discriminator's packed weights; f[0..6]: its feature maps;
 // ln[0..6]: their lengths.  Everything is enqueued on q.
@@ -319,37 +340,27 @@ static int disc_chain(const uint8_t *blob, const float *y, int sc, int Bt, int L
                       int *status, bool group_tc, cudaStream_t q) {
     const float *fw = reinterpret_cast<const float *>(blob);
     const int Ls = sc == 0 ? L : sc == 1 ? L1 : L2;
-    int rc;
     dim3 gpre((Ls + 255) / 256, Bt);
     if (sc == 0) disc_pre_kernel<0><<<gpre, 256, 0, q>>>(y, f[0], fw, L, L1, L2);
     else if (sc == 1) disc_pre_kernel<1><<<gpre, 256, 0, q>>>(y, f[0], fw, L, L1, L2);
     else disc_pre_kernel<2><<<gpre, 256, 0, q>>>(y, f[0], fw, L, L1, L2);
     MG_CUDA_TRY(cudaGetLastError());
-    for (int l = 1; l <= 3; ++l) {  // stride-4 grouped convs: tensor cores (MG_DISC_GROUP=simt: the fp32 SIMT second implementation)
-        const DLayer d = d_layer(l);
-        if (group_tc)
-            rc = launch_disc_group_tc(f[l - 1], f[l], blob + d_gtc_start() + d_gtc_offset(l), fw + d_bias_offset(l), Bt, d.cin,
-                                      d.cout, ln[l - 1], ln[l], status, q);
-        else
-            rc = launch_group<16, 4>(f[l - 1], f[l], fw + d_weight_offset(l), fw + d_bias_offset(l), Bt, d.cin, d.cout, ln[l - 1],
-                                     ln[l], q);
+    for (int l = 1; l < kDiscLayers; ++l) {
+        const int rc = disc_layer(blob, l, f[l - 1], f[l], Bt, ln[l - 1], ln[l], status, group_tc, q);
         if (rc) return rc;
     }
-    if (group_tc)
-        rc = launch_disc_group4_tc(f[3], f[4], blob + d_g4tc_start(), fw + d_bias_offset(4), Bt, ln[4], status, q);
-    else
-        rc = launch_group<4, 1>(f[3], f[4], fw + d_weight_offset(4), fw + d_bias_offset(4), Bt, 1024, 1024, ln[3], ln[4], q);
-    if (rc) return rc;
-    if ((rc = launch_disc_post1_tc(f[4], f[5], blob + d_tc_start(), fw + d_bias_offset(5), Bt, ln[4], status, q))) return rc;
-    dim3 gp2((ln[5] + 7) / 8, Bt);
-    disc_post2_kernel<<<gp2, 256, 0, q>>>(f[5], f[6], fw + d_weight_offset(6), fw + d_bias_offset(6), ln[5]);
-    MG_CUDA_TRY(cudaGetLastError());
     return MG_OK;
 }
 
 static bool disc_group_tc() {
     const char *gp = getenv("MG_DISC_GROUP");
     return !(gp && strcmp(gp, "simt") == 0);
+}
+
+// one layer (1..6) of one discriminator on a caller-given input (mg_msd_layer_forward): blob = that discriminator's weights
+int launch_disc_layer_forward(const void *blob, int l, const float *x, float *out, int Bt, int Lin, int Lout, int *status,
+                              cudaStream_t s) {
+    return disc_layer(reinterpret_cast<const uint8_t *>(blob), l, x, out, Bt, Lin, Lout, status, disc_group_tc(), s);
 }
 
 // stand-alone Discriminator.forward (models.py:87-103): x [Bt][1][L] -> fmaps[0..6] (lengths: the scale-0 row of msd_lengths)

@@ -103,6 +103,11 @@ def lib():
         L.mg_msd_forward.restype = ctypes.c_int
         L.mg_msd_forward.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                      ctypes.c_void_p, ctypes.c_void_p]
+        L.mg_msd_layer_forward.restype = ctypes.c_int
+        L.mg_msd_layer_forward.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+                                           ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
+        L.mg_disc_tc_element.restype = ctypes.c_int
+        L.mg_disc_tc_element.argtypes = [ctypes.c_size_t] + [ctypes.POINTER(ctypes.c_int)] * 4
         L.mg_msd_grouped_backward_workspace_bytes.restype = ctypes.c_size_t
         L.mg_msd_grouped_backward_workspace_bytes.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int]
         L.mg_msd_grouped_backward.restype = ctypes.c_int
@@ -748,6 +753,29 @@ class DiscriminatorDevice:
             check(fn(self.packed.data_ptr(), y.data_ptr(), Bt, L, ptrs, self.status.data_ptr(), stream))
             self._watch.arm(self.status[:1])
         return fmaps
+
+    def layer_forward(self, scale, layer, x, out=None):
+        """Layer `layer` (1..6) of discriminator `scale` alone on x [Bt, Cin, Lin] (mg_msd_layer_forward, the launcher the
+        forward runs): returns out [Bt, Cout, Lout], written into `out` (a flat fp32 buffer of at least that many elements,
+        e.g. one filled with a marker to see what the kernel writes) when given.  Asynchronous: check_status() reports a
+        timed-out pipeline wait."""
+        torch = self.torch
+        from .synth import DISCRIMINATOR_LAYERS
+        _n, cin, cout, k, stride, _g, pad = DISCRIMINATOR_LAYERS[layer]
+        if x.dim() != 3 or x.shape[1] != cin or x.device != self.device or x.dtype != torch.float32:
+            raise EngineError("layer %d expects x [Bt, %d, L] fp32 on %s" % (layer, cin, self.device))
+        x = x.contiguous()
+        Bt, _, Lin = x.shape
+        n = Bt * cout * ((Lin + 2 * pad - k) // stride + 1)
+        if out is None:
+            out = torch.empty(max(n, 1), dtype=torch.float32, device=self.device)
+        if out.numel() < n or out.dtype != torch.float32 or not out.is_contiguous():
+            raise EngineError("out must be a contiguous fp32 buffer of at least %d elements" % n)
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream().cuda_stream
+            check(lib().mg_msd_layer_forward(self.packed.data_ptr(), scale, layer, x.data_ptr(), out.data_ptr(), Bt, Lin,
+                                             self.status.data_ptr(), stream))
+        return out[:n].view(Bt, cout, n // (Bt * cout))
 
     def scale_backward(self, scale, x0, fmaps, grads, need_gx0):
         """The whole backward of discriminator `scale` in one host call (mg_msd_scale_backward): x0 [Bt, 1, L0] its input,
