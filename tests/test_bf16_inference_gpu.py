@@ -21,81 +21,15 @@ import os
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 import cases
 from melgan_multi_b200 import engine, models, synth
-from test_kernel_borders_gpu import config, lengths as border_lengths
-from test_layer_isolation_gpu import Gen64, g64, gdev, gstate, row_errors  # noqa: F401 (fixtures)
+from kernel_model import g64, gdev, gen, gstate  # noqa: F401 (fixtures)
+from kernel_model import bf16_emulation_bound, config, convt64, lengths as border_lengths, no_rounding, resblock64, row_errors
 
-DILATIONS = (1, 3, 9)
-EMU_X = 2.0        # kernel error <= EMU_X * emulation error + EMU_FLOOR, per item
-EMU_FLOOR = 2e-5
 ROW_TOL = 3e-2     # stage isolation: per (item, channel) row, max|d| / max|ref| against exact float64
 ITEMS = (0, 15, 16, 31, 32, 47, 48, 63)  # the borders of config 2's four batch slices
 CHAIN_CODES = {0: 8, 1: 64, 2: 128, 14: 256}  # bf16 ResBlock stage codes of the default chain -> positions per mel frame
-
-
-# ------------------------------------------------------------------------------------------------------------------
-# float64 references: exact, and the bf16 emulation
-# ------------------------------------------------------------------------------------------------------------------
-def _bf16(t):
-    return t.to(torch.bfloat16).to(torch.float64)
-
-
-def _same(t):
-    return t
-
-
-def convt64(g, s, x, q):
-    w, b = g.w["ups.%d" % s]
-    k = w.shape[2]
-    return F.conv_transpose1d(q(F.leaky_relu(x)), q(w), b, stride=k // 2, padding=k // 4)
-
-
-def resblock64(g, s, x, q):
-    for j, d in enumerate(DILATIONS):
-        w1, b1 = g.w["resblocks.%d.convs1.%d" % (s, j)]
-        w2, b2 = g.w["resblocks.%d.convs2.%d" % (s, j)]
-        h = F.conv1d(q(F.leaky_relu(x)), q(w1), b1, padding=d, dilation=d)
-        x = F.conv1d(q(F.leaky_relu(h)), q(w2), b2, padding=1) + x
-    return x
-
-
-def forward64(g, mel, emulate):
-    """Exact float64 forward (emulate=False) or the bf16 emulation, mel [B, 80, T] -> audio [B, 1, 256 T]."""
-    q = _bf16 if emulate else _same
-    x = g.conv_pre(mel.double())
-    for s in range(4):
-        x = resblock64(g, s, convt64(g, s, x, _same if s == 2 else q), q)
-    return g.post(x)
-
-
-def forward64_items(g, mel, emulate, chunk=16):
-    return torch.cat([forward64(g, mel[i:i + chunk], emulate) for i in range(0, mel.shape[0], chunk)])
-
-
-def item_max_abs(y, ref):
-    return (y.double() - ref).abs().flatten(1).amax(dim=1)
-
-
-@pytest.fixture(scope="module")
-def gen(gstate):
-    g = models.Generator()
-    g.load_state_dict({k: torch.from_numpy(v) for k, v in gstate.items()})
-    return g.cuda().eval()
-
-
-def _emulation_bound(gen, g64, mel, what):
-    """bf16 forward of mel, its per-item error against exact float64 and the emulation's; asserts the bound."""
-    y = gen.generate(mel, precision="bf16")
-    gen._dev.check_status(mel.shape[0], mel.shape[2])
-    exact = forward64_items(g64, mel, False)
-    emu = forward64_items(g64, mel, True)
-    e_k, e_e = item_max_abs(y, exact), item_max_abs(emu, exact)
-    ratio = float(((e_k - EMU_FLOOR) / e_e).max())
-    assert bool((e_k <= EMU_X * e_e + EMU_FLOOR).all()), (what, e_k.tolist(), e_e.tolist())
-    return y, exact, e_k, e_e, ratio
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -115,7 +49,7 @@ def test_config2_full_size(gen, g64, config2_golden, realistic):
     mg_gen_forward_precision is mg_gen_forward bit for bit."""
     B, T = 64, 32
     mel = torch.from_numpy(synth.mel_input(B, T, 0, realistic)).cuda()
-    y, exact, e_k, e_e, ratio = _emulation_bound(gen, g64, mel, ("config2", realistic))
+    y, exact, e_k, e_e, ratio = bf16_emulation_bound(gen, g64, mel, ("config2", realistic))
     pos = torch.from_numpy(config2_golden["gen_B64_T32_positions"]).cuda()
     ref = torch.from_numpy(config2_golden["gen_B64_T32_s0_r%d" % int(realistic)]).cuda().double()
     d = y[:, :, pos].double() - ref
@@ -153,7 +87,7 @@ def test_goldens_within_twice_the_emulation_error(gen, g64, golden, case):
     emulation's + 2e-5.  The float64 forward itself is checked against the stored reference output first."""
     B, T, seed, realistic = case
     mel = torch.from_numpy(synth.mel_input(B, T, seed, realistic)).cuda()
-    y, exact, e_k, e_e, ratio = _emulation_bound(gen, g64, mel, case)
+    y, exact, e_k, e_e, ratio = bf16_emulation_bound(gen, g64, mel, case)
     if T == 1000:
         ref, got = golden["gen_T1000_head"], exact[0, 0, :4096]
     else:
@@ -184,7 +118,7 @@ def test_stage_taps_against_float64(gdev, g64):
     worst = []
     for s in range(4):
         x = taps[s][items].double()
-        y64 = resblock64(g64, s, convt64(g64, s, x, _same), _same)
+        y64 = resblock64(g64, s, convt64(g64, s, x, no_rounding), no_rounding)
         got, ref = (taps[s + 1][items], y64) if s < 3 else (audio[items], g64.post(y64))
         r = float(row_errors(got, ref).max())
         worst.append(r)
@@ -229,9 +163,9 @@ def test_ragged_items_equal_their_own_bf16_forward(gen, gstate):
 # ------------------------------------------------------------------------------------------------------------------
 # 6: tile and cluster borders
 # ------------------------------------------------------------------------------------------------------------------
-def border_frames():
+def bf16_border_frames():
     """Mel lengths that put an end of the sequence at (or one frame either side of) every tile and cluster border of the
-    default chain's bf16 ResBlock kernels, derived from the geometry the library reports (test_kernel_borders_gpu)."""
+    default chain's bf16 ResBlock kernels, derived from the geometry the library reports (kernel_model.lengths)."""
     out = set()
     for code, k in CHAIN_CODES.items():
         for L in border_lengths(config(code)):
@@ -242,12 +176,12 @@ def border_frames():
 
 @pytest.mark.gpu
 def test_borders_within_twice_the_emulation_error(gen, g64):
-    """Every border length of border_frames() as its own B = 1 forward, within the bound of the goldens."""
+    """Every border length of bf16_border_frames() as its own B = 1 forward, within the bound of the goldens."""
     worst = 0.0
-    Ts = border_frames()
+    Ts = bf16_border_frames()
     for T in Ts:
         mel = torch.from_numpy(synth.mel_input(1, T, 500 + T)).cuda()
-        _y, _exact, _e_k, _e_e, ratio = _emulation_bound(gen, g64, mel, T)
+        _y, _exact, _e_k, _e_e, ratio = bf16_emulation_bound(gen, g64, mel, T)
         worst = max(worst, ratio)
     print("\n%d border lengths (T = %s): worst (kernel - 2e-5) / emulation %.2f" % (len(Ts), Ts, worst))
 
@@ -311,7 +245,7 @@ def test_bf16_refuses_a_non_default_chain(mask):
 
 
 def test_border_frames_cover_every_bf16_code():
-    Ts = border_frames()
+    Ts = bf16_border_frames()
     assert Ts == sorted(set(Ts)) and Ts[0] >= 1
     for code, k in CHAIN_CODES.items():
         for L in border_lengths(config(code)):

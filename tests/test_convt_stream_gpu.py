@@ -16,8 +16,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from melgan_multi_b200 import engine, models, synth
-from test_layer_isolation_gpu import REL, TAU, folded64
+from melgan_multi_b200 import engine, models
+from kernel_model import gdev, gstate  # noqa: F401 (fixtures)
+from kernel_model import REL, TAU, check_items, folded64, ragged_batch
 
 CONFIG_RE = r"convt_stream_tc_kernel<StreamCfg<(\d+),(\d+),(\d+),(\d+)>>"
 
@@ -54,21 +55,6 @@ def border_cases(stage):
     return sorted(set(out))
 
 
-@pytest.fixture(scope="module")
-def state():
-    return synth.generator_state(1234)
-
-
-@pytest.fixture(scope="module")
-def dev(state):
-    gd = engine.GeneratorDevice("cuda:0")
-    order = [n for n, *_ in synth.GENERATOR_LAYERS]
-    to = lambda a: torch.from_numpy(a).cuda()
-    gd.pack([to(state[n + ".weight_v"]) for n in order], [to(state[n + ".weight_g"]) for n in order],
-            [to(state[n + ".bias"]) for n in order])
-    return gd
-
-
 def bound_ratio(state, stage, x, y):
     """Worst |y - y64| / (TAU A2 + 2^-20 |y64|) over every element."""
     w, b = folded64(state, "ups.%d" % stage)
@@ -87,44 +73,43 @@ def inputs(stage, B, L, seed):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("stage", [2, 3])
-def test_convt_stream_config2(state, dev, stage):
+def test_convt_stream_config2(gstate, gdev, stage):
     """The bench workload's shape (config 2: 64 items of 32 mel frames), every element within the bound; two calls agree bit
     for bit, and items 0, 31 and 63 equal their own B = 1 calls."""
     L = 32 * (64 if stage == 2 else 128)
     x = inputs(stage, 64, L, 20 + stage)
-    y = dev.convt(stage, x)
-    r = bound_ratio(state, stage, x, y)
+    y = gdev.convt(stage, x)
+    r = bound_ratio(gstate, stage, x, y)
     print("stage %d config 2: worst ratio to the bound %.3f" % (stage, r))
     assert r <= 1.0, r
-    assert torch.equal(dev.convt(stage, x), y)
+    assert torch.equal(gdev.convt(stage, x), y)
     for i in (0, 31, 63):
-        assert torch.equal(dev.convt(stage, x[i:i + 1].contiguous()), y[i:i + 1]), i
+        assert torch.equal(gdev.convt(stage, x[i:i + 1].contiguous()), y[i:i + 1]), i
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("stage", [2, 3])
-def test_convt_stream_tile_borders(state, dev, stage):
+def test_convt_stream_tile_borders(gstate, gdev, stage):
     worst = 0.0
     for B, L in border_cases(stage):
         x = inputs(stage, B, L, 1000 * stage + 7 * B + L)
-        y = dev.convt(stage, x)
-        r = bound_ratio(state, stage, x, y)
+        y = gdev.convt(stage, x)
+        r = bound_ratio(gstate, stage, x, y)
         worst = max(worst, r)
         assert r <= 1.0, (B, L, r)
-        assert torch.equal(dev.convt(stage, x), y), (B, L)
+        assert torch.equal(gdev.convt(stage, x), y), (B, L)
         for i in sorted({0, B // 2, B - 1}):
-            assert torch.equal(dev.convt(stage, x[i:i + 1].contiguous()), y[i:i + 1]), (B, L, i)
+            assert torch.equal(gdev.convt(stage, x[i:i + 1].contiguous()), y[i:i + 1]), (B, L, i)
     print("stage %d tile borders: worst ratio to the bound %.3f" % (stage, worst))
 
 
 @pytest.mark.gpu
-def test_convt_stream_ragged(state):
+def test_convt_stream_ragged(gstate):
     """Ragged batches through the generator (stage 2's ConvT is its own chain kernel): item boundaries of the stage-2 input
     (64 positions per mel frame + one zero row) at every offset into a tile, NaN past each length; each item equals its
     own forward bit for bit and the audio past its end is 0."""
-    from test_ragged_gpu import check_items, ragged_batch
     g = models.Generator()
-    g.load_state_dict({k: torch.from_numpy(v) for k, v in state.items()})
+    g.load_state_dict({k: torch.from_numpy(v) for k, v in gstate.items()})
     g = g.cuda().eval()
     R = geometry(2)["ROWS"]
     lens = [1, 2, 3, R // 64, R // 64 + 1, 2 * R // 64 - 1, 7, 32, 31, 33, 5, 1, 20]

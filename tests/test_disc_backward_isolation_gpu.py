@@ -34,16 +34,16 @@ Measured on an H100 80GB HBM3 (400 W power limit), printed by the tests (-s).  W
     weight-norm backward 0.237.  CPU calibration: fp32 sums 0.05 - 0.16 of tau_simt(n), one product dropped >= 13x;
     split-bf16 backward 0.06 - 0.08 of TAU, one pass dropped >= 13.8x.  The GPU tests of this file take about 20 s.
 """
-import math
-
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 from torch.nn.grad import conv1d_input, conv1d_weight
 
-from melgan_multi_b200 import engine, models, synth
-from test_layer_isolation_gpu import REL, TAU, _bf16, ddev, dstate, folded64, split_conv  # noqa: F401 (fixtures)
+from melgan_multi_b200 import engine, synth
+from kernel_model import ddev, dstate  # noqa: F401 (fixtures)
+from kernel_model import (POST1_PAD, POST1_ROWS, REL, SIMT_N, TAU, WG_PANEL, WG_STAGE, bf16_rn, cdiv, folded64,
+                          post1_lengths, post1_straddles, tau_simt, upstream)
 
 LAYERS = synth.DISCRIMINATOR_LAYERS
 SLOPE = 0.01  # kSlope (csrc/mg_layout.h)
@@ -54,21 +54,7 @@ DX4_TILE = 512                   # grouped_dx4_kernel: input positions per CTA, 
 DX1_TILE, DX1_VEC = 128, 8       # grouped_dx1_kernel: positions per CTA, per thread (two float4 stores if p + 8 <= Lin)
 DW_TILE = 128                    # grouped_dw4_kernel / grouped_dw1_kernel: output positions per tile
 PRE_TILE, PRE_HALO = 512, 7      # disc_pre_bwd_kernel
-POST1_ROWS, POST1_PAD = 128, 2   # conv_rows_tc_kernel<Post1DgradCfg>: virtual rows per CTA, L + 2 rows per item
-WG_PANEL, WG_STAGE = 8, 32       # post1_wgrad_tc_kernel: positions per k-panel (per item) and per stage
 POST2_THREADS = 256              # disc_post2_dw_kernel: threads along the flattened (item, position) axis
-
-
-def tau_simt(n):
-    """Element-wise tau of an fp32 SIMT sum of n products (module docstring)."""
-    return 2.0 ** -20 * math.sqrt(n)
-
-
-SIMT_N = (3, 24, 164, 176, 240, 393, 1024, 2048)  # calibrated n; every n a GPU test uses must be <= the largest
-
-
-def cdiv(a, b):
-    return -(-a // b)
 
 
 def grouped_plan(layer, Bt, Lout):
@@ -189,27 +175,6 @@ def scale_input(y, s):
     return x
 
 
-def upstream(fm, pattern):
-    """Gradients w.r.t. the 21 stacked maps fm[s][l] (first half real, second half generated), through the package's
-    loss functions: "generator" = feature-map L1 + LSGAN generator term (every map), "discriminator" = the LSGAN
-    discriminator loss (the logits only), "map 3" = the generator step's gradient on map 3 alone."""
-    leaves = [[f.detach().clone().requires_grad_(True) for f in sc] for sc in fm]
-    B = leaves[0][0].shape[0] // 2
-    d_r = [torch.flatten(sc[6][:B], 1) for sc in leaves]
-    d_g = [torch.flatten(sc[6][B:], 1) for sc in leaves]
-    if pattern == "discriminator":
-        loss = models.discriminator_loss(d_r, d_g)[0]
-    else:
-        loss = models.feature_loss([[f[:B] for f in sc] for sc in leaves], [[f[B:] for f in sc] for sc in leaves])
-        loss = loss + models.generator_loss(d_g)
-    flat = [f for sc in leaves for f in sc]
-    gr = torch.autograd.grad(loss, flat, allow_unused=True)
-    G = [list(gr[7 * s:7 * s + 7]) for s in range(3)]
-    if pattern == "map 3":
-        G = [[g if l == 3 else None for l, g in enumerate(Gs)] for Gs in G]
-    return G
-
-
 def forward(dd, Bt, L):
     y = torch.from_numpy(synth.audio_input(Bt, L, 11 * L + Bt)).cuda()
     fm = dd.forward(y)
@@ -249,8 +214,8 @@ def test_tau_calibration_on_emulated_fp32_sums(n):
 def split_bilinear(f, a, b, passes=(0, 1, 2)):
     """A bilinear contraction f(a, b) the way the tensor cores run it on fp32 operands: passes (ah, bh), (al, bh), (ah, bl)
     of the bf16 hi / lo split, exact products accumulated (in float64 here, rounded to fp32 at the end)."""
-    ah, bh = _bf16(a), _bf16(b)
-    al, bl = _bf16(a - ah), _bf16(b - bh)
+    ah, bh = bf16_rn(a), bf16_rn(b)
+    al, bl = bf16_rn(a - ah), bf16_rn(b - bh)
     ops = [(ah, bh), (al, bh), (ah, bl)]
     return sum(f(ops[p][0].double(), ops[p][1].double()) for p in passes).float()
 
@@ -337,14 +302,6 @@ def pre_lengths():
     return [5, T - H, T - 1, T, T + 1, T + H, 2 * T, 2 * T + H]
 
 
-def post1_lengths():
-    """conv_post1 dgrad (128 virtual rows, L + 2 rows per item) and wgrad (8-position k-panels per item, 32-position
-    stages): L < 5, L % 4 != 0, L % 8 != 0, part-filled stages, items that tile the 128 rows exactly or straddle two."""
-    R, P = POST1_ROWS, POST1_PAD
-    return [1, 3, 4, 5, 7, WG_PANEL + 1, 17, WG_STAGE - 1, WG_STAGE, WG_STAGE + 1, R // 2 - P, R // 2 - P + 1, 65,
-            R - P, R - P + 1]
-
-
 BORDER_CASES = ([(l, L) for l in (1, 2, 3) for L in dx4_lengths()] + [(4, L) for L in dx1_lengths()] +
                 [(0, L) for L in pre_lengths()] + [(5, L) for L in post1_lengths()])
 # (layer, Bt, Lout) of the grouped weight-gradient chunk plan: chunks that straddle two items with a short last chunk,
@@ -357,11 +314,6 @@ def chunk_claims(layer, Bt, Lout):
     tiles, tpc, chunks = grouped_plan(layer, Bt, Lout)
     straddle = any((c * tpc) // tiles != (min(Bt * tiles, (c + 1) * tpc) - 1) // tiles for c in range(chunks))
     return straddle, (Bt * tiles) % tpc != 0, chunks == 1
-
-
-def post1_straddles(Bt, L):
-    """An item's L + 2 virtual rows straddle two 128-row tiles of the dgrad launch."""
-    return any((i * (L + POST1_PAD)) // POST1_ROWS != ((i + 1) * (L + POST1_PAD) - 1) // POST1_ROWS for i in range(Bt))
 
 
 def test_border_cases_sit_on_the_kernel_borders():

@@ -4,8 +4,8 @@ convs (disc_group_tc_kernel, disc_group4_tc_kernel), conv_post1's forward and da
 
 Blob.  disc_pack_kernel keeps, per discriminator, a Toeplitz copy of grouped_convs.0-2 (each weight once per output parity,
 zero slots where a panel's tap falls outside 0..40), the 8-outputs-per-lane Toeplitz copy of grouped_convs.3 (each weight
-once per e), conv_post1's copy and its transposed, tap-flipped copy for the data gradient.  The layouts are restated here
-(numpy) and checked against mg_disc_tc_element on every element of one group per copy and a seeded sample of the rest.
+once per e), conv_post1's copy and its transposed, tap-flipped copy for the data gradient.  The layouts are restated in
+kernel_model (numpy) and checked against mg_disc_tc_element on every element of one group per copy and a seeded sample of the rest.
 On the GPU: every element of the grouped copies is split_bf16 of the fp32 folded weight in the blob, hi = bf16_rn(w),
 lo = bf16_rn(w - hi), bit for bit, every structural zero +0.0; conv_post1's transposed copy equals the forward copy at
 (ci, co, 4 - tap) bit for bit, each lo is at most half a bf16 ulp of its hi and hi + lo is within 2^-16 |w64| of the float64
@@ -78,9 +78,11 @@ import torch.nn.functional as F
 from torch.nn.grad import conv1d_weight
 
 from melgan_multi_b200 import engine, synth
-from test_disc_backward_isolation_gpu import WG_PANEL, WG_STAGE, post1_lengths, post1_straddles, upstream
-from test_disc_forward_borders_gpu import GROUP4_TARGETS, GROUP_TARGETS, batches, group4_plan, group_tc_plan
-from test_layer_isolation_gpu import ddev, dstate, folded64  # noqa: F401 (fixtures)
+from kernel_model import ddev, dstate  # noqa: F401 (fixtures)
+from kernel_model import (BLOB_BYTES, G4TC_GROUP, G4TC_START, GROUP4_TARGETS, GROUP_TARGETS, GROUPS, GTC_GROUP, TC_BYTES,
+                          TC_START, TCT_START, WG_PANEL, WG_STAGE, batches, cdiv, disc_bias_offset, disc_weight_offset,
+                          folded64, group4_plan, group_tc_plan, gtc_start, guard_ok, nan_buffer, post1_lengths,
+                          post1_offset, post1_straddles, slots, split_np, split_passes, split_rn, toeplitz_slots, upstream)
 
 LAYERS = synth.DISCRIMINATOR_LAYERS
 TAU_E = 3 * 2.0 ** -16       # the generator's emulation bound (test_gen_front_kernels_gpu), K = 1024 x 5
@@ -88,91 +90,13 @@ TAU_G = 2.0 ** -16           # the grouped convs, K = 4 x 41: their MMAs add 28 
 REL_E = 2.0 ** -22
 MUTANT_X = 4                 # each operand mutant exceeds the bound by at least this factor
 SLOPE32 = float(np.float32(0.01))
-GUARD = 1024                 # floats after each output buffer
-FILL = 0x7FC0DEAD            # quiet NaN with a payload: arithmetic on NaN gives the canonical NaN, never this
 EXACT_N = (64, 16, 4, 1)     # nonzeros per v row of the exact-operand state
 EX, EW = 0, -4               # exponents of the exact operands' hi halves: x and dz, weights
 
 
-def cdiv(a, b):
-    return -(-a // b)
-
-
 # ------------------------------------------------------------------------------------------------------------------
-# the blob of one discriminator (restated from csrc/mg_layout.h)
+# the blob of one discriminator: kernel_model's restatement of csrc/mg_layout.h against the library
 # ------------------------------------------------------------------------------------------------------------------
-def _fp32_floats():
-    w = sum(0 if n == "conv_post1" else cout * (cin // g) * k for n, cin, cout, k, _s, g, _p in LAYERS)
-    return w + sum(cout for _n, _ci, cout, *_ in LAYERS)
-
-
-def weight_offset(l):
-    """Float offset of layer l's fp32 weights (grouped layers: [group][ci 4][tap 41][co within group])."""
-    return sum(0 if n == "conv_post1" else cout * (cin // g) * k for n, cin, cout, k, _s, g, _p in LAYERS[:l])
-
-
-def bias_offset(l):
-    return weight_offset(7) + sum(cout for _n, _ci, cout, *_ in LAYERS[:l])
-
-
-TC_BYTES = 1024 * 1024 * 5 * 4
-GTC_GROUP, G4TC_GROUP = 7 * 2 * 2 * 64 * 16, 6 * 2 * 2 * 64 * 16
-GROUPS = {1: 4, 2: 16, 3: 64, 4: 256}
-TC_START = cdiv(_fp32_floats() * 4, 256) * 256
-GTC_START = TC_START + TC_BYTES
-G4TC_START = GTC_START + (4 + 16 + 64) * GTC_GROUP
-TCT_START = G4TC_START + 256 * G4TC_GROUP
-BLOB_BYTES = TCT_START + TC_BYTES + 4096
-
-
-def gtc_start(l):
-    return GTC_START + sum(GROUPS[i] for i in range(1, l)) * GTC_GROUP
-
-
-def toeplitz_slots(l):
-    """Every bf16 element of layer l's Toeplitz copy (l = 1..4) as arrays (offset, h, co, ci, tap), h = 2 for a structural
-    zero.  l = 1..3: block row n = [half][parity e][co 16], element (pos, ci) of k-panel kp of phase r holds tap
-    4 q + r, q = 2 kp + pos - 1 - e.  l = 4: n = [half][e 8][co 4], element i of k-panel kp of channel ci holds tap
-    8 kp + i - e."""
-    if l <= 3:
-        grp, kp, r, half, e, col, pos, ci = np.meshgrid(*(np.arange(v) for v in (GROUPS[l], 7, 4, 2, 2, 16, 2, 4)), indexing="ij")
-        n = half * 32 + e * 16 + col
-        idx = (((kp * 2 + r // 2) * 2 + r % 2) * 64 + n) * 8 + pos * 4 + ci
-        off = gtc_start(l) + grp * GTC_GROUP + 2 * idx
-        q = 2 * kp + pos - 1 - e
-        tap = 4 * q + r
-        valid = (q >= 0) & (tap <= 40)
-        co = grp * 16 + col
-    else:
-        grp, kp, ci, half, e, col, i = np.meshgrid(*(np.arange(v) for v in (256, 6, 4, 2, 8, 4, 8)), indexing="ij")
-        n = half * 32 + e * 4 + col
-        idx = (((kp * 2 + ci // 2) * 2 + ci % 2) * 64 + n) * 8 + i
-        off = G4TC_START + grp * G4TC_GROUP + 2 * idx
-        tap = 8 * kp + i - e
-        valid = (tap >= 0) & (tap <= 40)
-        co = grp * 4 + col
-    h = np.where(valid, half, 2)
-    return tuple(a.ravel() for a in (off, h, co, ci, tap))
-
-
-def post1_offset(co, ci, tap, h, transposed=False):
-    """Byte offset of half h of conv_post1's w[co][ci][tap]: ring slots of (128-channel group, 16-channel chunk, tap), each
-    [half][k-panel][row][8]; the transposed copy holds it at row ci, column co, tap 4 - tap.  numpy arrays welcome."""
-    a, b, t = (ci, co, 4 - tap) if transposed else (co, ci, tap)
-    i = (((((a // 128) * 64 + b // 16) * 5 + t) * 2 + h) * 2 + (b % 16) // 8) * 1024 + (a % 128) * 8 + b % 8
-    return (TCT_START if transposed else TC_START) + 2 * i
-
-
-def post1_slots(transposed):
-    co, ci, tap, h = np.meshgrid(np.arange(1024), np.arange(1024), np.arange(5), np.arange(2), indexing="ij")
-    return tuple(a.ravel() for a in (post1_offset(co, ci, tap, h, transposed), h, co, ci, tap))
-
-
-def slots(copy):
-    """(offset, h, co, ci, tap) of every element of copy 1..6 (mg_disc_tc_element's numbering)."""
-    return toeplitz_slots(copy) if copy <= 4 else post1_slots(copy == 6)
-
-
 def tc_element(offset):
     out = [ctypes.c_int(-9) for _ in range(4)]
     h = engine.lib().mg_disc_tc_element(int(offset), *(ctypes.byref(v) for v in out))
@@ -285,13 +209,6 @@ def exact_weights():
                 w[d][l] = (g.astype(np.float64) / np.sqrt((v != 0).sum((1, 2), keepdims=True)) * v).astype(np.float32)
         _EXACT.update(state=st, w=w)
     return _EXACT["state"], _EXACT["w"]
-
-
-def split_np(v):
-    """(hi, lo) of split_bf16 on an fp32 array, as float64 (round to nearest even, through torch)."""
-    t = torch.from_numpy(np.ascontiguousarray(v, np.float32))
-    hi = t.to(torch.bfloat16).float()
-    return hi.double().numpy(), (t - hi).to(torch.bfloat16).double().numpy()
 
 
 def test_exact_state_folds_to_split_halves():
@@ -429,16 +346,6 @@ def test_exact_operands_sum_exactly():
 # ------------------------------------------------------------------------------------------------------------------
 # the emulation, and the bound calibrated on the CPU
 # ------------------------------------------------------------------------------------------------------------------
-def bf16_rn(v):
-    return v.to(torch.bfloat16).to(v.dtype)
-
-
-def split_rn(v):
-    """hi = bf16_rn(v), lo = bf16_rn(v - hi) of an fp32 tensor (split2_bf16), as float64."""
-    hi = bf16_rn(v)
-    return hi.double(), bf16_rn(v - hi).double()
-
-
 def conv_fn(kind, l=None):
     """f(a, w) of a kernel's contraction: grouped conv l, conv_post1 forward / data gradient (a conv on the transposed
     weights [ci][co][k']), or the weight gradient (a = dz, w = x: returns [co][ci][tap])."""
@@ -448,11 +355,6 @@ def conv_fn(kind, l=None):
     if kind in ("post1", "dgrad"):
         return lambda a, w: F.conv1d(a, w, padding=2)
     return lambda a, w: conv1d_weight(w, (a.shape[1], w.shape[1], 5), a, 1, 2)
-
-
-def emulate(f, ah, al, wh, wl):
-    """float64 sum of the passes (ah, wh) + (al, wh) + (ah, wl) ((ah + al) is exact in float64)."""
-    return f(ah + al, wh) + f(ah, wl)
 
 
 def act(pre):
@@ -510,7 +412,7 @@ def test_tau_calibration(kind, l, size):
     wh, wl = split_rn(w)
     a64, w64 = a.double(), w.double()
     a2 = f(a64 * a64, w64 * w64).sqrt()
-    pre = emulate(f, ah, al, wh, wl)
+    pre = split_passes(f, ah, al, wh, wl)
     acc = mma_acc(kind, K)
     lrelu = kind in ("group", "post1")
     r = lambda y: float(ratio(act(y) if lrelu else y, pre, a2, lrelu, acc, TAU_G if kind == "group" else TAU_E).max())
@@ -595,7 +497,7 @@ def fp32_grouped(dd, s, l):
     _n, _cin, cout, _k, _s, groups, _p = LAYERS[l]
     cog = cout // groups
     f = dd.packed[s * BLOB_BYTES // 4:(s + 1) * BLOB_BYTES // 4]
-    blk = f[weight_offset(l):weight_offset(l) + cout * 164].view(groups, 164, cog)
+    blk = f[disc_weight_offset(l):disc_weight_offset(l) + cout * 164].view(groups, 164, cog)
     return blk.permute(0, 2, 1).reshape(cout, 4, 41)
 
 
@@ -686,17 +588,9 @@ def cached_halves(dd, s, l):
     return _HALVES[key]
 
 
-def nan_buffer(n):
-    return torch.full((n + GUARD,), FILL, dtype=torch.int32, device="cuda").view(torch.float32)
-
-
-def guard_ok(buf, n):
-    return bool((buf.view(torch.int32)[n:] == FILL).all())
-
-
 def bias_of(dd, s, l):
     f = dd.packed[s * BLOB_BYTES // 4:(s + 1) * BLOB_BYTES // 4]
-    return f[bias_offset(l):bias_offset(l) + LAYERS[l][2]].double()
+    return f[disc_bias_offset(l):disc_bias_offset(l) + LAYERS[l][2]].double()
 
 
 def run_layer(dd, s, l, x):
@@ -716,7 +610,7 @@ def forward_emulation(dd, s, l, x):
     f = conv_fn(kind, l)
     wh, wl = cached_halves(dd, s, l)
     ah, al = split_rn(x)
-    pre = emulate(f, ah, al, wh, wl) + bias_of(dd, s, l)[None, :, None]
+    pre = split_passes(f, ah, al, wh, wl) + bias_of(dd, s, l)[None, :, None]
     w = wh + wl
     x64 = x.double()
     return pre, f(x64 * x64, w * w).sqrt()
@@ -746,14 +640,14 @@ def dgrad_emulation(dd, s, dz):
     f = conv_fn("dgrad")
     w = wh + wl
     d64 = dz.double()
-    return emulate(f, ah, al, wh, wl), f(d64 * d64, w * w).sqrt()
+    return split_passes(f, ah, al, wh, wl), f(d64 * d64, w * w).sqrt()
 
 
 def wgrad_emulation(x, dz):
     ah, al = split_rn(dz)
     bh, bl = split_rn(x)
     f = conv_fn("wgrad")
-    return emulate(f, ah, al, bh, bl), f(dz.double() ** 2, x.double() ** 2).sqrt()
+    return split_passes(f, ah, al, bh, bl), f(dz.double() ** 2, x.double() ** 2).sqrt()
 
 
 class Worst:

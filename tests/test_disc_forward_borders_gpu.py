@@ -1,8 +1,9 @@
 """Every discriminator forward kernel at each tile and packed-item border of its launch geometry, against float64; the
 fp32 SIMT grouped convs (MG_DISC_GROUP=simt) at the same lengths.
 
-The input lengths are derived from the launch geometry (mirrored below from the kernels' sources) rather than picked by
-hand: for each border length of a kernel, find_L gives the shortest input that puts it at that layer.  Around it:
+The input lengths are derived from the launch geometry (mirrored from the kernels' sources, here and in kernel_model)
+rather than picked by hand: for each border length of a kernel, find_L gives the shortest input that puts it at that
+layer.  Around it:
   * disc_group_tc_kernel (grouped_convs.0-2): ni = 134 // (ceil(Lout/2) + 6) items share a CTA as virtual rows while two
     fit (Lout <= 122); from Lout = 123 each CTA is one 256-output tile of one item; odd Lout takes the scalar store;
   * disc_group4_tc_kernel (grouped_convs.3): ni = 133 // (ceil(L/8) + 5) items per tile, one single-item tile up to
@@ -49,20 +50,15 @@ import pytest
 import torch
 
 from melgan_multi_b200 import engine, synth
-from test_disc_backward_isolation_gpu import SIMT_N, post1_lengths, post1_straddles, tau_simt
-from test_layer_isolation_gpu import TAU, conv_bound_ratio, ddev, dstate, folded64  # noqa: F401 (fixtures)
+from kernel_model import ddev, dstate  # noqa: F401 (fixtures)
+from kernel_model import (GROUP4_TARGETS, GROUP_TARGETS, LANE4, POST1_PAD, POST1_ROWS, SIMT_N, TAU, batches,
+                          conv_bound_ratio, folded64, group4_plan, group_tc_plan, post1_lengths, post1_straddles, tau_simt)
 
 LAYERS = synth.DISCRIMINATOR_LAYERS
 GROUP_BT_LIMIT = 65535  # mg_msd_forward / mg_disc_forward (csrc/mg_api.cu): items go on grid.y / grid.z
 
 # launch geometry of the forward kernels
 TILE = 256                       # dg::TILE (csrc/mg_disc_tc.cu): outputs per disc_group_tc_kernel CTA, 128 rows x 2 parities
-PANELS = 7                       # kDgPanels (csrc/mg_layout.h): an item's halo is PANELS - 1 units
-UNITS = 134                      # dg::UNITS = 128 + kDgPanels - 1: 16-byte units (output pairs) per phase buffer
-PANELS4 = 6                      # kDg4Panels (csrc/mg_layout.h)
-UNITS4 = 133                     # dg4::UNITS = 128 + kDg4Panels - 1 (disc_group4_tc_kernel): units of 8 positions
-LANE4 = 8                        # disc_group4_tc_kernel: outputs per accumulator row
-POST1_ROWS, POST1_PAD = 128, 2   # Post1Cfg (csrc/mg_conv_tc.cu): virtual rows per CTA, zero rows after each item
 PRE_TILE, PRE_HALO = 256, 7      # disc_pre_kernel (csrc/mg_disc.cu): outputs per CTA, halo on each side
 POST2_TILE = 8                   # disc_post2_kernel (csrc/mg_disc.cu): positions per CTA
 SIMT_TILE = 128                  # disc_group_kernel (csrc/mg_disc.cu): outputs per CTA; input windows from 4 (t0 - 5)
@@ -71,10 +67,6 @@ SIMT_TILE = 128                  # disc_group_kernel (csrc/mg_disc.cu): outputs 
 N_PRE = (15, 18, 21)             # conv_pre: 15 products + 3 adds per AvgPool level, per scale
 N_POST2 = 32 * 3 + 2 + 8         # conv_post2: per-thread products, shuffle adds, combine of the 8 warp partials
 N_SIMT_GROUP = 4 * 41            # disc_group_kernel: input channels x taps, one fmaf chain
-
-
-def cdiv(a, b):
-    return -(-a // b)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -115,24 +107,6 @@ def find_L(scale, layer, target):
     return lo if at(lo) == target else None
 
 
-def group_tc_plan(Lout):
-    """(rp, ni) of launch_disc_group_tc: ni items per CTA at a pitch of rp units (the item's ceil(Lout / 2) output pairs
-    + 6 halo units) while two fit, else (None, 1): 256-output tiles of one item."""
-    rp = cdiv(Lout, 2) + PANELS - 1
-    ni = UNITS // rp
-    return (rp, ni) if ni > 1 else (None, 1)
-
-
-def group4_plan(L):
-    """(ni, segs) of launch_disc_group4_tc: ni = 133 // (nb + 5) items per tile with nb = ceil(L / 8) lanes each; items
-    longer than 128 lanes take segs = ceil(nb / 128) tiles of one item."""
-    nb = cdiv(L, LANE4)
-    ni = UNITS4 // (nb + PANELS4 - 1)
-    return (ni, 1) if ni >= 1 else (1, cdiv(nb, 128))
-
-
-GROUP_TARGETS = (1, 2, 3, 13, 14, 121, 122, 123, 124, 255, 256, 257, 512, 513)  # Lout of grouped_convs.0-2
-GROUP4_TARGETS = (1, 7, 8, 9, 487, 488, 489, 1023, 1024, 1025, 2048, 2049)      # L of grouped_convs.3
 PRE_TARGETS = (1, 2, 3, 4, 5, 255, 256, 257, 511, 512, 513)                     # Ls of conv_pre, every scale
 POST2_TARGETS = (1, 2, 7, 8, 9, 15, 16, 17)                                      # L of conv_post2
 SIMT_TARGETS = GROUP_TARGETS + (SIMT_TILE - 1, SIMT_TILE, SIMT_TILE + 1)         # Lout of the SIMT grouped convs
@@ -141,10 +115,6 @@ SIMT_TARGETS = GROUP_TARGETS + (SIMT_TILE - 1, SIMT_TILE, SIMT_TILE + 1)        
 def shortest(layer, target):
     """The smallest L over the three scales that gives `target` at `layer`."""
     return min(L for L in (find_L(s, layer, target) for s in range(3)) if L is not None)
-
-
-def batches(ni):
-    return {1, ni - 1, ni, ni + 1, 2 * ni + 1} - {0} if ni > 1 else {1, 3}
 
 
 def border_cases():

@@ -6,7 +6,7 @@ Emulation.  Each kernel multiplies bf16 operands exactly and accumulates in fp32
 with the accumulation in float64:
   * x is split into hi = bf16_rn(x), lo = bf16_rn(x - hi), as split2_bf16 does (csrc/mg_tc.cuh); the ConvTs split
     LeakyReLU(x) = fmaxf(x, x * 0.01f), taken in fp32;
-  * the weights' hi and lo halves are read back from the packed blob (at the layout restated below), not re-split from a
+  * the weights' hi and lo halves are read back from the packed blob (at the layout kernel_model restates), not re-split from a
     float64 fold: a few dozen of the ~1 M folded fp32 weights sit within an ulp of a bf16 rounding midpoint, and a
     re-split would round them the other way, a 2^-8 error on that product;
   * fp32 runs the passes (xh, wh) + (xl, wh) + (xh, wl), bf16 (up0, up1) the first alone; the bias is added exactly.
@@ -67,23 +67,15 @@ import torch
 import torch.nn.functional as F
 
 from melgan_multi_b200 import engine
-from test_layer_isolation_gpu import ROW_TOL, Gen64, g64, gdev, gstate, row_errors  # noqa: F401 (fixtures)
-from test_narrow_stage_gpu import res_base
+from kernel_model import g64, gdev, gstate  # noqa: F401 (fixtures)
+from kernel_model import (MUTANT_X, REL_E, ROW_TOL, SHAPE, TAU_E, bf16_of, bf16_rn, fill_faults, gen_weight_offset,
+                          lib_offset, lrelu32, nan_buffer, row_errors, split_passes, split_rn, up_tc_bytes, valid_mask,
+                          weight_grid)
 
-# 2^-16 covers a float32-accumulated emulation with room (test_tau_calibration); the H100's MMA accumulation measured up to
-# 1.43 x 2^-16 (up0, spread over the whole tile rather than at its borders: module docstring), so TAU_E is about twice that
-TAU_E = 3 * 2.0 ** -16
-REL_E = 2.0 ** -22
-MUTANT_X = 4  # each operand mutant exceeds the bound by at least this factor
 OLD_TAU, OLD_REL = 2.0 ** -12, 2.0 ** -20  # test_layer_isolation_gpu, against the exact product
 NUM_SMS = 132  # kNumSMs (csrc/mg_common.cuh)
-GUARD = 1024  # floats after each output buffer
-FILL = 0x7FC0DEAD  # quiet NaN with a payload: arithmetic on NaN gives the canonical NaN, never this
 
 KERNELS = ("pre", "up0", "up1", "up2", "up3")
-# (Cin, Cout, R = outputs per input position, K); layer index in the blob: pre 0, up s -> 1 + s
-SHAPE = {"pre": (80, 512, 1, 7), "up0": (512, 256, 8, 16), "up1": (256, 128, 8, 16), "up2": (128, 64, 2, 4),
-         "up3": (64, 32, 2, 4)}
 LAYER = {"pre": 0, "up0": 1, "up1": 2, "up2": 3, "up3": 4}
 CHAIN = {"pre": 0, "up0": 1, "up1": 3, "up2": 5}  # index in the default chain (up3 runs fused into kernel 7)
 RES_TABLES = {2: "up0", 4: "up1", 6: "up2", 7: "up3"}  # ResBlock chain kernel -> whose ragged tables it runs
@@ -212,48 +204,8 @@ def test_sweeps_contain_every_situation(kernel):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# where the blob keeps conv_pre's and the ConvTs' weights (restated from csrc/mg_layout.h)
+# where the blob keeps conv_pre's and the ConvTs' weights (restated in kernel_model.gen_weight_offset)
 # ------------------------------------------------------------------------------------------------------------------
-def up_tc_bytes(s):
-    return (512 >> s) * (256 >> s) * (16 if s < 2 else 4) * 4
-
-
-def up_base(s):
-    """ConvT s's block: after the 24 ResBlock convs, the ConvTs in stage order; conv_pre after the four."""
-    return res_base(29) + sum(up_tc_bytes(i) for i in range(s))
-
-
-def weight_offset(layer, a, b, tap, h):
-    """Byte offset of half h of w[a = co][b = ci][tap] (conv_pre, layer 0) or W[a = ci][b = co][tap] (ups[layer - 1]);
-    numpy arrays welcome.  conv_pre: ring slots of (128-channel group, 16-channel chunk, tap), each [half][k-panel][co][8];
-    a ConvT: slots of (NG-channel group, 16-channel chunk), each [tap][half][k-panel][phase * NG + co][8]."""
-    if layer == 0:
-        co, ci, NG = a, b, 128
-        i = ((((co // NG * 5 + ci // 16) * 7 + tap) * 2 + h) * 2 + ci % 16 // 8) * NG * 8 + co % NG * 8 + ci % 8
-        return up_base(4) + 2 * i
-    s = layer - 1
-    ci, co = a, b
-    S, NG, CIN = (8 if s < 2 else 2), (64 if s == 2 else 32), 512 >> s
-    phi, t = tap % S, tap // S
-    i = ((((co // NG * (CIN // 16) + ci // 16) * 2 + t) * 2 + h) * 2 + ci % 16 // 8) * (S * NG) * 8 + (phi * NG + co % NG) * 8 + ci % 8
-    return up_base(s) + 2 * i
-
-
-def weight_grid(layer):
-    """Index arrays over the whole weight tensor, in its torch layout."""
-    k = ("pre", "up0", "up1", "up2", "up3")[layer]
-    cin, cout, _, K = SHAPE[k]
-    dims = (cout, cin, K) if layer == 0 else (cin, cout, K)
-    return np.meshgrid(*(np.arange(n) for n in dims), indexing="ij")
-
-
-def lib_offset():
-    f = engine.lib().mg_gen_tc_weight_offset
-    f.restype = ctypes.c_size_t
-    f.argtypes = [ctypes.c_int] * 6
-    return f
-
-
 @pytest.mark.parametrize("layer", range(5))
 def test_layout_restatement_matches_the_library(layer):
     """Every weight of conv_pre and a seeded sample of each ConvT's, both halves; out-of-range arguments give -1."""
@@ -263,7 +215,7 @@ def test_layout_restatement_matches_the_library(layer):
         pick = np.random.RandomState(layer).choice(a.size, min(a.size, 20000), replace=False)
         a, b, tap = a[pick], b[pick], tap[pick]
     for h in (0, 1):
-        want = weight_offset(layer, a, b, tap, h)
+        want = gen_weight_offset(layer, a, b, tap, h)
         got = np.array([off(0, layer, int(co_or_ci), int(ci_or_co), int(t), h) for co_or_ci, ci_or_co, t in zip(
             (a if layer == 0 else b), (b if layer == 0 else a), tap)], dtype=np.int64)
         assert np.array_equal(got, want), (layer, h, int(np.argmax(got != want)))
@@ -303,20 +255,6 @@ def test_chain_kernel_refuses_bad_arguments_before_any_cuda_call():
 # ------------------------------------------------------------------------------------------------------------------
 # the emulation, and TAU_E calibrated on the CPU
 # ------------------------------------------------------------------------------------------------------------------
-def bf16_rn(v):
-    return v.to(torch.bfloat16).to(v.dtype)
-
-
-def lrelu32(x):
-    return torch.maximum(x, x * torch.tensor(0.01, dtype=torch.float32, device=x.device))
-
-
-def split_rn(v):
-    """hi = bf16_rn(v), lo = bf16_rn(v - hi) of an fp32 tensor (split2_bf16), as float64."""
-    hi = bf16_rn(v)
-    return hi.double(), bf16_rn(v - hi).double()
-
-
 def conv_fn(kernel):
     S = SHAPE[kernel][2]
     if kernel == "pre":
@@ -327,14 +265,6 @@ def conv_fn(kernel):
 def operand(kernel, x):
     """The fp32 value the kernel splits: x (conv_pre) or LeakyReLU(x) (the ConvTs)."""
     return x if kernel == "pre" else lrelu32(x)
-
-
-def emulate(kernel, ah, al, wh, wl, passes):
-    """float64 sum of the kernel's passes on given operands (no bias)."""
-    conv = conv_fn(kernel)
-    if passes == 1:
-        return conv(ah, wh)
-    return conv(ah + al, wh) + conv(ah, wl)  # (ah + al) and each product are exact in float64
 
 
 def bound(emu, a2):
@@ -368,14 +298,14 @@ def test_tau_calibration(kernel, cin, k, S):
     exact = conv(a64, w64)
     old = lambda y: float(((y - exact).abs() / (OLD_TAU * a2 + OLD_REL * exact.abs()).clamp_min(1e-300)).max())
     r = lambda y, emu: float(ratio(y, emu, a2).max())
-    emu3, emu1 = emulate(kernel, ah, al, wh, wl, 3), emulate(kernel, ah, al, wh, wl, 1)
+    emu3, emu1 = split_passes(conv, ah, al, wh, wl), split_passes(conv, ah, al, wh, wl, "bf16")
     f = lambda t: t.float()
     f32_3 = (conv(f(ah), f(wh)) + conv(f(al), f(wh)) + conv(f(ah), f(wl))).double()
     f32_1 = conv(f(ah), f(wh)).double()
     mutants = {}
     m = al.clone()
     m[:, 8:16, 150] = 0
-    mutants["lo of one k-panel of one row zeroed"] = (emulate(kernel, ah, m, wh, wl, 3), emu3)
+    mutants["lo of one k-panel of one row zeroed"] = (split_passes(conv, ah, m, wh, wl), emu3)
     drop_xl = al.clone()
     drop_xl[:, 8:16, :] = 0
     drop_wl = wl.clone()
@@ -383,14 +313,14 @@ def test_tau_calibration(kernel, cin, k, S):
         drop_wl[:, 8:16, :] = 0
     else:
         drop_wl[8:16] = 0
-    mutants["pass (xl, wh) dropped for one k-panel"] = (emulate(kernel, ah, drop_xl, wh, wl, 3), emu3)
-    mutants["pass (xh, wl) dropped for one k-panel"] = (emulate(kernel, ah, al, wh, drop_wl, 3), emu3)
+    mutants["pass (xl, wh) dropped for one k-panel"] = (split_passes(conv, ah, drop_xl, wh, wl), emu3)
+    mutants["pass (xh, wl) dropped for one k-panel"] = (split_passes(conv, ah, al, wh, drop_wl), emu3)
     trunc = (a.view(torch.int32) & -65536).view(torch.float32).double()
-    mutants["hi truncated (bf16)"] = (emulate(kernel, trunc, None, wh, None, 1), emu1)
+    mutants["hi truncated (bf16)"] = (split_passes(conv, trunc, None, wh, None, "bf16"), emu1)
     if kernel != "pre":
         xh, xl = split_rn(x)
         mutants["LeakyReLU after the split"] = (
-            emulate(kernel, bf16_rn(lrelu32(xh.float())).double(), bf16_rn(lrelu32(xl.float())).double(), wh, wl, 3), emu3)
+            split_passes(conv, bf16_rn(lrelu32(xh.float())).double(), bf16_rn(lrelu32(xl.float())).double(), wh, wl), emu3)
     clean3, clean1 = r(f32_3, emu3), r(f32_1, emu1)
     print("\n%s (Cin %d, K %d, S %d): float32 accumulation %.3f (fp32) / %.3f (bf16) of the bound" % (
         kernel, cin, k, S, clean3, clean1))
@@ -404,11 +334,6 @@ def test_tau_calibration(kernel, cin, k, S):
 # ------------------------------------------------------------------------------------------------------------------
 # GPU: the kernels
 # ------------------------------------------------------------------------------------------------------------------
-def bf16_of(blob_i16, offsets):
-    idx = torch.from_numpy(np.ascontiguousarray(offsets // 2)).to(blob_i16.device)
-    return (blob_i16[idx].to(torch.int32) << 16).view(torch.float32)
-
-
 @pytest.fixture(scope="module")
 def halves(gdev):
     """layer -> (hi, lo) of its weights in torch layout, fp32, read back from the packed blob."""
@@ -416,7 +341,7 @@ def halves(gdev):
     out = {}
     for layer in range(5):
         grid = weight_grid(layer)
-        out[layer] = tuple(bf16_of(blob, weight_offset(layer, *grid, h)) for h in (0, 1))
+        out[layer] = tuple(bf16_of(blob, gen_weight_offset(layer, *grid, h)) for h in (0, 1))
     return out
 
 
@@ -435,10 +360,6 @@ def test_blob_holds_the_split_of_the_folded_weights(g64, halves, layer):
     assert bool((d <= 2.0 ** -16 * w.abs() + 2.0 ** -40).all()), (layer, float((d / w.abs().clamp_min(1e-30)).max()))
 
 
-def nan_buffer(n):
-    return torch.full((n + GUARD,), FILL, dtype=torch.int32, device="cuda").view(torch.float32)
-
-
 def run(gdev, kernel, x, lengths=None, precision="fp32"):
     """(output [B, Cout, R L] in a FILL-ed buffer, the buffer) of a ConvT / conv_pre kernel or ResBlock chain kernel."""
     B, _, L = x.shape
@@ -454,22 +375,6 @@ def run(gdev, kernel, x, lengths=None, precision="fp32"):
         return buf[:B * cout * R * L].view(B, cout, R * L), buf
     k = kernel if isinstance(kernel, int) else CHAIN[kernel]
     return gdev.chain_kernel(k, x, lengths, precision, out=buf), buf
-
-
-def valid_mask(lengths, R, n, device="cuda"):
-    """[B, n]: True at the first R lengths[i] of n positions of item i (the outputs of its own positions)."""
-    lens = torch.tensor(lengths, device=device)
-    return torch.arange(n, device=device)[None, :] < R * lens[:, None]
-
-
-def fill_faults(y, buf, lengths, R, zero_tail=False):
-    """Items with an output past their valid ones that no longer holds FILL (zero_tail: that is not +0.0); all items
-    if the guard after the buffer was overwritten."""
-    if not bool((buf.view(torch.int32)[y.numel():] == FILL).all()):
-        return set(range(len(lengths)))
-    past = ~valid_mask(lengths, R, y.shape[-1])[:, None, :]
-    bad = (past & (y.contiguous().view(torch.int32) != (0 if zero_tail else FILL))).flatten(1).any(1)
-    return set(torch.nonzero(bad).flatten().tolist())
 
 
 def own_call_faults(gdev, kernel, x, y, lengths, R, precision):
@@ -491,7 +396,7 @@ def emulation(g64, halves, kernel, x, lengths, precision):
     ah, al = split_rn(a)
     wh, wl = (t.double() for t in halves[LAYER[kernel]])
     w64, b64 = g64.w["conv_pre" if kernel == "pre" else "ups.%d" % (LAYER[kernel] - 1)]
-    emu = emulate(kernel, ah, al, wh, wl, 3 if precision == "fp32" else 1) + b64[None, :, None]
+    emu = split_passes(conv_fn(kernel), ah, al, wh, wl, precision) + b64[None, :, None]
     a64 = a.double()
     return emu, conv_fn(kernel)(a64 * a64, w64 * w64).sqrt()
 

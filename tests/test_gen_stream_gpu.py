@@ -5,19 +5,13 @@ import numpy as np
 import pytest
 import torch
 
-from melgan_multi_b200 import engine, models, synth
-from test_ragged_gpu import border_frames
+from melgan_multi_b200 import engine, synth
+from kernel_model import gen, gstate  # noqa: F401 (fixtures)
+from kernel_model import cluster_border_frames
 
 pytestmark = pytest.mark.gpu
 
 END, RESET = engine.STREAM_END, engine.STREAM_RESET
-
-
-@pytest.fixture(scope="module")
-def gen():
-    g = models.Generator()
-    g.load_state_dict({k: torch.from_numpy(v) for k, v in synth.generator_state(1234).items()})
-    return g.cuda().eval()
 
 
 def mel_of(T, seed):
@@ -107,7 +101,7 @@ def test_chain_is_translation_invariant(gen):
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 def test_sessions_equal_their_whole_forward(gen, precision):
-    lens = [1, 2, 5, 6, 7, 31, 32, 33, 257, 1000] + border_frames()[:4]
+    lens = [1, 2, 5, 6, 7, 31, 32, 33, 257, 1000] + cluster_border_frames()[:4]
     rng = np.random.default_rng(17)
     utts = [mel_of(T, 100 + i) for i, T in enumerate(lens)]
     P = 32

@@ -1,5 +1,7 @@
 """CPU-only checks: module ABI vs the reference, C-ABI symbols, loud failure without a GPU."""
+import ast
 import ctypes
+import glob
 import json
 import os
 import re
@@ -11,6 +13,7 @@ import torch
 
 from conftest import ROOT
 from melgan_multi_b200 import engine, synth
+from kernel_model import NORMS, check_grad_digest, mel_option_cases, train_case
 
 warnings.filterwarnings("ignore")
 
@@ -224,31 +227,6 @@ def test_cabi_argument_errors_are_reported_not_thrown():
     assert L.mg_msd_scale_backward(p, 0, p, seven, seven, None, seven, seven, None, p, 16, 2, 1024, p, None) == -4
 
 
-def _train_case():
-    return dict(B=2, T=4, mel_seed=21, audio_seed=22)  # tests/golden/make_golden.py TRAIN_CASE
-
-
-def check_grad_digest(golden_grads, prefix, named_params, rtol):
-    """Every parameter's gradient against the reference digest (L2 norm, sum, first 16 values)."""
-    worst = 0.0
-    for n, p in named_params:
-        g = p.grad.detach().double().reshape(-1).cpu()
-        l2 = float(golden_grads[prefix + n + "/l2"])
-        scale = max(l2, 1e-12)
-        if n.endswith("weight_g") and g.numel() == 1:
-            # d weight_g = <dw, v> / ||v|| of a ONE-row layer (conv_post, conv_post2): a projection that cancels to a value far
-            # below |dw| |v| (1e-5 against 1e-2 at B=16), so its error is set by the size of dw, i.e. of the sibling weight_v's
-            # gradient, not by its own magnitude
-            scale = max(scale, 0.02 * float(golden_grads[prefix + n[:-1] + "v/l2"]))
-        assert abs(float(g.norm()) - l2) <= rtol * scale, (prefix, n, float(g.norm()), l2)
-        assert abs(float(g.sum()) - float(golden_grads[prefix + n + "/sum"])) <= rtol * scale * max(1.0, g.numel() ** 0.5), (prefix, n)
-        head = golden_grads[prefix + n + "/head"]
-        err = np.abs(g[:16].numpy() - head).max()
-        assert err <= rtol * max(np.abs(head).max(), scale / max(1.0, g.numel() ** 0.5)), (prefix, n, err)
-        worst = max(worst, abs(float(g.norm()) - l2) / scale)
-    return worst
-
-
 def test_backward_restatement_matches_reference_gradients():
     """The stock-op graphs the autograd path differentiates (Generator._torch_forward / MultiScaleDiscriminator.
     _torch_forward + the reference's loss formulas), run on CPU through one train.py:108-129 step, against the gradient digests of
@@ -256,7 +234,7 @@ def test_backward_restatement_matches_reference_gradients():
     import os
     from melgan_multi_b200 import models
     gg = np.load(os.path.join(os.path.dirname(__file__), "golden", "train_step_grads.npz"))
-    c = _train_case()
+    c = train_case()
     gen = models.Generator()
     gen.load_state_dict({k: torch.from_numpy(v) for k, v in synth.generator_state(1234).items()})
     msd = models.MultiScaleDiscriminator()
@@ -315,8 +293,7 @@ def test_mel_tables_match_the_oracle_filterbank():
     assert L.mg_mel_tables_build(22050, 200, ctypes.c_float(55), ctypes.c_float(9000), 1, buf.ctypes.data_as(ctypes.c_void_p)) == -1
     # every setting of the GPU option sweep (tests/test_mel_isolation_gpu.py) against the float64 filter bank: the sparse
     # runs hold exactly the positive bins, and each weight is its float64 value to fp32 rounding
-    from test_mel_isolation_gpu import _option_cases, NORMS
-    for sr, n_mels, fmin, fmax, norm in _option_cases():
+    for sr, n_mels, fmin, fmax, norm in mel_option_cases():
         assert L.mg_mel_tables_build(sr, n_mels, ctypes.c_float(fmin), ctypes.c_float(fmax), norm, buf.ctypes.data_as(ctypes.c_void_p)) == 0
         ib = buf.view(np.int32)
         assert ib[2048] == n_mels
@@ -335,3 +312,19 @@ def test_mel_tables_match_the_oracle_filterbank():
     from melgan_multi_b200 import meldataset
     with pytest.raises(engine.EngineError):
         meldataset.mel_spectrogram(torch.zeros(8192), 1024, 80, 22050, 256, 1024, 55, 9000)
+
+
+def test_no_test_module_imports_another():
+    """Test modules share code through kernel_model (or conftest), never by importing each other: a test file can then be
+    renamed or split without breaking unrelated ones."""
+    bad = []
+    for path in sorted(glob.glob(os.path.join(ROOT, "tests", "test_*.py"))):
+        for node in ast.walk(ast.parse(open(path).read(), path)):
+            if isinstance(node, ast.Import):
+                names = [a.name for a in node.names]
+            elif isinstance(node, ast.ImportFrom) and not node.level:
+                names = [node.module]
+            else:
+                continue
+            bad += ["%s:%d imports %s" % (os.path.basename(path), node.lineno, n) for n in names if n.startswith("test_")]
+    assert not bad, bad

@@ -21,90 +21,19 @@ branch error (plain ResBlocks), worst (error near a border) / (error elsewhere) 
 Every chain variant (tail masks 0, 2, .., 14) against float64: worst per-item error 7.0e-6 at (3, 5), 9.3e-6 at (40, 32).
 """
 import ctypes
-import re
 
 import numpy as np
 import pytest
 import torch
 
 from melgan_multi_b200 import engine, models, synth
-from test_layer_isolation_gpu import BRANCH_TOL, ROW_TOL, Gen64, g64, gdev, gstate, row_errors  # noqa: F401 (fixtures)
+from kernel_model import g64, gdev, gstate  # noqa: F401 (fixtures)
+from kernel_model import (BAND, BRANCH_TOL, ROW_TOL, borders, config, ctas, input_shape, lengths, parse_config, row_errors,
+                          run_with_reference)
 
 CODES = (0, 1, 2, 3, 4, 12, 13, 14, 20, 21, 22)
-BAND = 20        # rows either side of a border
 BORDER_X = 4.0   # border error <= BORDER_X * interior error + FLOOR
 FLOOR = 1e-7
-
-
-# ------------------------------------------------------------------------------------------------------------------
-# geometry (pure functions: tested without a GPU)
-# ------------------------------------------------------------------------------------------------------------------
-def parse_config(name):
-    """"resblock_tc_kernel<RbCfg<C,NRB,RPW,NCP,NSTAGE,POST,UPF,UPT,CS>>" -> dict with the tiling constants."""
-    m = re.fullmatch(r"resblock_tc_kernel<RbCfg<(\d+(?:,\d+){8})>>", name)
-    if not m:
-        raise ValueError("not a ResBlock configuration: %r" % (name,))
-    C, NRB, RPW, NCP, NSTAGE, POST, UPF, UPT, CS = (int(v) for v in m.group(1).split(","))
-    g = dict(C=C, NRB=NRB, RPW=RPW, NCP=NCP, NSTAGE=NSTAGE, POST=POST, UPF=UPF, UPT=UPT, CS=CS)
-    g["P"] = 64 * NRB
-    g["HALO"] = 16 + 3 * POST
-    g["HL"] = g["HALO"] + (UPT > 0)
-    g["PC"] = CS * g["P"]
-    g["PVB"] = g["PC"] - g["HALO"] - g["HL"]
-    return g
-
-
-def config(code):
-    return parse_config(engine.lib().mg_gen_resblock_config(code).decode())
-
-
-def ctas(g, L):
-    """[(cluster, rank, o, first owned, end of owned)] of one item at length L, positions in the ResBlock's own
-    coordinates; exactly the index arithmetic of resblock_tc_kernel."""
-    P, CS, PC, PVB, HALO, HL = g["P"], g["CS"], g["PC"], g["PVB"], g["HALO"], g["HL"]
-    n = 1 + ((L - PC + PVB - 1) // PVB if L > PC else 0)
-    out = []
-    for c in range(n):
-        oc = 0 if c == 0 else (PC - HALO) + (c - 1) * PVB - HL
-        for r in range(CS):
-            o = oc + r * P
-            p_lo = 0 if (c == 0 or r > 0) else HL
-            p_hi = P if (r < CS - 1 or oc + PC >= L) else P - HALO
-            out.append((c, r, o, o + p_lo, min(o + p_hi, L)))
-    return out
-
-
-def borders(g, L):
-    """Positions where ownership passes from one CTA to the next (cluster and CTA-rank borders) inside [1, L)."""
-    return sorted({lo for (_c, _r, _o, lo, hi) in ctas(g, L) if 0 < lo < L and hi > lo})
-
-
-def lengths(g):
-    """Lengths that put a border next to the end of the sequence or a CTA at a special fill."""
-    P, CS, PC, PVB, HALO, HL = g["P"], g["CS"], g["PC"], g["PVB"], g["HALO"], g["HL"]
-    out = set()
-    for k in range(3):  # the first three cluster borders: ownership border, and the length at which cluster k + 1 appears
-        for b in (PC - HALO + k * PVB, PC + k * PVB):
-            out |= {b - 1, b, b + 1}
-    if CS > 1:  # the first CTA-rank border inside a cluster
-        out |= {P - 1, P, P + 1}
-    for c in (1, 2):  # the last cluster (the second or third) with 1, 2, .. CS CTAs holding rows
-        oc = PC - HALO + (c - 1) * PVB - HL
-        lo_L, hi_L = PC + (c - 1) * PVB + 1, PC + c * PVB  # lengths with exactly c + 1 clusters
-        for m in range(1, CS + 1):
-            a, b = max(oc + (m - 1) * P + 1, lo_L), min(oc + m * P, hi_L)
-            if a <= b:
-                out |= {a, b}
-    for c in range(3):  # L - 1 on the first or the last row of a CTA (the tail ConvT's fp32 fix-up for position L)
-        oc = 0 if c == 0 else PC - HALO + (c - 1) * PVB - HL
-        for r in range(CS):
-            o = oc + r * P
-            for L in (o + 1, o + P):
-                if any(oo in (L - 1, L - P) and lo <= L - 1 < hi for (_c, _r, oo, lo, hi) in ctas(g, L)):
-                    out.add(L)
-    if g["UPF"]:  # the output length of a stride-2 ConvT is even: the even neighbours of an odd length
-        out = {v for L in out for v in ((L,) if L % 2 == 0 else (L - 1, L + 1))}
-    return sorted(L for L in out if L >= 1)
 
 
 def test_config_strings_parse_for_every_stage_code():
@@ -149,29 +78,6 @@ def test_parser_and_lengths_on_known_geometry():
 # ------------------------------------------------------------------------------------------------------------------
 # the sweep
 # ------------------------------------------------------------------------------------------------------------------
-def run_code(dev, g64, code, x):
-    """(kernel output, float64 reference, float64 ResBlock input or None) of stage code `code` on x."""
-    x64 = x.double()
-    if code <= 3:
-        return dev.resblock(code, x), g64.resblock(code, x64), x64
-    if code == 4:
-        return dev.resblock_post(x), g64.post(g64.resblock(3, x64)), None
-    if code in (12, 13):
-        s = code - 10
-        c64 = g64.convt(s, x64)
-        return dev.upres(s, x), g64.resblock(s, c64), c64
-    if code == 14:
-        return dev.upres_post(x), g64.post(g64.resblock(3, g64.convt(3, x64))), None
-    s = code - 20
-    return dev.resup(s, x), g64.convt(s + 1, g64.resblock(s, x64)), None
-
-
-def input_shape(g, code, B, L):
-    if g["UPF"]:
-        return (B, 2 * g["C"], L // 2)
-    return (B, g["C"], L)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("code", CODES)
 def test_border_sweep(gdev, g64, code):
@@ -183,7 +89,7 @@ def test_border_sweep(gdev, g64, code):
         for B in (1, 3):
             rs = np.random.RandomState(code * 100003 + L * 7 + B)
             x = torch.from_numpy(rs.standard_normal(input_shape(g, code, B, L)).astype(np.float32)).cuda()
-            y, ref, x64 = run_code(gdev, g64, code, x)
+            y, ref, x64 = run_with_reference(gdev, g64, code, x)
             assert y.shape == ref.shape, (code, L, tuple(y.shape), tuple(ref.shape))
             e = row_errors(y, ref)
             rows = float(e.max())

@@ -29,94 +29,18 @@ Worst per-row max|d| / max|ref| (branch alone in brackets), config 2 / config 5:
     up2+res2 1.7e-5 (4.5e-5) / 1.6e-5 (4.7e-5), up3+res3+post 6.5e-6 / 8.4e-6
 (The branch of up0+res0 also carries the ConvT kernel's own error, which the float64 input of the branch does not.)
 """
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
 from melgan_multi_b200 import engine, synth
-
-TAU = 2.0 ** -12
-REL = 2.0 ** -20
-ROW_TOL = 1e-4      # per (item, channel) row, max|d| / max|ref|
-BRANCH_TOL = 3e-4   # the residual branch (y - x) alone, per row
-DILATIONS = (1, 3, 9)
+from kernel_model import ddev, dstate, g64, gdev, gstate  # noqa: F401 (fixtures)
+from kernel_model import BRANCH_TOL, ROW_TOL, conv_bound_ratio, folded64, row_errors, split_conv
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# float64 restatements of the layers (reference models.py:32-40, 61-71, 87-103)
+# the bound itself, calibrated on the CPU (split_conv: the split's arithmetic, conv_bound_ratio: the bound; kernel_model)
 # ------------------------------------------------------------------------------------------------------------------
-def folded64(state, name, device="cuda"):
-    w = synth.fold_weight_norm(state[name + ".weight_g"], state[name + ".weight_v"])
-    return (torch.from_numpy(w).to(device, torch.float64), torch.from_numpy(state[name + ".bias"]).to(device, torch.float64))
-
-
-class Gen64:
-    """The generator's layers in float64 on the GPU."""
-
-    def __init__(self, state, device="cuda"):
-        self.w = {n: folded64(state, n, device) for n, *_ in synth.GENERATOR_LAYERS}
-
-    def conv_pre(self, mel):
-        w, b = self.w["conv_pre"]
-        return F.conv1d(mel, w, b, padding=3)
-
-    def convt(self, stage, x):
-        w, b = self.w["ups.%d" % stage]
-        k = w.shape[2]
-        return F.conv_transpose1d(F.leaky_relu(x), w, b, stride=k // 2, padding=k // 4)
-
-    def resblock(self, stage, x):
-        for j, d in enumerate(DILATIONS):
-            w1, b1 = self.w["resblocks.%d.convs1.%d" % (stage, j)]
-            w2, b2 = self.w["resblocks.%d.convs2.%d" % (stage, j)]
-            h = F.conv1d(F.leaky_relu(x), w1, b1, padding=d, dilation=d)
-            x = F.conv1d(F.leaky_relu(h), w2, b2, padding=1) + x
-        return x
-
-    def post(self, x):
-        w, b = self.w["conv_post"]
-        return torch.tanh(F.conv1d(F.leaky_relu(x), w, b, padding=3))
-
-
-def conv_bound_ratio(got, x64, w64, b64, stride=1, padding=0, groups=1, lrelu=False, tau=TAU):
-    """Worst |y - y64| / (tau A2 + 2^-20 |y64 before the activation|) of one conv (<= 1: within the bound)."""
-    pre = F.conv1d(x64, w64, b64, stride=stride, padding=padding, groups=groups)
-    a2 = F.conv1d(x64 * x64, w64 * w64, None, stride=stride, padding=padding, groups=groups).sqrt()
-    ref = F.leaky_relu(pre) if lrelu else pre
-    assert got.shape == ref.shape, (tuple(got.shape), tuple(ref.shape))
-    d = (got.double() - ref).abs()
-    return float((d / (tau * a2 + REL * pre.abs()).clamp_min(1e-300)).max())
-
-
-def row_errors(got, ref):
-    """|got - ref| / max|ref| of its (item, channel) row, element-wise.  The row scale is at least 1/8 of the largest
-    |ref| of the call: a row of a few positions can cancel to near zero (y = x + branch at L = 1), and its error is then
-    that of the rows around it, not a fraction of its own value."""
-    d = (got.double() - ref).abs()
-    a = ref.abs()
-    return d / a.amax(dim=-1, keepdim=True).clamp_min(float(a.max()) / 8).clamp_min(1e-30)
-
-
-# ------------------------------------------------------------------------------------------------------------------
-# the bound itself, calibrated on the CPU
-# ------------------------------------------------------------------------------------------------------------------
-def _bf16(t):
-    return t.to(torch.bfloat16).to(t.dtype)
-
-
-def split_conv(x, w, stride, padding, groups, passes=(0, 1, 2)):
-    """The tensor cores' arithmetic on fp32 operands: hi = bf16(v), lo = bf16(v - hi); passes (xh, wh), (xl, wh), (xh, wl)
-    accumulated in fp32."""
-    xh, wh = _bf16(x), _bf16(w)
-    xl, wl = _bf16(x - xh), _bf16(w - wh)
-    ops = [(xh, wh), (xl, wh), (xh, wl)]
-    y = torch.zeros(())
-    for p in passes:
-        y = y + F.conv1d(ops[p][0], ops[p][1], None, stride=stride, padding=padding, groups=groups)
-    return y
-
-
 # (Cin, Cout, k, stride, groups): K = Cin / groups * k from 15 to 5120 -- the discriminators' conv_pre, a grouped conv,
 # the generator's conv_pre and ResBlock convs, conv_post2, conv_post1
 CALIBRATION = [(1, 16, 15, 1, 1), (64, 64, 41, 4, 16), (80, 128, 7, 1, 1), (256, 64, 3, 1, 1), (1024, 1, 3, 1, 1),
@@ -145,26 +69,6 @@ def test_tau_calibration_on_emulated_split_bf16(cin, cout, k, stride, groups):
 # ------------------------------------------------------------------------------------------------------------------
 CHAIN = ["conv_pre", "up0", "res0", "up1", "res1", "up2", "res2", "up3+res3+post"]
 ITEMS = (0, 15, 16, 31, 32, 47, 48, 63)  # the borders of config 2's four batch slices
-
-
-@pytest.fixture(scope="module")
-def gstate():
-    return synth.generator_state(1234)
-
-
-@pytest.fixture(scope="module")
-def gdev(gstate):
-    gd = engine.GeneratorDevice("cuda:0")
-    order = [n for n, *_ in synth.GENERATOR_LAYERS]
-    to = lambda a: torch.from_numpy(a).cuda()
-    gd.pack([to(gstate[n + ".weight_v"]) for n in order], [to(gstate[n + ".weight_g"]) for n in order],
-            [to(gstate[n + ".bias"]) for n in order])
-    return gd
-
-
-@pytest.fixture(scope="module")
-def g64(gstate):
-    return Gen64(gstate)
 
 
 @pytest.mark.gpu
@@ -208,21 +112,6 @@ def test_generator_layers_on_their_own_inputs(gdev, g64, B, T):
 # ------------------------------------------------------------------------------------------------------------------
 # discriminators: all 21 layers, layer l on the feature map the engine returned for layer l - 1
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def dstate():
-    return synth.discriminator_state(4321)
-
-
-@pytest.fixture(scope="module")
-def ddev(dstate):
-    dd = engine.DiscriminatorDevice("cuda:0")
-    names = ["discriminators.%d.%s" % (d, n) for d in range(3) for n, *_ in synth.DISCRIMINATOR_LAYERS]
-    to = lambda a: torch.from_numpy(a).cuda()
-    dd.pack([to(dstate[n + ".weight_v"]) for n in names], [to(dstate[n + ".weight_g"]) for n in names],
-            [to(dstate[n + ".bias"]) for n in names])
-    return dd
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("Bt,L", [(32, 8192), (2, 64), (6, 257), (4, 2050), (2, 4097)])
 def test_discriminator_layers_on_their_own_inputs(ddev, dstate, Bt, L):

@@ -23,7 +23,6 @@ What this anchors is the kernel against its own restatement of librosa's algorit
 parity with it stays unpinned (DESIGN.md section 2).
 """
 import ctypes
-import random
 
 import numpy as np
 import pytest
@@ -31,14 +30,13 @@ import torch
 
 from melgan_multi_b200 import engine, meldataset
 from oracle import mel_oracle as mo
+from kernel_model import DEFAULT, NORMS, mel_option_cases
 
 TAU_F = 2.0 ** -17
 U = 2.0 ** -24
 CLIP = 1e-5
 NFFT, HOP, PAD = 1024, 256, 384
 WIN64 = 0.5 - 0.5 * np.cos(2 * np.pi * np.arange(NFFT) / NFFT)   # periodic Hann
-DEFAULT = (22050, 80, 55.0, 9000.0, 1)                           # the reference's config.json: sr, n_mels, fmin, fmax, norm
-NORMS = {0: None, 1: 1, 2: "l1"}
 
 
 def frames_of(y, shift=0):
@@ -215,32 +213,16 @@ def _check(y, got, opts, floor):
     return worst
 
 
-def _option_cases():
-    full = []
-    for sr in (16000, 22050, 24000, 44100):
-        for n_mels in (1, 40, 80, 128):
-            for norm in (0, 1, 2):
-                for fmin in (0.0, 55.0):
-                    for fmax in sorted({8000.0, 9000.0, sr / 2.0}):
-                        if fmax <= sr / 2.0:
-                            full.append((sr, n_mels, fmin, fmax, norm))
-    picked = random.Random(2024).sample(full, 28)
-    # the reference's setting; every thread of a frame a mel (128) at each norm; filters that cover no bin
-    must = [DEFAULT, (44100, 128, 0.0, 22050.0, 0), (44100, 128, 55.0, 9000.0, 1), (22050, 128, 0.0, 11025.0, 2),
-            (16000, 1, 0.0, 8000.0, 1), (44100, 128, 0.0, 4000.0, 1)]
-    return must + [c for c in picked if c not in must]
-
-
 @pytest.mark.gpu
 def test_option_sweep_against_float64(floor):
     """Sampling rates, 1 - 128 mels, norm none / Slaney / L1, fmin 0 / 55, fmax 8000 / 9000 / sr/2."""
     worst = 0.0
-    for i, opts in enumerate(_option_cases()):
+    for i, opts in enumerate(mel_option_cases()):
         y = _signals(8192 + 77 * i, 100 + i)
         r = _check(y, _gpu_mel(y, *opts), opts, floor)
         assert r <= 1, (opts, r)
         worst = max(worst, r)
-    print("\noption sweep (%d settings): worst %.3f of the bound" % (len(_option_cases()), worst))
+    print("\noption sweep (%d settings): worst %.3f of the bound" % (len(mel_option_cases()), worst))
 
 
 def test_empty_filters_sit_on_the_clip_floor():
@@ -248,7 +230,7 @@ def test_empty_filters_sit_on_the_clip_floor():
     reaches 8 kHz): the tables give them no bins, and the GPU sweep checks their rows are the floor."""
     fb = mo.mel_filterbank64(44100, NFFT, 128, 0.0, 4000.0, 1)
     assert ((fb > 0).sum(axis=1) == 0).sum() >= 5
-    assert (44100, 128, 0.0, 4000.0, 1) in _option_cases()
+    assert (44100, 128, 0.0, 4000.0, 1) in mel_option_cases()
 
 
 def _frames(L):

@@ -18,45 +18,13 @@ import numpy as np
 import pytest
 import torch
 
-from melgan_multi_b200 import engine, synth
-from test_bf16_inference_gpu import _emulation_bound, gen  # noqa: F401 (fixture)
-from test_kernel_borders_gpu import config, lengths, input_shape, run_code
-from test_layer_isolation_gpu import ROW_TOL, Gen64, g64, gdev, gstate, row_errors  # noqa: F401 (fixtures)
+from melgan_multi_b200 import synth
+from kernel_model import g64, gdev, gen, gstate  # noqa: F401 (fixtures)
+from kernel_model import (ROW_TOL, bf16_emulation_bound, bf16_of, config, fp32_blob_bytes, front_index, in_chunk,
+                          input_shape, lengths, lib_offset, res_base, res_index, row_errors, run_with_reference, tc_kc)
 
 NARROW = (64, 32)
 STAGE_OF = {64: 2, 32: 3}
-
-
-def tc_kc(C):
-    return 4096 // C if C >= 128 else C
-
-
-def fp32_blob_bytes():
-    n = 80 * 512 * 7 + 32 * 7 + 512 + 1
-    for i in range(4):
-        cin, cout, k = 512 >> i, 256 >> i, (16 if i < 2 else 4)
-        n += cin * cout * k + cout + 6 * (cout * cout * 3 + cout)
-    return (n * 4 + 255) // 256 * 256
-
-
-def res_base(layer):
-    """Byte offset of a ResBlock conv's tensor-core block: after the fp32 blob, 12 C^2 bytes per conv in layer order."""
-    return fp32_blob_bytes() + sum(12 * (256 >> ((l - 5) // 6)) ** 2 for l in range(5, layer))
-
-
-def in_chunk(C, co, cik, h):
-    """bf16 element index inside a chunk (numpy arrays welcome): stacked for C <= 64, halves back to back above."""
-    KC = tc_kc(C)
-    if C <= 64:
-        return ((cik // 8 * 2 + h) * C + co) * 8 + cik % 8
-    return ((h * (KC // 8) + cik // 8) * C + co) * 8 + cik % 8
-
-
-def lib_offset():
-    f = engine.lib().mg_gen_tc_weight_offset
-    f.restype = ctypes.c_size_t
-    f.argtypes = [ctypes.c_int] * 6
-    return f
 
 
 @pytest.mark.parametrize("C", NARROW + (128,))
@@ -99,30 +67,22 @@ def test_front_convt_chunks_are_stacked_too(C):
     assert off(1, 1, 0, 0, 0, 0) == ctypes.c_size_t(-1).value and off(0, 29, 0, 0, 0, 0) == ctypes.c_size_t(-1).value
 
 
-def _bf16_at(blob_u16, byte_offsets):
-    v = blob_u16[torch.from_numpy(byte_offsets // 2).cuda()].to(torch.int32) << 16
-    return v.view(torch.float32).double()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("C", NARROW)
 def test_packed_blob_holds_hi_and_lo_where_the_descriptors_read_them(gdev, g64, C):
-    blob = gdev.packed.view(torch.int16).to(torch.int32) & 0xFFFF
-    stage, KC = STAGE_OF[C], tc_kc(C)
+    blob = gdev.packed.view(torch.int16)
+    stage = STAGE_OF[C]
     co, ci, tap = np.meshgrid(np.arange(C), np.arange(C), np.arange(3), indexing="ij")
     for j in range(3):
         for which in ("convs1", "convs2"):
             layer = 5 + 6 * stage + j + (3 if which == "convs2" else 0)
             w = g64.w["resblocks.%d.%s.%d" % (stage, which, j)][0]  # [co][ci][tap], float64
-            idx = lambda h: res_base(layer) + 2 * ((tap * (C // KC) + ci // KC) * 2 * KC * C + in_chunk(C, co, ci % KC, h))
-            hi, lo = _bf16_at(blob, idx(0)), _bf16_at(blob, idx(1))
+            hi, lo = (bf16_of(blob, res_index(C, layer, co, ci, tap, h)).double() for h in (0, 1))
             assert float((hi + lo - w).abs().max()) <= 2.0 ** -15 * float(w.abs().max()), (layer, "hi + lo")
             assert bool((lo.abs() <= 2.0 ** -8 * hi.abs() + 1e-30).all()), (layer, "lo rows")
     w = g64.w["ups.%d" % stage][0]  # [ci][co][k]
     ci, co, k = np.meshgrid(np.arange(2 * C), np.arange(C), np.arange(4), indexing="ij")
-    base = lib_offset()(1, stage, 0, 0, 0, 0)
-    idx = lambda h: base + 2 * ((k * (2 * C // KC) + ci // KC) * 2 * KC * C + in_chunk(C, co, ci % KC, h))
-    hi, lo = _bf16_at(blob, idx(0)), _bf16_at(blob, idx(1))
+    hi, lo = (bf16_of(blob, front_index(C, stage, ci, co, k, h)).double() for h in (0, 1))
     assert float((hi + lo - w).abs().max()) <= 2.0 ** -15 * float(w.abs().max())
     assert bool((lo.abs() <= 2.0 ** -8 * hi.abs() + 1e-30).all())
 
@@ -136,7 +96,7 @@ def test_narrow_codes_at_tile_borders(gdev, g64, code):
         for B in (1, 3):
             rs = np.random.RandomState(code * 7919 + L * 13 + B)
             x = torch.from_numpy(rs.standard_normal(input_shape(g, code, B, L)).astype(np.float32)).cuda()
-            y, ref, _x64 = run_code(gdev, g64, code, x)
+            y, ref, _x64 = run_with_reference(gdev, g64, code, x)
             assert y.shape == ref.shape
             e = float(row_errors(y, ref).max())
             assert e < ROW_TOL, (code, B, L, e)
@@ -151,5 +111,5 @@ def test_bf16_variants_at_their_borders(gen, g64, code, per_frame):
     worst = 0.0
     for T in Ts:
         mel = torch.from_numpy(synth.mel_input(1, T, 700 + T)).cuda()
-        worst = max(worst, _emulation_bound(gen, g64, mel, (code, T))[4])
+        worst = max(worst, bf16_emulation_bound(gen, g64, mel, (code, T))[4])
     print("\nbf16 code %d: T = %s, worst (kernel - 2e-5) / emulation %.2f" % (code, Ts, worst))

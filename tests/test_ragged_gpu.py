@@ -3,7 +3,7 @@ different lengths equals that utterance's own forward bit for bit, and the audio
 
 The kernels place their tiles per item and apply each item's zero padding at the item's own end, so the per-item
 arithmetic of a ragged batch is the single-item forward's.  The lengths include the stage-0 and stage-1 ResBlock
-cluster and CTA-rank borders (test_kernel_borders_gpu.lengths) mapped back to mel frames, so a border sits at or next
+cluster and CTA-rank borders (kernel_model.lengths) mapped back to mel frames, so a border sits at or next
 to an item's end; the mel past every length is NaN, which any read would carry into the audio."""
 import numpy as np
 import pytest
@@ -11,55 +11,16 @@ import torch
 
 import cases
 from conftest import rel_errors
-from melgan_multi_b200 import engine, models, synth
-from test_kernel_borders_gpu import config, lengths as border_lengths
+from melgan_multi_b200 import engine, synth
+from kernel_model import gen, gstate  # noqa: F401 (fixtures)
+from kernel_model import check_items, cluster_border_frames, ragged_batch
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4  # test_generator_gpu's bound against the reference
 
 
-@pytest.fixture(scope="module")
-def state():
-    return synth.generator_state(1234)
-
-
-@pytest.fixture(scope="module")
-def gen(state):
-    g = models.Generator()
-    g.load_state_dict({k: torch.from_numpy(v) for k, v in state.items()})
-    return g.cuda().eval()
-
-
-def ragged_batch(lens, seed):
-    """mel [B, 80, max(lens)] of seeded per-item inputs, NaN past each length."""
-    T = max(lens)
-    mel = np.full((len(lens), 80, T), np.nan, np.float32)
-    for i, L in enumerate(lens):
-        mel[i, :, :L] = synth.mel_input(1, L, seed + i)[0]
-    return torch.from_numpy(mel).cuda()
-
-
-def check_items(gen, mel, lens, audio):
-    assert audio.shape == (len(lens), 1, 256 * mel.shape[2])
-    with torch.no_grad():
-        for i, L in enumerate(lens):
-            own = gen(mel[i:i + 1, :, :L].contiguous())
-            assert torch.equal(audio[i:i + 1, :, :256 * L], own), (i, L)
-            assert bool((audio[i, :, 256 * L:] == 0).all()), (i, L)
-    gen._dev.check_status(len(lens), mel.shape[2])
-
-
-def border_frames():
-    """Mel lengths whose stage-0 (x8) or stage-1 (x64) length lies at or next to a cluster or CTA-rank border."""
-    out = set()
-    for code, scale in ((0, 8), (1, 64)):
-        for L in border_lengths(config(code)):
-            out |= {max(1, L // scale), (L + scale - 1) // scale}
-    return sorted(out)
-
-
 def test_per_item_bit_identity(gen):
-    lens = sorted({1, 2, 3, 7, 31, 32, 33, 1000} | set(border_frames()))
+    lens = sorted({1, 2, 3, 7, 31, 32, 33, 1000} | set(cluster_border_frames()))
     assert len(lens) <= 256  # MG_GEN_RAGGED_MAX_B
     rng = np.random.default_rng(7)
     lens = [int(v) for v in rng.permutation(lens)]
@@ -141,13 +102,13 @@ def test_stage_taps(gen):
         engine.check(engine.lib().mg_gen_set_pipeline(-1))
 
 
-def test_host_engine_equals_device_path(gen, state):
+def test_host_engine_equals_device_path(gen, gstate):
     lens = [40, 7, 1, 64, 33]
     mel = ragged_batch(lens, 900)
     ref = gen.generate(mel, lens).cpu().numpy()
     gen._dev.check_status(len(lens), max(lens))
     host = engine.GeneratorHost(2, 8)
-    host.load_state(state)
+    host.load_state(gstate)
     try:
         mel_np = mel.cpu().numpy()
         assert np.array_equal(host.forward_ragged(mel_np, lens), ref)  # pageable buffers

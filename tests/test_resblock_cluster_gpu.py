@@ -6,7 +6,8 @@ import pytest
 import torch
 
 from conftest import rel_errors
-from test_tc_gpu import TOL, dev, oracle_resblock, state  # noqa: F401 (fixtures)
+from kernel_model import gdev, gstate  # noqa: F401 (fixtures)
+from kernel_model import TOL, oracle_resblock
 
 pytestmark = pytest.mark.gpu
 
@@ -27,11 +28,11 @@ def _lengths(stage):
 
 @pytest.mark.parametrize("stage,B,L", [(s, B, L) for s in (0, 1) for L in _lengths(s) for B in (1, 3)]
                          + [(0, 64, 256), (1, 2, 2048), (1, 1, 1000)])
-def test_clustered_resblock_matches_oracle(state, dev, stage, B, L):  # noqa: F811
+def test_clustered_resblock_matches_oracle(gstate, gdev, stage, B, L):
     C = 256 >> stage
     rs = np.random.RandomState(1000 * stage + L + B)
     x = rs.standard_normal((B, C, L)).astype(np.float32)
-    ref = oracle_resblock(state, stage, x)
-    y = dev.resblock(stage, torch.from_numpy(x).cuda()).cpu().numpy()
+    ref = oracle_resblock(gstate, stage, x)
+    y = gdev.resblock(stage, torch.from_numpy(x).cuda()).cpu().numpy()
     m, l2 = rel_errors(y, ref)
     assert m < TOL and l2 < TOL, (stage, B, L, m, l2)

@@ -82,12 +82,10 @@ import torch
 import torch.nn.functional as F
 
 from melgan_multi_b200 import engine, synth
-from test_gen_front_kernels_gpu import (REL_E, TAU_E, MUTANT_X, bf16_of, bf16_rn, fill_faults, lrelu32, nan_buffer,
-                                        split_rn, weight_grid)
-from test_gen_front_kernels_gpu import weight_offset as up_offset
-from test_kernel_borders_gpu import BAND, borders, config, input_shape, lengths
-from test_layer_isolation_gpu import DILATIONS, Gen64, gstate  # noqa: F401 (fixture)
-from test_narrow_stage_gpu import in_chunk, lib_offset, res_base, tc_kc
+from kernel_model import gstate  # noqa: F401 (fixture)
+from kernel_model import (BAND, DILATIONS, MUTANT_X, REL_E, TAU_E, Gen64, bf16_of, bf16_rn, borders, config, fill_faults,
+                          front_index, gen_weight_offset, input_shape, lengths, lrelu32, nan_buffer, res_index, split_op,
+                          split_passes, split_rn, weight_grid)
 
 RHO = 11 * 2.0 ** -20  # residual term of a C >= 128 c2 (per |x|): about twice the worst measured (module docstring)
 HL_E = 2.0 ** -16    # |hi + lo - v| <= 2^-16 |v| (two bf16 roundings of 8 significant bits)
@@ -210,15 +208,6 @@ def conv_d(a, w, d):
     return F.conv1d(a, w, padding=d, dilation=d)
 
 
-def passes(conv, ah, al, wh, wl, prec):
-    return conv(ah, wh) if prec == "bf16" else conv(ah + al, wh) + conv(ah, wl)
-
-
-def split_op(a, prec):
-    ah, al = split_rn(a)
-    return ah, (None if prec == "bf16" else al)
-
-
 def resblock_emu(P, s, r, prec):
     """(mid, rad, rabs) of ResBlock s on the exact fp32 input r; rad excludes RHO * rabs."""
     pat, r64 = P.pat, r.double()
@@ -235,7 +224,7 @@ def resblock_emu(P, s, r, prec):
     if pat[:2] == "c1":
         w64, b64 = P.g64.w["resblocks.%d.convs1.%d" % (s, j)]
         wh, wl = P.halves[("c1", s, j)]
-        h = passes(lambda u, w: conv_d(u, w, d), ah, al, wh, wl, prec) + b64[None, :, None]
+        h = split_passes(lambda u, w: conv_d(u, w, d), ah, al, wh, wl, prec) + b64[None, :, None]
         a64 = a.double()
         B = TAU_E * conv_d(a64 * a64, w64 * w64, d).sqrt() + REL_E * h.abs()
         vlo, vhi = F.leaky_relu(h - B), F.leaky_relu(h + B)
@@ -253,7 +242,7 @@ def resblock_emu(P, s, r, prec):
     vh, vl = split_op(v, prec)
     w64, _ = P.g64.w["resblocks.%d.convs2.%d" % (s, j)]
     wh, wl = P.halves[("c2", s, j)]
-    c = passes(lambda u, w: conv_d(u, w, 1), vh, vl, wh, wl, prec)
+    c = split_passes(lambda u, w: conv_d(u, w, 1), vh, vl, wh, wl, prec)
     v64 = v.double()
     mid = base + c
     rad = TAU_E * conv_d(v64 * v64, w64 * w64, 1).sqrt() + REL_E * c.abs() + ULP_E * (
@@ -274,7 +263,7 @@ def front_emu(P, s, x, prec):
         return (conv(hl, w01).float() + b), None
     w64, b64 = P.g64.w["ups.%d" % s]
     wh, wl = P.halves[("front", s, 0)]
-    mid = passes(conv, ah, al, wh, wl, prec) + b64[None, :, None]
+    mid = split_passes(conv, ah, al, wh, wl, prec) + b64[None, :, None]
     a64 = a.double()
     return mid, TAU_E * conv(a64 * a64, w64 * w64).sqrt() + REL_E * mid.abs()
 
@@ -303,7 +292,7 @@ def tail_emu(P, s, mid, rad):
     a = lrelu32(mid.float())  # (fused: the ResBlock output is exact, rad is a few ulps)
     ah, al = split_rn(a)
     wh, wl = P.halves[("tail", s, 0)]
-    out = passes(conv, ah, al, wh, wl, "fp32") + bias
+    out = split_passes(conv, ah, al, wh, wl, "fp32") + bias
     a64 = a.double()
     rad_out = TAU_E * conv(a64 * a64, w64 * w64).sqrt() + REL_E * out.abs() + conv(rad, w64.abs())
     # fix-up: outputs [S L - pad, S L) from x[L - 1] and the fp32 weights
@@ -367,7 +356,7 @@ def cpu_halves(state):
 
 
 def reference64(g, code, x):
-    """The float64 layers (test_layer_isolation_gpu.Gen64) of stage code `code`."""
+    """The float64 layers (kernel_model.Gen64) of stage code `code`."""
     s = STAGE[code]
     if code in (12, 13, 14):
         x = g.convt(s, x)
@@ -423,7 +412,7 @@ def test_calibration(C, d, kind):
         c = (emu - r64).abs()
         return float(((y.double() - emu).abs() / (TAU_E * a2 + REL_E * c + res)).max())
 
-    emu3, emu1 = r64 + passes(conv, ah, al, wh, wl, "fp32"), r64 + passes(conv, ah, al, wh, wl, "bf16")
+    emu3, emu1 = r64 + split_passes(conv, ah, al, wh, wl, "fp32"), r64 + split_passes(conv, ah, al, wh, wl, "bf16")
     # float32, in the kernel's order: per (tap, 16-channel k-step, pass) an fp32 partial sum onto the accumulator
     f = lambda t: t.float()
 
@@ -442,11 +431,11 @@ def test_calibration(C, d, kind):
     mutants = {}
     m = al.clone()
     m[:, 8:16, 150] = 0
-    mutants["lo of one k-panel of one row zeroed"] = (r64 + passes(conv, ah, m, wh, wl, "fp32"), emu3)
+    mutants["lo of one k-panel of one row zeroed"] = (r64 + split_passes(conv, ah, m, wh, wl, "fp32"), emu3)
     dwl = wl.clone()
     dwl[:, 16:32, 1] = 0
-    mutants["xh * wl of one stacked k-step dropped"] = (r64 + passes(conv, ah, al, wh, dwl, "fp32"), emu3)
-    mutants["pass (xl, wh) dropped"] = (r64 + passes(conv, ah, torch.zeros_like(al), wh, wl, "fp32"), emu3)
+    mutants["xh * wl of one stacked k-step dropped"] = (r64 + split_passes(conv, ah, al, wh, dwl, "fp32"), emu3)
+    mutants["pass (xl, wh) dropped"] = (r64 + split_passes(conv, ah, torch.zeros_like(al), wh, wl, "fp32"), emu3)
     trunc = (a.view(torch.int32) & -65536).view(torch.float32).double()
     mutants["hi truncated (bf16)"] = (r64 + conv(trunc, wh), emu1)
     print("\nC %d, dilation %d, %s: float32 accumulation %.3f (fp32) / %.3f (bf16) of the bound" % (C, dd, kind, clean3, clean1))
@@ -460,16 +449,6 @@ def test_calibration(C, d, kind):
 # ------------------------------------------------------------------------------------------------------------------
 # GPU
 # ------------------------------------------------------------------------------------------------------------------
-def res_index(C, layer, co, ci, tap, h):
-    KC = tc_kc(C)
-    return res_base(layer) + 2 * ((tap * (C // KC) + ci // KC) * 2 * KC * C + in_chunk(C, co, ci % KC, h))
-
-
-def front_index(C, s, ci, co, k, h):
-    KC = tc_kc(C)
-    return lib_offset()(1, s, 0, 0, 0, 0) + 2 * ((k * (2 * C // KC) + ci // KC) * 2 * KC * C + in_chunk(C, co, ci % KC, h))
-
-
 def blob_halves(dev):
     blob = dev.packed.view(torch.int16)
     out = {}
@@ -480,7 +459,7 @@ def blob_halves(dev):
             for kind, l in (("c1", 5 + 6 * s + j), ("c2", 5 + 6 * s + 3 + j)):
                 out[(kind, s, j)] = tuple(bf16_of(blob, res_index(C, l, co, ci, tap, h)).double() for h in (0, 1))
     for s in (1, 2, 3):  # the tail ConvT streams ups.s's blob (the ConvT kernel's own layout)
-        out[("tail", s - 1, 0)] = tuple(bf16_of(blob, up_offset(1 + s, *weight_grid(1 + s), h)).double() for h in (0, 1))
+        out[("tail", s - 1, 0)] = tuple(bf16_of(blob, gen_weight_offset(1 + s, *weight_grid(1 + s), h)).double() for h in (0, 1))
     for s in (2, 3):
         C = 256 >> s
         ci, co, k = np.meshgrid(np.arange(2 * C), np.arange(C), np.arange(4), indexing="ij")

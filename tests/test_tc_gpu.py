@@ -8,36 +8,10 @@ import cases
 from conftest import rel_errors
 from melgan_multi_b200 import engine, synth
 from oracle import cport
+from kernel_model import gdev, gstate  # noqa: F401 (fixtures)
+from kernel_model import TOL, oracle_resblock
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-4
-
-
-@pytest.fixture(scope="module")
-def state():
-    return synth.generator_state(1234)
-
-
-@pytest.fixture(scope="module")
-def dev(state):
-    gd = engine.GeneratorDevice("cuda:0")
-    order = [n for n, *_ in synth.GENERATOR_LAYERS]
-    to = lambda a: torch.from_numpy(a).cuda()
-    gd.pack([to(state[n + ".weight_v"]) for n in order], [to(state[n + ".weight_g"]) for n in order],
-            [to(state[n + ".bias"]) for n in order])
-    return gd
-
-
-def oracle_resblock(state, stage, x):
-    """ResBlock.forward (models.py:32-40) with the oracle's primitives."""
-    lr = lambda a: np.where(a > 0, a, a * np.float32(0.01)).astype(np.float32)
-    for j, d in enumerate((1, 3, 9)):
-        n1, n2 = "resblocks.%d.convs1.%d" % (stage, j), "resblocks.%d.convs2.%d" % (stage, j)
-        w1 = cport.fold_weight_norm(state[n1 + ".weight_g"], state[n1 + ".weight_v"])
-        w2 = cport.fold_weight_norm(state[n2 + ".weight_g"], state[n2 + ".weight_v"])
-        h = cport.conv1d(lr(x), w1, state[n1 + ".bias"], 1, d, d, 1)
-        x = cport.conv1d(lr(h), w2, state[n2 + ".bias"], 1, 1, 1, 1) + x
-    return x
 
 
 @pytest.mark.parametrize("stage,B,L", [(3, 2, 2100), (2, 2, 1000), (1, 2, 500), (0, 2, 200), (3, 1, 5), (0, 1, 8),
@@ -48,28 +22,28 @@ def oracle_resblock(state, stage, x):
                                        # border lengths of every stage from the kernels' configuration
                                        (0, 1, 129), (0, 2, 144), (0, 3, 256), (0, 1, 257), (0, 2, 480), (0, 1, 481), (0, 2, 1000),
                                        (0, 1, 128), (0, 64, 256)])
-def test_resblock_tc_matches_oracle(state, dev, stage, B, L):
+def test_resblock_tc_matches_oracle(gstate, gdev, stage, B, L):
     C = 256 >> stage
     rs = np.random.RandomState(stage * 100 + L)
     x = rs.standard_normal((B, C, L)).astype(np.float32)
-    ref = oracle_resblock(state, stage, x)
-    y = dev.resblock(stage, torch.from_numpy(x).cuda()).cpu().numpy()
+    ref = oracle_resblock(gstate, stage, x)
+    y = gdev.resblock(stage, torch.from_numpy(x).cuda()).cpu().numpy()
     m, l2 = rel_errors(y, ref)
     assert m < TOL and l2 < TOL, (stage, B, L, m, l2)
 
 
 @pytest.mark.parametrize("stage,B,L", [(0, 2, 32), (0, 64, 32), (0, 1, 1), (0, 3, 130), (1, 2, 256), (1, 1, 5),
                                        (2, 2, 700), (2, 1, 1), (3, 2, 1500), (3, 1, 511), (3, 1, 512), (3, 1, 513)])
-def test_convt_tc_matches_oracle(state, dev, stage, B, L):
+def test_convt_tc_matches_oracle(gstate, gdev, stage, B, L):
     cin = 512 >> stage
     S, pad = (8, 4) if stage < 2 else (2, 1)
     rs = np.random.RandomState(stage * 1000 + L + B)
     x = rs.standard_normal((B, cin, L)).astype(np.float32)
     name = "ups.%d" % stage
-    w = cport.fold_weight_norm(state[name + ".weight_g"], state[name + ".weight_v"])
+    w = cport.fold_weight_norm(gstate[name + ".weight_g"], gstate[name + ".weight_v"])
     lr = np.where(x > 0, x, x * np.float32(0.01)).astype(np.float32)
-    ref = cport.conv_transpose1d(lr, w, state[name + ".bias"], S, pad)
-    y = dev.convt(stage, torch.from_numpy(x).cuda()).cpu().numpy()
+    ref = cport.conv_transpose1d(lr, w, gstate[name + ".bias"], S, pad)
+    y = gdev.convt(stage, torch.from_numpy(x).cuda()).cpu().numpy()
     assert y.shape == ref.shape
     m, l2 = rel_errors(y, ref)
     assert m < TOL and l2 < TOL, (stage, B, L, m, l2)
@@ -79,7 +53,7 @@ def test_convt_tc_matches_oracle(state, dev, stage, B, L):
                                        (1, 2, 300), (1, 1, 2), (1, 1, 222), (1, 1, 223), (1, 2, 2048),
                                        (0, 1, 3), (0, 2, 128), (0, 1, 129), (0, 3, 256), (0, 1, 223), (0, 2, 224), (0, 1, 600),
                                        (0, 64, 256)])
-def test_resblock_with_tail_convt_matches_oracle(state, dev, stage, B, L):
+def test_resblock_with_tail_convt_matches_oracle(gstate, gdev, stage, B, L):
     """ResBlock `stage` + the NEXT stage's LeakyReLU -> ConvTranspose1d fused at its tail (what the tail-fused pipelines run:
     res0+up1, res1+up2, res2+up3) against the oracle's ResBlock followed by its conv_transpose1d.  Lengths straddle the tile
     borders of the tail-fused tiling (one more halo row on the left, position L owned by the last tile)."""
@@ -87,12 +61,12 @@ def test_resblock_with_tail_convt_matches_oracle(state, dev, stage, B, L):
     S, pad = (8, 4) if stage == 0 else (2, 1)
     rs = np.random.RandomState(9000 + 100 * stage + L + B)
     x = rs.standard_normal((B, C, L)).astype(np.float32)
-    h = oracle_resblock(state, stage, x)
+    h = oracle_resblock(gstate, stage, x)
     name = "ups.%d" % (stage + 1)
-    w = cport.fold_weight_norm(state[name + ".weight_g"], state[name + ".weight_v"])
+    w = cport.fold_weight_norm(gstate[name + ".weight_g"], gstate[name + ".weight_v"])
     lr = np.where(h > 0, h, h * np.float32(0.01)).astype(np.float32)
-    ref = cport.conv_transpose1d(lr, w, state[name + ".bias"], S, pad)
-    y = dev.resup(stage, torch.from_numpy(x).cuda()).cpu().numpy()
+    ref = cport.conv_transpose1d(lr, w, gstate[name + ".bias"], S, pad)
+    y = gdev.resup(stage, torch.from_numpy(x).cuda()).cpu().numpy()
     assert y.shape == ref.shape
     m, l2 = rel_errors(y, ref)
     assert m < TOL and l2 < TOL, (stage, B, L, m, l2)
@@ -100,7 +74,7 @@ def test_resblock_with_tail_convt_matches_oracle(state, dev, stage, B, L):
 
 @pytest.mark.parametrize("stage,B,Lin", [(2, 2, 500), (2, 1, 1), (2, 1, 64), (2, 3, 129), (2, 1, 2048), (3, 2, 1050), (3, 1, 1),
                                          (3, 1, 128), (3, 1, 255), (3, 2, 256), (3, 1, 4096)])
-def test_fused_convt_resblock_matches_oracle(state, dev, stage, B, Lin):
+def test_fused_convt_resblock_matches_oracle(gstate, gdev, stage, B, Lin):
     """Stage 2 / 3 as ONE kernel (LeakyReLU -> ConvT k4 s2 -> ResBlock; what the default pipeline runs for stage 3) against the oracle's
     conv_transpose1d + ResBlock; odd and tiny lengths cover the pair de-interleave at both sequence ends, long ones the
     tile borders."""
@@ -108,20 +82,20 @@ def test_fused_convt_resblock_matches_oracle(state, dev, stage, B, Lin):
     rs = np.random.RandomState(stage * 777 + Lin + B)
     x = rs.standard_normal((B, cin, Lin)).astype(np.float32)
     name = "ups.%d" % stage
-    w = cport.fold_weight_norm(state[name + ".weight_g"], state[name + ".weight_v"])
+    w = cport.fold_weight_norm(gstate[name + ".weight_g"], gstate[name + ".weight_v"])
     lr = np.where(x > 0, x, x * np.float32(0.01)).astype(np.float32)
-    ref = oracle_resblock(state, stage, cport.conv_transpose1d(lr, w, state[name + ".bias"], 2, 1))
-    y = dev.upres(stage, torch.from_numpy(x).cuda()).cpu().numpy()
+    ref = oracle_resblock(gstate, stage, cport.conv_transpose1d(lr, w, gstate[name + ".bias"], 2, 1))
+    y = gdev.upres(stage, torch.from_numpy(x).cuda()).cpu().numpy()
     assert y.shape == ref.shape
     m, l2 = rel_errors(y, ref)
     assert m < TOL and l2 < TOL, (stage, B, Lin, m, l2)
 
 
 @pytest.mark.parametrize("case", cases.GEN_CASES)
-def test_tc_pipeline_matches_golden(golden, state, case):
+def test_tc_pipeline_matches_golden(golden, gstate, case):
     B, T, seed, realistic = case
     eng = engine.GeneratorHost(B, T)
-    eng.load_state(state)
+    eng.load_state(gstate)
     y = eng.forward(synth.mel_input(B, T, seed, realistic))
     eng.close()
     m, l2 = rel_errors(y, golden[cases.gen_key(*case)])
@@ -129,28 +103,28 @@ def test_tc_pipeline_matches_golden(golden, state, case):
 
 
 @pytest.mark.parametrize("B,T", [(1, 1), (2, 32), (64, 32), (3, 130), (1, 1000)])
-def test_conv_pre_kernel_matches_oracle(state, dev, B, T):
+def test_conv_pre_kernel_matches_oracle(gstate, gdev, B, T):
     """conv_pre alone (conv_rows_tc_kernel<80,512,k7>; models.py:46,62) against the oracle's conv1d."""
     x = synth.mel_input(B, T, 50 + T)
-    w = cport.fold_weight_norm(state["conv_pre.weight_g"], state["conv_pre.weight_v"])
-    ref = cport.conv1d(x, w, state["conv_pre.bias"], 1, 3, 1, 1)
-    y = dev.conv_pre(torch.from_numpy(x).cuda()).cpu().numpy()
+    w = cport.fold_weight_norm(gstate["conv_pre.weight_g"], gstate["conv_pre.weight_v"])
+    ref = cport.conv1d(x, w, gstate["conv_pre.bias"], 1, 3, 1, 1)
+    y = gdev.conv_pre(torch.from_numpy(x).cuda()).cpu().numpy()
     assert y.shape == ref.shape
     m, l2 = rel_errors(y, ref)
     assert m < TOL and l2 < TOL, (B, T, m, l2)
 
 
 @pytest.mark.parametrize("B,L", [(2, 2100), (1, 5), (1, 1), (3, 487), (1, 488), (2, 8192)])
-def test_resblock_post_tanh_matches_oracle(state, dev, B, L):
+def test_resblock_post_tanh_matches_oracle(gstate, gdev, B, L):
     """The last stage's kernel on its own: ResBlock(32) -> LeakyReLU -> conv_post(32->1, k7) -> tanh fused in one epilogue
     (models.py:66-69) against the oracle's ResBlock + conv1d + tanh; lengths straddle the 512-position tiles (valid part 474)."""
     rs = np.random.RandomState(4000 + L)
     x = rs.standard_normal((B, 32, L)).astype(np.float32)
-    h = oracle_resblock(state, 3, x)
+    h = oracle_resblock(gstate, 3, x)
     lr = np.where(h > 0, h, h * np.float32(0.01)).astype(np.float32)
-    w = cport.fold_weight_norm(state["conv_post.weight_g"], state["conv_post.weight_v"])
-    ref = np.tanh(cport.conv1d(lr, w, state["conv_post.bias"], 1, 3, 1, 1).astype(np.float64))
-    y = dev.resblock_post(torch.from_numpy(x).cuda()).cpu().numpy()
+    w = cport.fold_weight_norm(gstate["conv_post.weight_g"], gstate["conv_post.weight_v"])
+    ref = np.tanh(cport.conv1d(lr, w, gstate["conv_post.bias"], 1, 3, 1, 1).astype(np.float64))
+    y = gdev.resblock_post(torch.from_numpy(x).cuda()).cpu().numpy()
     assert y.shape == ref.shape == (B, 1, L)
     m, l2 = rel_errors(y, ref)
     assert m < TOL and l2 < TOL, (B, L, m, l2)

@@ -14,7 +14,7 @@ import torch
 
 from conftest import rel_errors
 from melgan_multi_b200 import synth
-from test_host import _train_case, check_grad_digest
+from kernel_model import check_grad_digest, train_case
 
 pytestmark = pytest.mark.gpu
 
@@ -36,7 +36,7 @@ def test_train_step_losses_and_gradients_match_reference(strict_fp32, which):
     (B=2, 1024 samples) and BASELINE config 3 at full size (B=16 x 8192 samples; golden written by make_golden.py
     --train-step-b16)."""
     from melgan_multi_b200 import models
-    fname, c = (("train_step_grads.npz", _train_case()) if which == "small" else ("train_step_grads_b16.npz", TRAIN_CASE_B16))
+    fname, c = (("train_step_grads.npz", train_case()) if which == "small" else ("train_step_grads_b16.npz", TRAIN_CASE_B16))
     gg = np.load(os.path.join(os.path.dirname(__file__), "golden", fname))
     gen = models.Generator()
     gen.load_state_dict({k: torch.from_numpy(v) for k, v in synth.generator_state(1234).items()})
