@@ -3,9 +3,21 @@
 PyTorch is plumbing here: it owns device memory and streams; every kernel that runs on the hot
 path lives in the shared library.  There is no CPU or eager-PyTorch fallback: if the library
 is missing, or the device is not sm_90 (H100), calls raise.
+
+Streams and threads: every call enqueues its work on the caller's current CUDA stream.  Inference calls of one
+GeneratorDevice or DiscriminatorDevice (and so of one Generator, Discriminator or MultiScaleDiscriminator) may run
+concurrently on distinct streams, from one host thread or several: the scratch memory a call writes (the generator's
+workspace, the discriminator's status word and backward workspace, the status copy to the host) is kept per stream, is
+allocated while that stream is current, and so is only ever used and freed in that stream's order (_PerStream).  Calls
+on one stream are ordered by the stream.  Every read of the packed weights waits for the last pack, whichever stream
+enqueued it (_PackedBlob).  Training steps that update the parameters need the caller's ordering, as in stock PyTorch.
+A GeneratorStream handle is the exception: its steps must stay on one stream (GeneratorStream).
 """
+import collections
 import ctypes
 import os
+import threading
+import weakref
 
 import numpy as np
 
@@ -227,17 +239,16 @@ class _StatusWatch:
     word is copied to pinned host memory on the same stream (4 bytes, asynchronous), and the copy is inspected at the
     next forward of the same module, or at the next host synchronisation point the training loop has anyway
     (``discriminator_loss``' read-back, ``poll_status``).  A non-zero word raises EngineError.  Skipped while the stream
-    is being captured into a CUDA graph (no host-visible copy can be made there; replays are checked by check_status)."""
-    _live = None  # weak set of watches with a copy in flight
+    is being captured into a CUDA graph (no host-visible copy can be made there; replays are checked by check_status).
+    One watch serves one stream at a time (_PerStream): a second call in flight on another stream has its own slot and
+    event."""
+    _live = weakref.WeakSet()  # watches with a copy in flight
 
     def __init__(self, torch, device, what):
-        import weakref
         self.torch, self.what = torch, what
         self.pin = torch.zeros(1, dtype=torch.int32).pin_memory()
         self.event = torch.cuda.Event()
         self.pending = False
-        if _StatusWatch._live is None:
-            _StatusWatch._live = weakref.WeakSet()
 
     def arm(self, status_word):
         """status_word: int32 CUDA tensor view [1] holding the pipeline's status after the work just enqueued."""
@@ -265,16 +276,140 @@ class _StatusWatch:
 
 
 def poll_status(wait=False):
-    """Checks every status copy in flight (all modules, this process); ``wait=True`` blocks on the copies' events."""
-    for w in list(_StatusWatch._live or ()):
+    """Checks every status copy in flight (all modules and streams, this process); ``wait=True`` blocks on the copies'
+    events."""
+    for w in list(_StatusWatch._live):
         w.check(wait)
+
+
+class _StreamScratch:
+    """The scratch buffers and the status watch one module uses on one CUDA stream."""
+
+    def __init__(self, owner):
+        self.owner = owner
+        self.bufs = {}
+        self._watch = None
+
+    def buffer(self, name, nbytes, zeros=False):
+        """The stream's buffer `name` of at least nbytes (grown on demand; an int32 tensor when zeros, else fp32).  Called
+        with the stream current, so the caching allocator ties the memory to it: a buffer dropped by regrowth or
+        eviction is handed out again only in this stream's order."""
+        torch, device = self.owner.torch, self.owner.device
+        t = self.bufs.get(name)
+        if t is None or t.numel() * 4 < nbytes:
+            n = (nbytes + 3) // 4
+            t = self.bufs[name] = (torch.zeros(n, dtype=torch.int32, device=device) if zeros else
+                                   torch.empty(n, dtype=torch.float32, device=device))
+        if torch.cuda.is_current_stream_capturing():
+            self.owner.hold(t)
+        return t
+
+    @property
+    def watch(self):
+        if self._watch is None:
+            self._watch = self.owner.take_watch()
+        return self._watch
+
+    def check(self):
+        """Raises for a timed-out wait of an earlier call of this module whose status copy has landed: this stream's
+        previous call, or a call on a stream whose scratch has since been dropped (_PerStream.check_retired)."""
+        self.owner.check_retired()
+        if self._watch is not None:
+            self._watch.check()
+
+    def arm(self, status_word):
+        if not self.owner.torch.cuda.is_current_stream_capturing():  # (no pinned allocation while capturing)
+            self.watch.arm(status_word)
+
+
+class _PerStream:
+    """One _StreamScratch per CUDA stream of a module, keyed by the current stream's handle, so that calls on distinct
+    streams or threads never share a byte of scratch memory.
+
+    At most LIMIT streams keep their scratch, as many as PyTorch's pool hands out per priority (torch.cuda.Stream()):
+    the least recently used one beyond them is dropped.  Its buffers return to the caching allocator's pool of their own
+    stream, which keeps them reserved for that stream, so reserved memory follows the number of distinct streams that
+    ever called, not LIMIT.  Its status watch is retired: the module's next call checks it without blocking (raising
+    for a timed-out wait whose copy has landed), and once its copy has landed it is reused by a new stream's scratch,
+    so pinned slots and events are bounded by LIMIT plus the copies still in flight.  Buffers a captured CUDA graph
+    writes stay allocated for the module's lifetime."""
+    LIMIT = 32
+
+    def __init__(self, torch, device, what):
+        self.torch, self.device, self.what = torch, device, what
+        self._by_stream = collections.OrderedDict()
+        self._held = []     # buffers captured CUDA graphs write
+        self._retired = []  # watches of dropped scratch: copies in flight first, then idle ones for reuse
+        self._lock = threading.Lock()  # streams of several host threads share the tables
+
+    def current(self):
+        key = self.torch.cuda.current_stream(self.device).cuda_stream
+        with self._lock:
+            s = self._by_stream.get(key)
+            if s is None:
+                s = self._by_stream[key] = _StreamScratch(self)
+                while len(self._by_stream) > self.LIMIT:
+                    _, old = self._by_stream.popitem(last=False)
+                    if old._watch is not None:
+                        self._retired.append(old._watch)
+            else:
+                self._by_stream.move_to_end(key)
+        return s
+
+    def hold(self, t):
+        with self._lock:
+            if not any(h is t for h in self._held):
+                self._held.append(t)
+
+    def take_watch(self):
+        """An idle retired watch (no copy in flight), or a new one."""
+        with self._lock:
+            for i, w in enumerate(self._retired):
+                if not w.pending:
+                    return self._retired.pop(i)
+        return _StatusWatch(self.torch, self.device, self.what)
+
+    def check_retired(self):
+        with self._lock:
+            try:
+                for w in self._retired:
+                    w.check()  # (non-blocking; marks a landed copy checked before it raises)
+            finally:
+                idle = [w for w in self._retired if not w.pending]
+                self._retired = [w for w in self._retired if w.pending] + idle[:self.LIMIT]
+
+
+class _PackedBlob:
+    """The packed weight blob of a GeneratorDevice / DiscriminatorDevice.  ``pack`` enqueues its writes on the caller's
+    stream and records an event after them; until that event has completed, every read of ``packed`` makes the current
+    stream wait for it, so a call on any stream reads the weights of the last pack, even when the pack is still queued
+    behind other work on its own stream.  (A re-pack while calls on other streams still read the old weights needs the
+    caller's ordering, as any parameter update does.)"""
+
+    @property
+    def packed(self):
+        ev = self._pack_done
+        if ev is not None and not self.torch.cuda.is_current_stream_capturing():  # (no event query while capturing)
+            if ev.query():
+                self._pack_done = None
+            else:
+                self.torch.cuda.current_stream(self.device).wait_event(ev)
+        return self._packed
+
+    def _pack_enqueued(self):
+        if not self.torch.cuda.is_current_stream_capturing():
+            ev = self.torch.cuda.Event()
+            ev.record(self.torch.cuda.current_stream(self.device))
+            self._pack_done = ev
 
 
 # ------------------------------------------------------------------------------------------
 # Device-pointer path (what models.Generator.forward uses with torch tensors)
 # ------------------------------------------------------------------------------------------
-class GeneratorDevice:
-    """Packed weights + workspace cache on one CUDA device, driven with torch tensors."""
+class GeneratorDevice(_PackedBlob):
+    """Packed weights + workspace cache on one CUDA device, driven with torch tensors.  Each CUDA stream gets its own
+    workspace and status watch (_PerStream), so forwards on distinct streams or threads may run concurrently; the
+    methods that read a workspace back (check_status, stage_output) read the current stream's."""
 
     def __init__(self, device):
         import torch
@@ -284,10 +419,18 @@ class GeneratorDevice:
             raise EngineError("the native engine runs on CUDA devices only (got %s)" % (device,))
         with torch.cuda.device(self.device):
             check(lib().mg_device_check())
-        self.packed = torch.empty((lib().mg_gen_packed_bytes() + 3) // 4, dtype=torch.float32, device=self.device)
-        self._ws = None
-        self._ws_key = None
-        self._watch = _StatusWatch(torch, self.device, "Generator.forward")
+        self._packed = torch.empty((lib().mg_gen_packed_bytes() + 3) // 4, dtype=torch.float32, device=self.device)
+        self._pack_done = None
+        self._scratch = _PerStream(torch, self.device, "Generator.forward")
+
+    @property
+    def _ws(self):
+        """The current stream's workspace (None before its first forward)."""
+        return self._scratch.current().bufs.get("ws")
+
+    @property
+    def _watch(self):
+        return self._scratch.current().watch
 
     def pack(self, vs, gs, bs):
         """vs/gs/bs: 30 contiguous fp32 CUDA tensors each (weight_v, weight_g, bias; reference order)."""
@@ -307,14 +450,13 @@ class GeneratorDevice:
             raise EngineError("expected %d layers" % NUM_LAYERS)
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            check(lib().mg_gen_pack(ptrs(vs), ptrs(gs), ptrs(bs), self.packed.data_ptr(), stream))
+            check(lib().mg_gen_pack(ptrs(vs), ptrs(gs), ptrs(bs), self._packed.data_ptr(), stream))
+            self._pack_enqueued()
         del keep
 
     def workspace(self, B, T):
-        need = lib().mg_gen_workspace_bytes(B, T)
-        if self._ws is None or self._ws.numel() * 4 < need:
-            self._ws = self.torch.empty((need + 3) // 4, dtype=self.torch.float32, device=self.device)
-        return self._ws
+        """The current stream's workspace, grown to mg_gen_workspace_bytes(B, T)."""
+        return self._scratch.current().buffer("ws", lib().mg_gen_workspace_bytes(B, T))
 
     def forward(self, mel, out=None, precision="fp32"):
         """mel [B, 80, T] -> audio [B, 1, 256 T].  precision "fp32" (the default) or "bf16" (one bf16 pass per tensor-core
@@ -329,8 +471,9 @@ class GeneratorDevice:
         B, _, T = mel.shape
         if out is None:
             out = torch.empty((B, 1, 256 * T), dtype=torch.float32, device=self.device)
-        self._watch.check()  # the previous forward's status word, if its copy has landed
-        ws = self.workspace(B, T)
+        sc = self._scratch.current()
+        sc.check()  # the previous forward's status word on this stream, if its copy has landed
+        ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
             if code == 0:
@@ -340,7 +483,7 @@ class GeneratorDevice:
                 check(lib().mg_gen_forward_precision(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, None, code,
                                                      ws.data_ptr(), ws.numel() * 4, stream))
             off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4  # the status word sits after the activation buffers
-            self._watch.arm(ws.view(torch.int32)[off:off + 1])
+            sc.arm(ws.view(torch.int32)[off:off + 1])
         return out
 
     def forward_ragged(self, mel, lengths, out=None, precision="fp32"):
@@ -358,8 +501,9 @@ class GeneratorDevice:
         lens = _lengths(lengths, B, T)
         if out is None:
             out = torch.empty((B, 1, 256 * T), dtype=torch.float32, device=self.device)
-        self._watch.check()
-        ws = self.workspace(B, T)
+        sc = self._scratch.current()
+        sc.check()
+        ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
             if code == 0:
@@ -369,7 +513,7 @@ class GeneratorDevice:
                 check(lib().mg_gen_forward_precision(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens, code,
                                                      ws.data_ptr(), ws.numel() * 4, stream))
             off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4
-            self._watch.arm(ws.view(torch.int32)[off:off + 1])
+            sc.arm(ws.view(torch.int32)[off:off + 1])
         return out
 
     def forward_timed(self, mel, out):
@@ -386,12 +530,19 @@ class GeneratorDevice:
                                              ws.data_ptr(), ws.numel() * 4, stream, ms))
         return [(lib().mg_gen_kernel_name(i).decode(), ms[i]) for i in range(n)]
 
+    def _last_ws(self):
+        ws = self._ws
+        if ws is None:
+            raise EngineError("no forward has run on the current stream of %s" % (self.device,))
+        return ws
+
     def check_status(self, B, T):
-        """Synchronises and raises if the tensor-core pipeline of the last forward timed out."""
+        """Synchronises the current stream and raises if the tensor-core pipeline of the last [B, 80, T] forward on it
+        timed out (for a replayed CUDA graph: call it on the stream the graph was captured on)."""
         torch = self.torch
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            check(lib().mg_gen_check_status(self._ws.data_ptr(), B, T, stream))
+            check(lib().mg_gen_check_status(self._last_ws().data_ptr(), B, T, stream))
 
     def convt(self, stage, x):
         """LeakyReLU -> ConvTranspose1d of stage 0..3 on the tensor cores; x [B, 512>>stage, Lin]; synchronous."""
@@ -517,13 +668,13 @@ class GeneratorDevice:
         return y
 
     def stage_output(self, which, B, T):
-        """Activation after conv_pre (0) or stage 0..2 (1..3) of the last forward, NCL."""
+        """Activation after conv_pre (0) or stage 0..2 (1..3) of the last forward on the current stream, NCL."""
         torch = self.torch
         shapes = [(B, 512, T), (B, 256, 8 * T), (B, 128, 64 * T), (B, 64, 128 * T)]
         out = torch.empty(shapes[which], dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            check(lib().mg_gen_stage_output(self._ws.data_ptr(), which, out.data_ptr(), B, T, stream))
+            check(lib().mg_gen_stage_output(self._last_ws().data_ptr(), which, out.data_ptr(), B, T, stream))
         return out
 
 
@@ -538,7 +689,12 @@ class GeneratorStream:
 
     packed_fn: a callable returning the GeneratorDevice whose packed weights a step reads (Generator._ensure_packed, so
     weights changed between steps are re-packed).  state: optional caller-provided uint8 CUDA tensor of at least
-    mg_gen_stream_state_bytes bytes (the stream never lets a byte it has not written reach an output)."""
+    mg_gen_stream_state_bytes bytes (the stream never lets a byte it has not written reach an output).
+
+    One thread drives a handle at a time, and all steps of one handle must be enqueued on one CUDA stream (or otherwise
+    ordered), as for mg_gen_stream_step: the state and the mel staging buffer that ``step`` copies each chunk into are
+    the handle's own, and the next step overwrites them in stream order.  Distinct handles of one generator may step
+    concurrently on distinct streams or threads."""
 
     def __init__(self, packed_fn, device, max_sessions=1, max_push_frames=32, precision="fp32", state=None):
         import torch
@@ -691,9 +847,10 @@ def loss_backward(a, b, modes, grad_out, need_b, out_a=None, out_b=None):
     return ga, gb
 
 
-class DiscriminatorDevice:
+class DiscriminatorDevice(_PackedBlob):
     """Packed discriminator weights on one CUDA device, driven with torch tensors: the three-scale stack of
-    MultiScaleDiscriminator (ndisc = 3) or one stand-alone Discriminator (ndisc = 1)."""
+    MultiScaleDiscriminator (ndisc = 3) or one stand-alone Discriminator (ndisc = 1).  The status word and the backward
+    workspace are kept per CUDA stream (_PerStream), so calls on distinct streams or threads may run concurrently."""
 
     def __init__(self, device, ndisc=3):
         import torch
@@ -707,9 +864,19 @@ class DiscriminatorDevice:
         with torch.cuda.device(self.device):
             check(lib().mg_device_check())
         nbytes = lib().mg_msd_packed_bytes() if ndisc == 3 else lib().mg_disc_packed_bytes()
-        self.packed = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=self.device)
-        self.status = torch.zeros(64, dtype=torch.int32, device=self.device)
-        self._watch = _StatusWatch(torch, self.device, "Discriminator forward")
+        self._packed = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=self.device)
+        self._pack_done = None
+        self._scratch = _PerStream(torch, self.device, "Discriminator forward")
+
+    @property
+    def status(self):
+        """The current stream's status word (int32 [64], zeroed when first made): every call on the stream reports a
+        timed-out tensor-core pipeline wait in it."""
+        return self._scratch.current().buffer("status", 64 * 4, zeros=True)
+
+    @property
+    def _watch(self):
+        return self._scratch.current().watch
 
     def pack(self, vs, gs, bs):
         """vs/gs/bs: 7 * ndisc fp32 CUDA tensors each (discriminator-major, layers in registration order)."""
@@ -731,7 +898,8 @@ class DiscriminatorDevice:
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
             fn = lib().mg_msd_pack if self.ndisc == 3 else lib().mg_disc_pack
-            check(fn(ptrs(vs), ptrs(gs), ptrs(bs), self.packed.data_ptr(), stream))
+            check(fn(ptrs(vs), ptrs(gs), ptrs(bs), self._packed.data_ptr(), stream))
+            self._pack_enqueued()
 
     def forward(self, y):
         """y [Bt, 1, L] -> list of ndisc lists of 7 feature maps [Bt, C, len] (fresh tensors)."""
@@ -743,15 +911,17 @@ class DiscriminatorDevice:
         y = y.contiguous()
         Bt, _, L = y.shape
         lens = msd_lengths(L)
-        self._watch.check()
+        scratch = self._scratch.current()
+        scratch.check()
+        status = scratch.buffer("status", 64 * 4, zeros=True)
         fmaps = [[torch.empty((Bt, D_CHANNELS[l], lens[s][l]), dtype=torch.float32, device=self.device)
                   for l in range(7)] for s in range(self.ndisc)]
         ptrs = _ptr_array([f.data_ptr() for sc in fmaps for f in sc])
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
             fn = lib().mg_msd_forward if self.ndisc == 3 else lib().mg_disc_forward
-            check(fn(self.packed.data_ptr(), y.data_ptr(), Bt, L, ptrs, self.status.data_ptr(), stream))
-            self._watch.arm(self.status[:1])
+            check(fn(self.packed.data_ptr(), y.data_ptr(), Bt, L, ptrs, status.data_ptr(), stream))
+            scratch.arm(status[:1])
         return fmaps
 
     def layer_forward(self, scale, layer, x, out=None):
@@ -781,8 +951,8 @@ class DiscriminatorDevice:
         """The whole backward of discriminator `scale` in one host call (mg_msd_scale_backward): x0 [Bt, 1, L0] its input,
         fmaps the 7 maps its forward returned, grads the gradient w.r.t. each (None: none).  Returns (gx0 | None, dws[7],
         dbs[7]) -- gradients of the FOLDED weights in torch layout; entries of layers the gradient does not reach are None.
-        The intermediate gradients live in a workspace that is reused by every call on this device (the calls are ordered
-        by the stream they are enqueued on)."""
+        The intermediate gradients live in the current stream's workspace, reused by every call on that stream (in the
+        stream's order)."""
         torch = self.torch
         from .synth import DISCRIMINATOR_LAYERS
         x0 = x0.contiguous()
@@ -794,9 +964,8 @@ class DiscriminatorDevice:
         dbs = [torch.empty((cout,), dtype=torch.float32, device=self.device) for _n, _cin, cout, *_ in DISCRIMINATOR_LAYERS]
         gx0 = torch.empty_like(x0) if need_gx0 else None
         nbytes = lib().mg_msd_scale_backward_workspace_bytes(Bt, L0)
-        ws = self.__dict__.get("_bwd_ws")
-        if ws is None or ws.numel() * 4 < nbytes:
-            ws = self._bwd_ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=self.device)
+        sc = self._scratch.current()
+        ws, status = sc.buffer("bwd", nbytes), sc.buffer("status", 64 * 4, zeros=True)
         reached = (ctypes.c_int * 7)()
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
@@ -804,7 +973,7 @@ class DiscriminatorDevice:
                 self.packed.data_ptr(), scale, x0.data_ptr(), _ptr_array([f.data_ptr() for f in keep]),
                 _ptr_array([g.data_ptr() if g is not None else None for g in gs]), gx0.data_ptr() if need_gx0 else None,
                 _ptr_array([t.data_ptr() for t in dws]), _ptr_array([t.data_ptr() for t in dbs]), reached, ws.data_ptr(),
-                ws.numel() * 4, Bt, L0, self.status.data_ptr(), stream))
+                ws.numel() * 4, Bt, L0, status.data_ptr(), stream))
         hit = [bool(r) for r in reached]
         return (gx0 if hit[0] else None), [w if h else None for w, h in zip(dws, hit)], [b if h else None for b, h in zip(dbs, hit)]
 

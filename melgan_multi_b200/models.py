@@ -22,6 +22,8 @@ What runs where
     feature maps layer by layer on hand-written kernels only (grouped convs, conv_post1 dgrad / wgrad on wgmma,
     conv_pre / conv_post2, LeakyReLU, weight-norm): no cuDNN call in a discriminator's backward.
 """
+import threading
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -30,6 +32,10 @@ from torch.nn.utils import weight_norm
 
 from . import engine as _engine
 from .synth import DISCRIMINATOR_LAYERS, GENERATOR_LAYERS
+
+# Makes a module's lazy (re-)pack one step when host threads call it at once: the first caller packs (engine
+# _PackedBlob orders every later read of the blob after that pack), the others see the weights already packed.
+_PACK_LOCK = threading.Lock()
 
 _RES_DILATIONS = (1, 3, 9)
 
@@ -128,14 +134,15 @@ class Generator(nn.Module):
             raise _engine.EngineError(
                 "melgan_multi_b200.Generator runs on CUDA (sm_90a) only; move the module with .to('cuda'). "
                 "There is deliberately no CPU fallback.")
-        if self._dev is None or self._dev.device != dev:
-            self._dev = _engine.GeneratorDevice(dev)
-            self._packed_key = None
-        key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
-        if key != self._packed_key:
-            self._dev.pack(vs, gs, bs)
-            self._packed_key = key
-        return self._dev
+        with _PACK_LOCK:
+            if self._dev is None or self._dev.device != dev:
+                self._dev = _engine.GeneratorDevice(dev)
+                self._packed_key = None
+            key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
+            if key != self._packed_key:
+                self._dev.pack(vs, gs, bs)
+                self._packed_key = key
+            return self._dev
 
     def _engine_forward(self, mel):
         return self._ensure_packed().forward(mel)
@@ -249,13 +256,14 @@ class Discriminator(nn.Module):
     def _engine_forward(self, x):
         vs, gs, bs = self._param_triplets()
         dev = vs[0].device
-        if getattr(self, "_dev", None) is None or self._dev.device != dev:
-            self._dev = _engine.DiscriminatorDevice(dev, ndisc=1)
-            self._packed_key = None
-        key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
-        if key != self._packed_key:
-            self._dev.pack(vs, gs, bs)
-            self._packed_key = key
+        with _PACK_LOCK:
+            if getattr(self, "_dev", None) is None or self._dev.device != dev:
+                self._dev = _engine.DiscriminatorDevice(dev, ndisc=1)
+                self._packed_key = None
+            key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
+            if key != self._packed_key:
+                self._dev.pack(vs, gs, bs)
+                self._packed_key = key
         return self._dev.forward(x)
 
     def forward(self, x):
@@ -344,13 +352,14 @@ class MultiScaleDiscriminator(nn.Module):
     def _engine_forward(self, y2):
         vs, gs, bs = self._param_triplets()
         dev = vs[0].device
-        if self._dev is None or self._dev.device != dev:
-            self._dev = _engine.DiscriminatorDevice(dev)
-            self._packed_key = None
-        key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
-        if key != self._packed_key:
-            self._dev.pack(vs, gs, bs)
-            self._packed_key = key
+        with _PACK_LOCK:
+            if self._dev is None or self._dev.device != dev:
+                self._dev = _engine.DiscriminatorDevice(dev)
+                self._packed_key = None
+            key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
+            if key != self._packed_key:
+                self._dev.pack(vs, gs, bs)
+                self._packed_key = key
         return self._dev.forward(y2)
 
     # -- stock-PyTorch restatement on folded weights, used ONLY to differentiate (backward) -----------------

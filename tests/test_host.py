@@ -328,3 +328,103 @@ def test_no_test_module_imports_another():
                 continue
             bad += ["%s:%d imports %s" % (os.path.basename(path), node.lineno, n) for n in names if n.startswith("test_")]
     assert not bad, bad
+
+
+class _Pinned(torch.Tensor):
+    def pin_memory(self):
+        return self
+
+
+def stand_in_cuda():
+    """(cuda, torch) stand-ins for what engine._PerStream and engine._StatusWatch call: the current stream's handle is
+    cuda.stream; an event has completed when its `done` is set (cuda.done_default for new ones)."""
+    import types
+
+    class Event:
+        def __init__(self):
+            self.done = cuda.done_default
+
+        def record(self, stream=None):
+            self.done = cuda.done_default
+
+        def query(self):
+            return self.done
+
+        def synchronize(self):
+            assert self.done
+
+    class Cuda:
+        stream, capturing, done_default, Event = 0, False, True, None
+
+        def current_stream(self, device=None):
+            return types.SimpleNamespace(cuda_stream=self.stream)
+
+        def is_current_stream_capturing(self):
+            return self.capturing
+
+    cuda = Cuda()
+    cuda.Event = Event
+    fake = types.SimpleNamespace(cuda=cuda, int32=torch.int32, float32=torch.float32,
+                                 zeros=lambda n, dtype, device=None: torch.zeros(n, dtype=dtype).as_subclass(_Pinned),
+                                 empty=lambda n, dtype, device=None: torch.empty(n, dtype=dtype))
+    return cuda, fake
+
+
+def test_per_stream_scratch_is_private_bounded_and_keeps_graph_buffers():
+    """engine._PerStream on a stand-in for torch.cuda: each stream has its own scratch, a stream's buffer grows in place
+    of the old one, the least recently used stream beyond LIMIT is dropped, and a buffer used while a CUDA graph was being
+    captured stays allocated after its stream is dropped."""
+    cuda, fake = stand_in_cuda()
+    per = engine._PerStream(fake, "cuda:0", "test")
+    bufs = {}
+    for s in range(1, per.LIMIT + 1):
+        cuda.stream = s
+        cuda.capturing = s == 2
+        bufs[s] = per.current().buffer("ws", 64)
+    cuda.capturing = False
+    assert len({id(b) for b in bufs.values()}) == per.LIMIT
+    cuda.stream = 1
+    assert per.current().buffer("ws", 64) is bufs[1] and per.current().buffer("ws", 16) is bufs[1]
+    grown = per.current().buffer("ws", 65)
+    assert grown is not bufs[1] and grown.numel() * 4 >= 65 and per.current().bufs["ws"] is grown
+    cuda.stream = per.LIMIT + 1  # stream 2 is now the least recently used: dropped, its captured buffer held
+    per.current().buffer("ws", 64)
+    assert 2 not in per._by_stream and 1 in per._by_stream and len(per._by_stream) == per.LIMIT
+    assert len(per._held) == 1 and per._held[0] is bufs[2]
+    status = per.current().buffer("status", 256, zeros=True)
+    assert status.dtype == torch.int32 and status.numel() == 64 and not status.any()
+
+
+def test_status_watches_of_dropped_streams_are_bounded_and_reported():
+    """A server that takes a new stream per request rotates through more streams than _PerStream.LIMIT.  The watches of
+    dropped streams must be checked at the module's next call and reused once their copy has landed: the pinned slots
+    and events stay bounded, and a timed-out wait of a call whose stream was dropped raises at the next call."""
+    cuda, fake = stand_in_cuda()
+    per = engine._PerStream(fake, "cuda:0", "test")
+
+    def call(stream, code=0):  # one forward's status handling, as GeneratorDevice.forward does it
+        cuda.stream = stream
+        sc = per.current()
+        sc.check()
+        word = sc.buffer("status", 4, zeros=True)
+        word.fill_(code)
+        sc.arm(word[:1])
+        return sc.watch
+
+    n_streams = per.LIMIT + 9
+    watches = {id(call(1 + k % n_streams)) for k in range(10 * n_streams)}
+    assert len(per._by_stream) == per.LIMIT
+    assert len(watches) <= per.LIMIT + 1, len(watches)
+    assert len(per._retired) <= per.LIMIT + 1
+    # a timed-out wait on stream 1000 whose copy is still in flight when 1000 is dropped
+    cuda.done_default = False
+    slow = call(1000, code=7)
+    cuda.done_default = True
+    for k in range(per.LIMIT):
+        call(2000 + k)
+    assert 1000 not in per._by_stream and any(w is slow for w in per._retired)
+    slow.event.done = True  # the copy lands
+    with pytest.raises(engine.EngineError, match="role code 7"):
+        call(3000)
+    call(3001)  # reported once
+    assert not slow.pending and len(per._retired) <= per.LIMIT + 1
