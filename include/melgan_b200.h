@@ -113,6 +113,25 @@ int mg_gen_forward_ragged(const void *packed, const float *mel, float *audio, in
 int mg_gen_forward_precision(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
                              int precision, void *workspace, size_t workspace_bytes, void *stream);
 
+/* Many voices in one forward: generators of the same architecture with different weights (a vocoder fine-tuned per
+ * speaker), each item on its own voice's weights, in one launch of the default chain's eight kernels (inference only).
+ *   packed: HOST array of n_voices >= 1 device pointers, each a blob of mg_gen_pack (16-byte aligned, none NULL)
+ *   voice:  HOST array of B ints in [0, n_voices): item i runs on packed[voice[i]]
+ *   mel, audio, T_max, lengths (NULL: every item T_max frames), precision (MG_GEN_PRECISION_*), workspace
+ *   (mg_gen_workspace_bytes(B, T_max)), stream: as for mg_gen_forward_precision.
+ * audio[i, 0, :256 L_i] is bit-identical to mg_gen_forward_precision of item i alone (mel[i:i+1, :, :L_i]) on
+ * packed[voice[i]] at the same precision, and 0.0 past it.  Limits: at most MG_GEN_RAGGED_MAX_B runs, a run being
+ * consecutive items of the same length and the same voice (B itself may exceed it when few runs remain).  Items need not
+ * be sorted by voice, but the call is fastest when they are: at every change of voice the conv_pre and ConvT grids start
+ * a new tile (a tile never holds two voices), and each persistent stride-2 ConvT CTA that walks into another voice
+ * reloads that layer's weights.  Refused with MG_ERR_INVALID_ARGUMENT before any CUDA call: n_voices < 1, a NULL or
+ * misaligned blob, a voice id out of range, any argument mg_gen_forward_precision refuses, and a chain other than the
+ * default one (mg_gen_set_pipeline, MG_GEN_TAIL, MG_GEN_FUSE_UP) at either precision.  mg_gen_check_status and
+ * mg_gen_stage_output work as after mg_gen_forward_precision.  Asynchronous on `stream`, no allocation; concurrent calls
+ * on different streams need different workspaces. */
+int mg_gen_forward_voices(const void *const *packed, int n_voices, const int *voice, const float *mel, float *audio, int B,
+                          int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream);
+
 /* Streaming vocoder: many live sessions, mel frames pushed a few at a time, each audio sample emitted once it is final.
  * A handle serves up to max_sessions (<= MG_GEN_RAGGED_MAX_B) slots at one precision.  Each mg_gen_stream_step gives slot i
  * (i < n) a push of frames[i] in [0, max_push_frames] new mel frames and flags[i] (flags NULL: all 0):

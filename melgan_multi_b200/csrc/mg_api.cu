@@ -16,12 +16,12 @@ static int *status_ptr(void *workspace, int B, int T) {
 
 // batch: mel lengths (stride T); mel_host / audio_host: optional pinned host buffers (the engine entry point); the copies
 // ride on the batch slices' streams
-static int run_generator(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, cudaStream_t s,
+static int run_generator(const float *mel, float *audio, const RunTable &batch, float *ws, cudaStream_t s,
                          cudaEvent_t *ev, const float *mel_host = nullptr, float *audio_host = nullptr,
                          int precision = MG_GEN_PRECISION_FP32) {
     int *st = status_ptr(ws, batch.items(), batch.stride);
     MG_CUDA_TRY(cudaMemsetAsync(st, 0, sizeof(int), s));
-    return launch_generator_tc(packed, mel, audio, batch, ws, st, s, ev, mel_host, audio_host, precision);
+    return launch_generator_tc(mel, audio, batch, ws, st, s, ev, mel_host, audio_host, precision);
 }
 
 // a known precision, and bf16 only on the default chain (the only one with single-pass kernels)
@@ -123,7 +123,7 @@ int mg_gen_forward(const void *packed, const float *mel, float *audio, int B, in
     int rc = check_shape("mg_gen_forward", B, T);
     if (!rc) rc = check_forward("mg_gen_forward", packed, mel, audio, B, T, workspace, workspace_bytes);
     if (rc) return rc;
-    return run_generator((const float *)packed, mel, audio, RunTable::uniform(B, T), (float *)workspace, (cudaStream_t)stream,
+    return run_generator(mel, audio, RunTable::uniform(B, T, (const float *)packed), (float *)workspace, (cudaStream_t)stream,
                          nullptr);
 }
 
@@ -132,7 +132,7 @@ int mg_gen_forward_ragged(const void *packed, const float *mel, float *audio, in
     int rc = check_lengths("mg_gen_forward_ragged", B, T_max, lengths);
     if (!rc) rc = check_forward("mg_gen_forward_ragged", packed, mel, audio, B, T_max, workspace, workspace_bytes);
     if (rc) return rc;
-    return run_generator((const float *)packed, mel, audio, RunTable::ragged(lengths, B, T_max), (float *)workspace,
+    return run_generator(mel, audio, RunTable::ragged(lengths, B, T_max, (const float *)packed), (float *)workspace,
                          (cudaStream_t)stream, nullptr);
 }
 
@@ -143,8 +143,44 @@ int mg_gen_forward_precision(const void *packed, const float *mel, float *audio,
     if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
     if (!rc) rc = check_forward(fn, packed, mel, audio, B, T_max, workspace, workspace_bytes);
     if (rc) return rc;
-    return run_generator((const float *)packed, mel, audio, lengths ? RunTable::ragged(lengths, B, T_max) : RunTable::uniform(B, T_max),
+    const float *w = (const float *)packed;
+    return run_generator(mel, audio, lengths ? RunTable::ragged(lengths, B, T_max, w) : RunTable::uniform(B, T_max, w),
                          (float *)workspace, (cudaStream_t)stream, nullptr, nullptr, nullptr, precision);
+}
+
+int mg_gen_forward_voices(const void *const *packed, int n_voices, const int *voice, const float *mel, float *audio, int B,
+                          int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream) {
+    const char *fn = "mg_gen_forward_voices";
+    int rc = check_precision(fn, precision);
+    if (rc) return rc;
+    if (!generator_tc_default_chain())
+        return set_error(MG_ERR_INVALID_ARGUMENT,
+                         "%s: runs the default chain only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected another "
+                         "(tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
+                         fn, generator_tc_tail(), generator_tc_fused_up());
+    if (n_voices < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, n_voices);
+    if (!packed || !voice) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null packed or voice array", fn);
+    for (int v = 0; v < n_voices; ++v) {
+        if (!packed[v]) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] is NULL", fn, v);
+        if ((uintptr_t)packed[v] % 16) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] must be 16-byte aligned", fn, v);
+    }
+    if ((rc = check_shape(fn, B, T_max))) return rc;
+    for (int i = 0; i < B; ++i) {
+        if (voice[i] < 0 || voice[i] >= n_voices)
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: voice[%d] = %d is outside [0, n_voices = %d)", fn, i, voice[i], n_voices);
+        if (lengths && (lengths[i] < 1 || lengths[i] > T_max))
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: lengths[%d] = %d is outside [1, T_max = %d]", fn, i, lengths[i], T_max);
+    }
+    const float *const *blobs = reinterpret_cast<const float *const *>(packed);
+    int runs = 1;  // what RunTable::voices merges: neighbours of equal length and blob
+    for (int i = 1; i < B; ++i)
+        runs += (lengths && lengths[i] != lengths[i - 1]) || blobs[voice[i]] != blobs[voice[i - 1]];
+    if (runs > MG_GEN_RAGGED_MAX_B)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %d runs of equal length and voice exceed MG_GEN_RAGGED_MAX_B = %d", fn, runs,
+                         MG_GEN_RAGGED_MAX_B);
+    if ((rc = check_forward(fn, packed[0], mel, audio, B, T_max, workspace, workspace_bytes))) return rc;
+    return run_generator(mel, audio, RunTable::voices(lengths, B, T_max, blobs, voice), (float *)workspace, (cudaStream_t)stream,
+                         nullptr, nullptr, nullptr, precision);
 }
 
 int mg_gen_forward_timed(const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
@@ -158,7 +194,7 @@ int mg_gen_forward_timed(const void *packed, const float *mel, float *audio, int
     const int n = mg_gen_forward_launches();  // events: one before each launch + one after the last
     cudaEvent_t ev[17];  // at most 12 kernels
     for (int i = 0; i <= n; ++i) MG_CUDA_TRY(cudaEventCreate(&ev[i]));
-    rc = run_generator((const float *)packed, mel, audio, RunTable::uniform(B, T), (float *)workspace, (cudaStream_t)stream, ev);
+    rc = run_generator(mel, audio, RunTable::uniform(B, T, (const float *)packed), (float *)workspace, (cudaStream_t)stream, ev);
     if (rc == MG_OK) {
         cudaError_t e = cudaEventSynchronize(ev[n]);
         if (e != cudaSuccess) rc = set_error(MG_ERR_CUDA, "mg_gen_forward_timed: %s", cudaGetErrorString(e));
@@ -315,21 +351,21 @@ int mg_gen_convt(const void *packed, int stage, const float *x, float *y, int B,
     if (!packed || !x || !y || x == y || stage < 0 || stage > 3 || B < 1 || Lin < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_convt: bad argument");
     return run_one_kernel("mg_gen_convt", (cudaStream_t)stream, [&](int *st) {
-        return launch_convt_tc(x, y, (const float *)packed, stage, RunTable::uniform(B, Lin), st, (cudaStream_t)stream);
+        return launch_convt_tc(x, y, stage, RunTable::uniform(B, Lin, (const float *)packed), st, (cudaStream_t)stream);
     });
 }
 
 int mg_gen_conv_pre(const void *packed, const float *mel, float *y, int B, int T, void *stream) {
     if (!packed || !mel || !y || B < 1 || T < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_conv_pre: bad argument");
     return run_one_kernel("mg_gen_conv_pre", (cudaStream_t)stream, [&](int *st) {
-        return launch_gen_pre_tc(mel, y, (const float *)packed, RunTable::uniform(B, T), st, (cudaStream_t)stream);
+        return launch_gen_pre_tc(mel, y, RunTable::uniform(B, T, (const float *)packed), st, (cudaStream_t)stream);
     });
 }
 
 int mg_gen_resblock_post(const void *packed, const float *x, float *audio, int B, int L, void *stream) {
     if (!packed || !x || !audio || B < 1 || L < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_resblock_post: bad argument");
     return run_one_kernel("mg_gen_resblock_post", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, audio, (const float *)packed, 4, RunTable::uniform(B, L), st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, audio, 4, RunTable::uniform(B, L, (const float *)packed), st, (cudaStream_t)stream);
     });
 }
 
@@ -350,7 +386,7 @@ int mg_gen_resblock_trace(const void *packed, int stage, const float *x, float *
     MG_CUDA_TRY(cudaMalloc(&tr, 128 * sizeof(long long)));
     cudaMemset(st, 0, sizeof(int));
     cudaMemset(tr, 0, 128 * sizeof(long long));
-    int rc = launch_resblock_tc(x, y, (const float *)packed, stage, RunTable::uniform(B, L), st, 0, tr);
+    int rc = launch_resblock_tc(x, y, stage, RunTable::uniform(B, L, (const float *)packed), st, 0, tr);
     if (rc == MG_OK && cudaDeviceSynchronize() != cudaSuccess) rc = set_error(MG_ERR_CUDA, "mg_gen_resblock_trace: kernel failed");
     if (rc == MG_OK) cudaMemcpy(trace_host, tr, 128 * sizeof(long long), cudaMemcpyDeviceToHost);
     cudaFree(st);
@@ -362,7 +398,7 @@ int mg_gen_resblock(const void *packed, int stage, const float *x, float *y, int
     if (!packed || !x || !y || x == y || stage < 0 || stage > 3 || B < 1 || L < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_resblock: bad argument");
     return run_one_kernel("mg_gen_resblock", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, y, (const float *)packed, stage, RunTable::uniform(B, L), st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, y, stage, RunTable::uniform(B, L, (const float *)packed), st, (cudaStream_t)stream);
     });
 }
 
@@ -370,7 +406,7 @@ int mg_gen_resup(const void *packed, int stage, const float *x, float *y, int B,
     if (!packed || !x || !y || x == y || stage < 0 || stage > 2 || B < 1 || L < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_resup: bad argument");
     return run_one_kernel("mg_gen_resup", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, y, (const float *)packed, 20 + stage, RunTable::uniform(B, L), st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, y, 20 + stage, RunTable::uniform(B, L, (const float *)packed), st, (cudaStream_t)stream);
     });
 }
 
@@ -378,7 +414,7 @@ int mg_gen_upres(const void *packed, int stage, const float *x, float *y, int B,
     if (!packed || !x || !y || x == y || (stage != 2 && stage != 3) || B < 1 || Lin < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_upres: bad argument");
     return run_one_kernel("mg_gen_upres", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, y, (const float *)packed, 10 + stage, RunTable::uniform(B, 2 * Lin), st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, y, 10 + stage, RunTable::uniform(B, 2 * Lin, (const float *)packed), st, (cudaStream_t)stream);
     });
 }
 
@@ -386,7 +422,7 @@ int mg_gen_upres_post(const void *packed, const float *x, float *audio, int B, i
     if (!packed || !x || !audio || (const void *)x == (const void *)audio || B < 1 || Lin < 1)
         return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_upres_post: bad argument");
     return run_one_kernel("mg_gen_upres_post", (cudaStream_t)stream, [&](int *st) {
-        return launch_resblock_tc(x, audio, (const float *)packed, 14, RunTable::uniform(B, 2 * Lin), st, (cudaStream_t)stream);
+        return launch_resblock_tc(x, audio, 14, RunTable::uniform(B, 2 * Lin, (const float *)packed), st, (cudaStream_t)stream);
     });
 }
 
@@ -440,9 +476,10 @@ int mg_gen_chain_kernel(const void *packed, int k, const float *x, float *y, int
                          "%s: runs the default chain's kernels only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected "
                          "another (tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
                          fn, generator_tc_tail(), generator_tc_fused_up());
-    const RunTable t = lengths ? RunTable::ragged(lengths, B, L_max) : RunTable::uniform(B, L_max);
+    const float *w = (const float *)packed;
+    const RunTable t = lengths ? RunTable::ragged(lengths, B, L_max, w) : RunTable::uniform(B, L_max, w);
     return run_one_kernel(fn, (cudaStream_t)stream, [&](int *st) {
-        return launch_chain_kernel(k, x, y, (const float *)packed, t, st, (cudaStream_t)stream, precision);
+        return launch_chain_kernel(k, x, y, t, st, (cudaStream_t)stream, precision);
     });
 }
 
@@ -669,7 +706,7 @@ static int engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_
     if (!e->pin_status) MG_CUDA_TRY(cudaMallocHost(&e->pin_status, sizeof(int)));
     MG_CUDA_TRY(cudaEventRecord(e->ev0, e->stream));
     // upload, kernels and download are enqueued per batch slice (launch_generator_tc); one synchronisation at the end
-    rc = run_generator(e->packed, e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : e->pin_out,
+    rc = run_generator(e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : e->pin_out,
                        precision);
     if (rc) return rc;
     MG_CUDA_TRY(cudaEventRecord(e->ev1, e->stream));
@@ -686,13 +723,13 @@ static int engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_
 int mg_gen_engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T) {
     int rc = engine_check("mg_gen_engine_forward", e, mel_host, audio_host);
     if (!rc) rc = check_shape("mg_gen_engine_forward", B, T);
-    return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::uniform(B, T));
+    return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::uniform(B, T, e->packed));
 }
 
 int mg_gen_engine_forward_ragged(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max, const int *lengths) {
     int rc = check_lengths("mg_gen_engine_forward_ragged", B, T_max, lengths);
     if (!rc) rc = engine_check("mg_gen_engine_forward_ragged", e, mel_host, audio_host);
-    return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::ragged(lengths, B, T_max));
+    return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::ragged(lengths, B, T_max, e->packed));
 }
 
 int mg_gen_engine_forward_precision(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max,
@@ -702,7 +739,8 @@ int mg_gen_engine_forward_precision(mg_gen_engine *e, const float *mel_host, flo
     if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
     if (!rc) rc = engine_check(fn, e, mel_host, audio_host);
     if (rc) return rc;
-    return engine_forward(e, mel_host, audio_host, lengths ? RunTable::ragged(lengths, B, T_max) : RunTable::uniform(B, T_max),
+    return engine_forward(e, mel_host, audio_host, lengths ? RunTable::ragged(lengths, B, T_max, e->packed)
+                                                         : RunTable::uniform(B, T_max, e->packed),
                           precision);
 }
 

@@ -37,39 +37,53 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
 
-// A generator batch as runs of consecutive items of equal length: items [item0[r], item0[r+1]) hold len[r] positions
-// each, stored `stride` positions apart (the longest item's length, at the tensor's scale).  A uniform batch is one run,
-// a ragged one (mg_gen_forward_ragged) at most MG_GEN_RAGGED_MAX_B.  Each generator kernel takes the table BY VALUE
-// (__grid_constant__: read in place from the parameter bank) once its launcher has filled in the kernel's units -- ResBlock
+// A generator batch as runs of consecutive items of equal length and voice: items [item0[r], item0[r+1]) hold len[r]
+// positions each, stored `stride` positions apart (the longest item's length, at the tensor's scale), and take their
+// weights from blob[r] (a blob of mg_gen_pack: the run's voice).  A uniform batch is one run, a ragged or multi-voice one
+// (mg_gen_forward_ragged, mg_gen_forward_voices) at most MG_GEN_RAGGED_MAX_B.  Each generator kernel takes the table BY
+// VALUE (__grid_constant__: read in place from the parameter bank; 6160 bytes with the blob pointers, under the 32764 bytes
+// of kernel parameters sm_90a allows since CUDA 12.1) once its launcher has filled in the kernel's units -- ResBlock
 // clusters, or virtual rows for conv_pre and the ConvTs: run r has per[r] units per item and starts at unit first[r].
-// A grid of first[n] units covers every item and nothing past any item's end.
+// A grid of first[n] units covers every item and nothing past any item's end.  Where the voice changes, first[r] is
+// rounded up to the kernel's tile (set_units): the units in between belong to no item, so no tile holds two voices.
 struct RunPos {
-    int item, unit, len;  // item -1: the unit lies past the last run
+    int item, unit, len;  // item -1: the unit lies past the last run, or in the gap before a voice's first tile
 };
 struct RunTable {
     int n, stride;
     int item0[MG_GEN_RAGGED_MAX_B + 1], len[MG_GEN_RAGGED_MAX_B];
     int first[MG_GEN_RAGGED_MAX_B + 1], per[MG_GEN_RAGGED_MAX_B];
+    const float *blob[MG_GEN_RAGGED_MAX_B];
 
-    static RunTable uniform(int B, int L) {
+    static RunTable uniform(int B, int L, const float *packed) {
         RunTable t;
         t.n = 1;
         t.stride = L;
         t.item0[0] = 0;
         t.item0[1] = B;
         t.len[0] = L;
+        t.blob[0] = packed;
         return t;
     }
     // lengths[0..B) (B <= MG_GEN_RAGGED_MAX_B, every length in [1, stride]), equal neighbours merged
-    static RunTable ragged(const int *lengths, int B, int stride) {
+    static RunTable ragged(const int *lengths, int B, int stride, const float *packed) {
+        return voices(lengths, B, stride, &packed, nullptr);
+    }
+    // item i: lengths[i] positions (lengths nullptr: stride), weights blobs[voice[i]] (voice nullptr: blobs[0]); neighbours
+    // of equal length and blob merged
+    static RunTable voices(const int *lengths, int B, int stride, const float *const *blobs, const int *voice) {
         RunTable t;
         t.n = 0;
         t.stride = stride;
-        for (int i = 0; i < B; ++i)
-            if (i == 0 || lengths[i] != lengths[i - 1]) {
+        for (int i = 0; i < B; ++i) {
+            const int L = lengths ? lengths[i] : stride;
+            const float *w = blobs[voice ? voice[i] : 0];
+            if (i == 0 || L != t.len[t.n - 1] || w != t.blob[t.n - 1]) {
                 t.item0[t.n] = i;
-                t.len[t.n++] = lengths[i];
+                t.blob[t.n] = w;
+                t.len[t.n++] = L;
             }
+        }
         t.item0[t.n] = B;
         return t;
     }
@@ -83,6 +97,7 @@ struct RunTable {
             const int a = item0[r] > i0 ? item0[r] : i0, b = item0[r + 1] < i1 ? item0[r + 1] : i1;
             if (a < b) {
                 t.item0[t.n] = a - i0;
+                t.blob[t.n] = blob[r];
                 t.len[t.n++] = len[r];
             }
         }
@@ -96,28 +111,41 @@ struct RunTable {
         for (int r = 0; r < n; ++r) t.len[r] *= k;
         return t;
     }
-    // per[r] = units(len[r]) units per item; first[] follows
+    // per[r] = units(len[r]) units per item; first[] follows, rounded up to a multiple of `tile` where the voice changes
+    // (with one voice the units are contiguous, whatever the tile)
     template <class F>
-    void set_units(F units) {
-        first[0] = 0;
+    void set_units(F units, int tile = 1) {
+        int f = 0;
         for (int r = 0; r < n; ++r) {
+            if (r > 0 && blob[r] != blob[r - 1]) f = (f + tile - 1) / tile * tile;
+            first[r] = f;
             per[r] = units(len[r]);
-            first[r + 1] = first[r] + (item0[r + 1] - item0[r]) * per[r];
+            f += (item0[r + 1] - item0[r]) * per[r];
         }
+        first[n] = f;
     }
-    // unit f -> (item, unit within the item, the item's length)
-    __device__ __forceinline__ RunPos find(int f) const {
-        if (f < 0 || f >= first[n]) return {-1, 0, 0};
+    // the run of unit f, 0 <= f < first[n]
+    __device__ __forceinline__ int run_of(int f) const {
         int lo = 0, hi = n;  // first[lo] <= f < first[hi]
         while (hi - lo > 1) {
             const int m = (lo + hi) >> 1;
             if (first[m] <= f) lo = m;
             else hi = m;
         }
+        return lo;
+    }
+    // the weights of unit f's voice, 0 <= f < first[n] (a gap unit: the voice before it, which owns the rest of its tile)
+    __device__ __forceinline__ const float *blob_at(int f) const { return blob[run_of(f)]; }
+    // unit f -> (item, unit within the item, the item's length)
+    __device__ __forceinline__ RunPos find(int f) const {
+        if (f < 0 || f >= first[n]) return {-1, 0, 0};
+        const int lo = run_of(f);
         const int u = f - first[lo], k = (int)((unsigned)u / (unsigned)per[lo]);  // (unsigned: the shorter division)
+        if (k >= item0[lo + 1] - item0[lo]) return {-1, 0, 0};  // the gap before the next voice's first tile
         return {item0[lo] + k, u - k * per[lo], len[lo]};
     }
 };
+static_assert(sizeof(RunTable) == 6160 && sizeof(RunTable) + 256 <= 32764, "a kernel's parameters: the table and a few more");
 
 // Launch helper of the tensor-core kernels: optional programmatic dependent launch
 // (mg_tc.cuh pdl_*; MG_PDL=0 in the environment turns the attribute off for A/B runs); cluster > 1: thread-block clusters
@@ -166,11 +194,11 @@ const char *generator_tc_kernel_name(int i);
 const char *generator_tc_kernel_config(int i, int T);
 const char *resblock_config_name(int stage, int L);
 int generator_tc_slices(int B, long long frames);  // batch slices (concurrent kernel chains) one forward is cut into
-// batch: the items' mel lengths, stride T_max (the layout of mel, audio and every workspace buffer)
-int launch_generator_tc(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
+// batch: the items' mel lengths, stride T_max (the layout of mel, audio and every workspace buffer), each run's weights
+int launch_generator_tc(const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
                         cudaStream_t s, cudaEvent_t *ev = nullptr, const float *mel_host = nullptr, float *audio_host = nullptr,
                         int precision = MG_GEN_PRECISION_FP32);
-int launch_gen_pre_tc(const float *mel, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s);
+int launch_gen_pre_tc(const float *mel, float *y, const RunTable &batch, int *status, cudaStream_t s);
 int launch_disc_post1_tc(const float *x, float *y, const uint8_t *wtc, const float *bias, int Bt, int L, int *status,
                          cudaStream_t s);
 int launch_disc_post1_dgrad_tc(const float *dz, float *dx, const uint8_t *wtcT, const float *zero_bias, int Bt, int L, int *status,
@@ -213,14 +241,14 @@ int launch_mel(const void *tables, const float *audio, float *mel, int B, int L,
 int launch_msd_forward(const void *packed, const float *y, int Bt, int L, float *const *fmaps, int *status, cudaStream_t s);
 // batch: lengths and stride of the kernel's input (ConvT) / of the ResBlock itself (the output length for codes 12..14)
 // precision: MG_GEN_PRECISION_FP32 (3-pass split bf16) or MG_GEN_PRECISION_BF16 (one pass; only the default chain's kernels)
-int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
+int launch_convt_tc(const float *x, float *y, int stage, const RunTable &batch, int *status, cudaStream_t s,
                     int precision = MG_GEN_PRECISION_FP32);
 const char *convt_config_name(int stage);
 const char *gen_pre_config_name();
 // kernel k (0..7) of the default chain; batch in kernel k's input units (mg_gen_stream.cu)
-int launch_chain_kernel(int k, const float *x, float *y, const float *w, const RunTable &t, int *status, cudaStream_t st,
+int launch_chain_kernel(int k, const float *x, float *y, const RunTable &t, int *status, cudaStream_t st,
                         int precision);
-int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
+int launch_resblock_tc(const float *x, float *y, int stage, const RunTable &batch, int *status, cudaStream_t s,
                        long long *trace = nullptr, int precision = MG_GEN_PRECISION_FP32);
 
 }  // namespace mg

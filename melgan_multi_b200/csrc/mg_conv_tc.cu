@@ -13,6 +13,8 @@
 // channels: [hi, lo][k-panel][N][8] bf16 = 64 N bytes) arrive by 1-D bulk TMA.
 // Warp roles: converter warpgroup (A slots), two MMA warpgroups (rows 0..63 / 64..127; accumulators in registers, they
 // also run the epilogue), one TMA producer warp.
+#include <type_traits>
+
 #include "mg_common.cuh"
 #include "mg_tc.cuh"
 
@@ -68,6 +70,11 @@ conv_rows_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const ui
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * ROWS, cg = blockIdx.y;
     const int L = rows.stride;  // positions between items in x and y
+    if constexpr (std::is_same<Rows, RunTable>::value) {  // conv_pre: the weights of the tile's voice (set_units keeps a
+        const float *vb = rows.blob_at(r0);               // tile within one voice; rows of the gap are never stored)
+        wtc = reinterpret_cast<const uint8_t *>(vb) + tc_region_start() + tc_pre_offset();
+        bias = vb + bias_offset(0);
+    }
 
     if (tid == 0) {
         for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NMW); }
@@ -243,12 +250,11 @@ using PreCfg = ConvCfg<80, 512, 7, 80, false, kPreNG>;  // generator conv_pre
 using Post1Cfg = ConvCfg<1024, 1024, 5, 32, true, kPost1NG>;
 using Post1DgradCfg = ConvCfg<1024, 1024, 5, 32, false, kPost1NG>;  // the same contraction on the transposed blob, no activation
 
-// mel [B][80][T_max] -> y [B][512][T_max]   (Generator.conv_pre), item i's first len_i positions
-int launch_gen_pre_tc(const float *mel, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s) {
-    const uint8_t *wtc = reinterpret_cast<const uint8_t *>(packed) + tc_region_start() + tc_pre_offset();
+// mel [B][80][T_max] -> y [B][512][T_max]   (Generator.conv_pre), item i's first len_i positions, on its run's blob
+int launch_gen_pre_tc(const float *mel, float *y, const RunTable &batch, int *status, cudaStream_t s) {
     RunTable rows = batch;
-    rows.set_units([](int L) { return L + PreCfg::PAD; });
-    return launch_conv_rows<PreCfg>(mel, y, wtc, packed + bias_offset(0), rows, rows.first[rows.n], status, s);
+    rows.set_units([](int L) { return L + PreCfg::PAD; }, PreCfg::ROWS);
+    return launch_conv_rows<PreCfg>(mel, y, nullptr, nullptr, rows, rows.first[rows.n], status, s);  // (weights: rows.blob)
 }
 
 // conv_pre's tile geometry: ROWS virtual rows per CTA (each item's positions followed by PAD zero rows), N output channels

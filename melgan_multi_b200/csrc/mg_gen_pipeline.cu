@@ -88,11 +88,11 @@ const char *generator_tc_kernel_config(int i, int T) {
     return st[i].kind == 0 ? "conv_rows_tc_kernel<ConvCfg<80,512,7>>" : "convt_tc_kernel";
 }
 
-// Tensor-core pipeline of one contiguous slice of the batch (mel lengths, stride T_max).  a0: conv_pre output; a[0]:
+// Tensor-core pipeline of one contiguous slice of the batch (mel lengths, stride T_max, each run's weights).  a0: conv_pre output; a[0]:
 // ResBlock-0 output (unfused chains); a[1], a[2], u: three buffers of 8192 T_max floats per item that the stages rotate
 // through (a kernel never writes its input).  Every kernel gets the batch at its own scale.  precision goes to the ConvT
 // and ResBlock kernels (conv_pre always runs its three passes).
-static int generator_tc_chain(const float *packed, const float *mel, float *audio, const RunTable &batch, float *a0,
+static int generator_tc_chain(const float *mel, float *audio, const RunTable &batch, float *a0,
                               float *const *a, float *u, int *status, cudaStream_t s, cudaEvent_t *ev, int precision) {
     ChainStep st[12];
     const int n = build_chain(st);
@@ -109,11 +109,11 @@ static int generator_tc_chain(const float *packed, const float *mel, float *audi
         if (ev) MG_CUDA_TRY(cudaEventRecord(ev[i], s));
         const ChainStep &k = st[i];
         if (k.kind == 0) {
-            if ((rc = launch_gen_pre_tc(cur, a0, packed, batch, status, s))) return rc;
+            if ((rc = launch_gen_pre_tc(cur, a0, batch, status, s))) return rc;
             cur = a0;
         } else if (k.kind == 1) {
             float *out = cur != u ? u : other(cur, nullptr);  // (unfused chain: ConvT outputs live in u, ResBlock i's in a[i])
-            if ((rc = launch_convt_tc(cur, out, packed, k.arg, batch.scaled(len), status, s, precision))) return rc;
+            if ((rc = launch_convt_tc(cur, out, k.arg, batch.scaled(len), status, s, precision))) return rc;
             cur = out;
             len *= stage_stride(k.arg);
         } else {
@@ -122,7 +122,7 @@ static int generator_tc_chain(const float *packed, const float *mel, float *audi
             const bool front = k.arg >= 12 && k.arg <= 14, tailf = k.arg >= 20;
             float *out = last ? audio : (k.arg <= 2 && cur != a[k.arg]) ? a[k.arg] : other(cur, nullptr);
             const int Lk = front ? 2 * len : len;  // the ResBlock's own length
-            if ((rc = launch_resblock_tc(cur, out, packed, k.arg, batch.scaled(Lk), status, s, nullptr, precision))) return rc;
+            if ((rc = launch_resblock_tc(cur, out, k.arg, batch.scaled(Lk), status, s, nullptr, precision))) return rc;
             cur = out;
             len = tailf ? Lk * stage_stride(k.arg - 20 + 1) : Lk;
         }
@@ -156,7 +156,8 @@ struct SliceStreams {
 // the block scheduler fills the SMs one chain's partial last wave leaves idle (stage 0 at config 2 is 512 one-per-SM
 // tiles on 132 SMs) with the other chain's tiles.  Same kernels, same per-item arithmetic: results are bit-identical
 // to the single-chain order.  ev != nullptr (per-kernel timing) keeps everything on one stream.
-// frames: mel frames of the whole batch (B T for a uniform one); the parts hold about equal shares of them.
+// frames: mel frames of the whole batch (B T for a uniform one); the parts hold about equal shares of them.  A cut goes
+// wherever the frame count puts it, between items of one voice or of two: each slice carries its items' blobs.
 int generator_tc_slices(int B, long long frames) {
     static const int forced = [] {  // MG_GEN_SLICES=n pins the slice count (experiments); default: chosen from the shape
         const char *e = getenv("MG_GEN_SLICES");
@@ -173,7 +174,7 @@ int generator_tc_slices(int B, long long frames) {
 // stream uploads its items' valid mel prefixes before its chain and downloads its audio rows (valid prefix and zero tail)
 // after it, so all but the last download overlap the other chains' kernels.  precision: MG_GEN_PRECISION_*; the caller
 // has checked that a bf16 forward runs the default chain.
-int launch_generator_tc(const float *packed, const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
+int launch_generator_tc(const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
                         cudaStream_t s, cudaEvent_t *ev, const float *mel_host, float *audio_host, int precision) {
     const int B = batch.items(), T = batch.stride;
     long long frames = 0;
@@ -228,7 +229,7 @@ int launch_generator_tc(const float *packed, const float *mel, float *audio, con
                                                   rows, cudaMemcpyHostToDevice, q));
             }
             float *a[3] = {base[1] + b0 * per_item[1], base[2] + b0 * per_item[2], base[3] + b0 * per_item[3]};
-            int r = generator_tc_chain(packed, mel + b0 * mel_item, audio + b0 * audio_item, part, base[0] + b0 * per_item[0], a,
+            int r = generator_tc_chain(mel + b0 * mel_item, audio + b0 * audio_item, part, base[0] + b0 * per_item[0], a,
                                        base[5] + b0 * per_item[5], status, q, ev, precision);
             if (r) return r;
             if (audio_host)

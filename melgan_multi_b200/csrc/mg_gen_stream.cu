@@ -173,17 +173,17 @@ struct Plan {
 
 // Kernel k of the default chain: x [B][kC[k]][stride] -> y [B][kC[k + 1]][kRatio[k] stride], t in kernel k's input units.
 // What mg_gen_stream_step launches per kernel, and mg_gen_chain_kernel alone.
-int launch_chain_kernel(int k, const float *x, float *y, const float *w, const RunTable &t, int *status, cudaStream_t st,
+int launch_chain_kernel(int k, const float *x, float *y, const RunTable &t, int *status, cudaStream_t st,
                         int precision) {
     switch (k) {
-        case 0: return launch_gen_pre_tc(x, y, w, t, status, st);
-        case 1: return launch_convt_tc(x, y, w, 0, t, status, st, precision);
-        case 2: return launch_resblock_tc(x, y, w, 0, t, status, st, nullptr, precision);
-        case 3: return launch_convt_tc(x, y, w, 1, t, status, st, precision);
-        case 4: return launch_resblock_tc(x, y, w, 1, t, status, st, nullptr, precision);
-        case 5: return launch_convt_tc(x, y, w, 2, t, status, st, precision);
-        case 6: return launch_resblock_tc(x, y, w, 2, t, status, st, nullptr, precision);
-        case 7: return launch_resblock_tc(x, y, w, 14, t.scaled(2), status, st, nullptr, precision);
+        case 0: return launch_gen_pre_tc(x, y, t, status, st);
+        case 1: return launch_convt_tc(x, y, 0, t, status, st, precision);
+        case 2: return launch_resblock_tc(x, y, 0, t, status, st, nullptr, precision);
+        case 3: return launch_convt_tc(x, y, 1, t, status, st, precision);
+        case 4: return launch_resblock_tc(x, y, 1, t, status, st, nullptr, precision);
+        case 5: return launch_convt_tc(x, y, 2, t, status, st, precision);
+        case 6: return launch_resblock_tc(x, y, 2, t, status, st, nullptr, precision);
+        case 7: return launch_resblock_tc(x, y, 14, t.scaled(2), status, st, nullptr, precision);
     }
     return set_error(MG_ERR_INVALID_ARGUMENT, "launch_chain_kernel: kernel %d", k);
 }
@@ -384,7 +384,7 @@ int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, c
         c.dst_row = stride;
         if ((rc = launch_window(c, p.asm_[k], p.asm_elems[k], st))) return rc;
         if (p.items[k] == 0) continue;  // (no later kernel has items either: nothing was made final here)
-        if ((rc = launch_chain_kernel(k, win, out, w, RunTable::ragged(p.lens[k], p.items[k], stride), status, st, s->precision)))
+        if ((rc = launch_chain_kernel(k, win, out, RunTable::ragged(p.lens[k], p.items[k], stride, w), status, st, s->precision)))
             return rc;
         prev = out;
         prev_row = kRatio[k] * stride;

@@ -116,8 +116,8 @@ __device__ __forceinline__ void acc_fence2(float (&a)[RPW][R]) {
 
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NT, 1)
-resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed, int stage,
-                   const __grid_constant__ RunTable clusters, int *__restrict__ status, long long *__restrict__ trace) {
+resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, int stage, const __grid_constant__ RunTable clusters,
+                   int *__restrict__ status, long long *__restrict__ trace) {
     constexpr int C = Cfg::C, P = Cfg::P, SLACK = Cfg::SLACK, HALO = Cfg::HALO, HL = Cfg::HL;
     constexpr int XPITCH = Cfg::XPITCH, XBYTES = Cfg::XBYTES, KC = Cfg::KC, CHUNK = Cfg::CHUNK, NSTAGE = Cfg::NSTAGE;
     constexpr int NCONS = Cfg::NCONS, NCP = Cfg::NCP, NCW = Cfg::NCW, RPW = Cfg::RPW, KSL = Cfg::KSL, NA = NCW / 2;
@@ -162,6 +162,14 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     const int crank = blockIdx.x % CS;
     const RunPos cp = clusters.find(blockIdx.x / CS);
     const int clus = cp.unit, Ls = clusters.stride;
+    // the weights of the item's voice: a cluster never spans two items, so every CTA of a cluster reads the same blob and
+    // the chunk one rank multicasts is the one each of them expects.  Looked up where it is used (the index opaque to the
+    // compiler): a pointer held across the MMA loops would cost registers the tiles need.
+    auto voice_blob = [&]() {
+        int c = blockIdx.x / CS;
+        asm volatile("" : "+r"(c));
+        return clusters.blob_at(c);
+    };
     auto item = [&]() { return *reinterpret_cast<volatile int *>(&item_len[0]); };
     auto len = [&]() { return *reinterpret_cast<volatile int *>(&item_len[1]); };
     // Edge-aware tiling: a halo is only needed where the cluster (one CTA for CS = 1) borders MORE sequence.  Cluster 0
@@ -175,7 +183,6 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     const bool interior = (o >= 0 && o + P <= cp.len);  // every row of the tile is a real position
     // consumption order of the six convs of ResBlock `stage`: c1[0], c2[0], c1[1], c2[1], c1[2], c2[2]
     const int l0 = 5 + 6 * stage;
-    const uint8_t *tc_base = reinterpret_cast<const uint8_t *>(packed) + tc_region_start();
 
     if (tid == 0) {
         item_len[0] = cp.item;
@@ -199,6 +206,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
     for (int i = tid; i < C; i += Cfg::NT) pend[i] = 0.f;
     // the constants come from the packed blob, not from the previous kernel: read before pdl_wait(), like the weight stream,
     // so that no global load sits between a hand-off and the next conv
+    const float *packed = voice_blob();
     for (int i = tid; i < Cfg::NCONST; i += Cfg::NT) {
         float v = 0.f;
         if (i < Cfg::CB_UPF) v = __ldg(packed + bias_offset(l0) + i);  // layers l0 .. l0 + 5 have C biases each
@@ -229,6 +237,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         // Single pass: only the first WBYTES = HALF bytes of a chunk, its hi half, are sent and expected; of a stacked chunk,
         // whose hi rows are not contiguous, all of it.)
         if (lane == 0) {
+            const uint8_t *tc_base = reinterpret_cast<const uint8_t *>(voice_blob()) + tc_region_start();
             int s = 0, ph = 0, j = 0;
             bool ok = true;
             auto put = [&](const uint8_t *src, uint32_t bytes) {
@@ -668,7 +677,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
         {
             const int pl = L - 1 - o;  // tile-local row of position L - 1
             if (pl >= p_lo && pl < p_hi) {  // CTA-uniform; b1s[] was written before the last hand-off's barrier
-                const float *wf = packed + weight_offset(1 + stage + 1);
+                const float *wf = voice_blob() + weight_offset(1 + stage + 1);
                 for (int i = tid; i < PADT * COT; i += NCONS) {
                     const int co = i / PADT, j = i - co * PADT;
                     const float *wp = wf + ((size_t)co * S + j) * 2 + 1;  // + ci * COT * S * 2
@@ -780,7 +789,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const flo
 }
 
 template <class Cfg>
-static int launch_resblock(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status,
+static int launch_resblock(const float *x, float *y, int stage, const RunTable &batch, int *status,
                            long long *trace, cudaStream_t s) {
     static bool configured = false;
     if (!configured) {
@@ -807,7 +816,7 @@ static int launch_resblock(const float *x, float *y, const float *packed, int st
         const long long v = n;
         MG_CUDA_TRY(cudaMemcpy(trace + 127, &v, sizeof(v), cudaMemcpyHostToDevice));
     }
-    MG_CUDA_TRY(launch_ex(resblock_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, CS, x, y, packed, stage, clusters,
+    MG_CUDA_TRY(launch_ex(resblock_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, CS, x, y, stage, clusters,
                           status, trace));
     return MG_OK;
 }
@@ -844,31 +853,31 @@ using Rb2Up3 = RbCfg<64, 4, 1, 1, 3, false, false, 2>;
 // x, y: [B][C][L] fp32 NCL with C = 256 >> stage, L = batch.stride, item i's first len_i positions its own; status: device
 // int, set non-zero if a pipeline wait timed out.  precision MG_GEN_PRECISION_BF16: the single-pass variant, which exists
 // for the default chain's stage codes 0, 1, 2 and 14.
-int launch_resblock_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
+int launch_resblock_tc(const float *x, float *y, int stage, const RunTable &batch, int *status, cudaStream_t s,
                        long long *trace, int precision) {
     if (precision == MG_GEN_PRECISION_BF16) {
         switch (stage) {
-            case 0: return launch_resblock<Bf16<Rb0>>(x, y, packed, 0, batch, status, trace, s);
-            case 1: return launch_resblock<Bf16<Rb1>>(x, y, packed, 1, batch, status, trace, s);
-            case 2: return launch_resblock<Bf16<Rb2>>(x, y, packed, 2, batch, status, trace, s);
-            case 14: return launch_resblock<Bf16<Up3Rb3Post>>(x, y, packed, 3, batch, status, trace, s);
+            case 0: return launch_resblock<Bf16<Rb0>>(x, y, 0, batch, status, trace, s);
+            case 1: return launch_resblock<Bf16<Rb1>>(x, y, 1, batch, status, trace, s);
+            case 2: return launch_resblock<Bf16<Rb2>>(x, y, 2, batch, status, trace, s);
+            case 14: return launch_resblock<Bf16<Up3Rb3Post>>(x, y, 3, batch, status, trace, s);
         }
         return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: stage code %d has no bf16 variant", stage);
     }
     if (precision != MG_GEN_PRECISION_FP32)
         return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: precision %d", precision);
     switch (stage) {
-        case 0: return launch_resblock<Rb0>(x, y, packed, 0, batch, status, trace, s);
-        case 1: return launch_resblock<Rb1>(x, y, packed, 1, batch, status, trace, s);
-        case 2: return launch_resblock<Rb2>(x, y, packed, 2, batch, status, trace, s);
-        case 3: return launch_resblock<Rb3>(x, y, packed, 3, batch, status, trace, s);
-        case 4: return launch_resblock<Rb3Post>(x, y, packed, 3, batch, status, trace, s);
-        case 12: return launch_resblock<Up2Rb2>(x, y, packed, 2, batch, status, trace, s);
-        case 13: return launch_resblock<Up3Rb3>(x, y, packed, 3, batch, status, trace, s);
-        case 14: return launch_resblock<Up3Rb3Post>(x, y, packed, 3, batch, status, trace, s);
-        case 20: return launch_resblock<Rb0Up1>(x, y, packed, 0, batch, status, trace, s);
-        case 21: return launch_resblock<Rb1Up2>(x, y, packed, 1, batch, status, trace, s);
-        case 22: return launch_resblock<Rb2Up3>(x, y, packed, 2, batch, status, trace, s);
+        case 0: return launch_resblock<Rb0>(x, y, 0, batch, status, trace, s);
+        case 1: return launch_resblock<Rb1>(x, y, 1, batch, status, trace, s);
+        case 2: return launch_resblock<Rb2>(x, y, 2, batch, status, trace, s);
+        case 3: return launch_resblock<Rb3>(x, y, 3, batch, status, trace, s);
+        case 4: return launch_resblock<Rb3Post>(x, y, 3, batch, status, trace, s);
+        case 12: return launch_resblock<Up2Rb2>(x, y, 2, batch, status, trace, s);
+        case 13: return launch_resblock<Up3Rb3>(x, y, 3, batch, status, trace, s);
+        case 14: return launch_resblock<Up3Rb3Post>(x, y, 3, batch, status, trace, s);
+        case 20: return launch_resblock<Rb0Up1>(x, y, 0, batch, status, trace, s);
+        case 21: return launch_resblock<Rb1Up2>(x, y, 1, batch, status, trace, s);
+        case 22: return launch_resblock<Rb2Up3>(x, y, 2, batch, status, trace, s);
     }
     return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: stage %d", stage);
 }

@@ -59,7 +59,7 @@ struct UpCfg {
     static constexpr int NCHUNK = CIN / 16;               // B slots per tile
     static constexpr int NCONV = 128;                     // converter threads
     static constexpr int NT = NCONV + 128 * NMW + 32;
-    static constexpr int SMEM_BYTES = NSA * ASLOT + NSB * BSLOT + (2 * NSA + 2 * NSB) * 8;
+    static constexpr int SMEM_BYTES = NSA * ASLOT + NSB * BSLOT + (2 * NSA + 2 * NSB + 1) * 8;  // (+ the tile's blob pointer)
     static_assert(N <= 256 && N % 16 == 0, "wgmma N");
     static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "shared memory budget");
     static_assert(CIN % KCA == 0, "A slot");
@@ -119,10 +119,16 @@ __device__ __forceinline__ void load_bslot(uint8_t *dst, const uint8_t *src, uin
     }
 }
 
+// The weights of the tile at virtual row r0: set_units keeps a tile within one voice.  Looked up where they are used
+// (r0 opaque to the compiler), so that no pointer stays live next to the accumulators.
+__device__ __forceinline__ const float *tile_blob(const RunTable &rows, int r0) {
+    asm volatile("" : "+r"(r0));
+    return rows.blob_at(r0);
+}
+
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NT, 1)
-convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed,
-                const __grid_constant__ RunTable rows, int *__restrict__ status) {
+convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const __grid_constant__ RunTable rows, int *__restrict__ status) {
     constexpr int CIN = Cfg::CIN, N = Cfg::N, NG = Cfg::NG;
     constexpr int ROWS = Cfg::ROWS, APITCH = Cfg::APITCH, ASLOT = Cfg::ASLOT, BSLOT = Cfg::BSLOT, KCA = Cfg::KCA;
     constexpr int NSA = Cfg::NSA, NSB = Cfg::NSB, NCHUNK = Cfg::NCHUNK, NCONV = Cfg::NCONV, NMW = Cfg::NMW;
@@ -131,6 +137,9 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
     uint8_t *aring = smem, *bring = smem + NSA * ASLOT;
     uint64_t *fullA = reinterpret_cast<uint64_t *>(bring + NSB * BSLOT);
     uint64_t *emptyA = fullA + NSA, *fullB = emptyA + NSA, *emptyB = fullB + NSB;
+    // the tile's weights, looked up once: the epilogue reads the pointer back instead of searching the table while the
+    // accumulators are live
+    const float **vblob = reinterpret_cast<const float **>(emptyB + NSB);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * ROWS;  // first virtual row of the tile
@@ -138,6 +147,7 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
     const int Lin = rows.stride;  // input positions between items
 
     if (tid == 0) {
+        *vblob = rows.blob_at(r0);  // set_units keeps a tile within one voice
         for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NMW); }
         for (int s = 0; s < NSB; ++s) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], NMW); }
         fence_mbar_init();
@@ -147,7 +157,7 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
     if (warp == (NCONV + 128 * NMW) / 32) {
         // ================= TMA producer: one B slot per 16 input channels =================
         if (lane == 0) {
-            const uint8_t *src = reinterpret_cast<const uint8_t *>(packed) + tc_region_start() + tc_up_offset(Cfg::STAGE) +
+            const uint8_t *src = reinterpret_cast<const uint8_t *>(*vblob) + tc_region_start() + tc_up_offset(Cfg::STAGE) +
                                  (size_t)cg * NCHUNK * BSLOT;
             int s = 0, ph = 0;
             bool ok = true;
@@ -202,7 +212,8 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
         if (!ok && t == 0) atomicExch(status, 13);
         pdl_trigger();  // MMAs done, only the output store is left: the next kernel of the chain may be scheduled
         pdl_wait();
-        convt_store<Cfg>(acc, y, packed + bias_offset(1 + Cfg::STAGE) + cg * NG, mw, t, cg, Cfg::S * Lin,
+        const float *vb = *reinterpret_cast<const float *volatile *>(vblob);
+        convt_store<Cfg>(acc, y, vb + bias_offset(1 + Cfg::STAGE) + cg * NG, mw, t, cg, Cfg::S * Lin,
                          [&](int m) { return rows.find(r0 + m); });
     } else {
         // ================= converter warps: A slots = split(lrelu(x)), KCA channels of every row =================
@@ -238,23 +249,23 @@ convt_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float 
     }
 }
 
-// Lin + 1 virtual rows per item: position s = Lin feeds the last `pad` outputs
-static RunTable convt_rows(const RunTable &batch) {
+// Lin + 1 virtual rows per item: position s = Lin feeds the last `pad` outputs; a voice starts at a multiple of `tile`
+static RunTable convt_rows(const RunTable &batch, int tile) {
     RunTable rows = batch;
-    rows.set_units([](int Lin) { return Lin + 1; });
+    rows.set_units([](int Lin) { return Lin + 1; }, tile);
     return rows;
 }
 
 template <class Cfg>
-static int launch_convt(const float *x, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s) {
+static int launch_convt(const float *x, float *y, const RunTable &batch, int *status, cudaStream_t s) {
     static bool configured = false;
     if (!configured) {
         MG_CUDA_TRY(cudaFuncSetAttribute(convt_tc_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         configured = true;
     }
-    const RunTable rows = convt_rows(batch);
+    const RunTable rows = convt_rows(batch, Cfg::ROWS);
     dim3 grid((unsigned)((rows.first[rows.n] + Cfg::ROWS - 1) / Cfg::ROWS), Cfg::NCG);
-    MG_CUDA_TRY(launch_ex(convt_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, 1, x, y, packed, rows, status));
+    MG_CUDA_TRY(launch_ex(convt_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, 1, x, y, rows, status));
     return MG_OK;
 }
 
@@ -262,7 +273,8 @@ static int launch_convt(const float *x, float *y, const float *packed, const Run
 // Streaming kernel of the stride-2 stages.  Per output element it computes exactly what convt_tc_kernel would (the same
 // A and B operands, MMA order, 3 passes and bias add); only the data movement differs:
 //  - persistent CTAs, one per SM (grid = min(tiles, SMs)), walk the row tiles blockIdx.x, + gridDim.x, ...  The layer's
-//    whole B operand (NCHUNK slots: 128 KB at stage 2, one channel group) is loaded once per CTA and stays resident;
+//    whole B operand (NCHUNK slots: 128 KB at stage 2, one channel group) is loaded once per CTA and stays resident,
+//    until the walk reaches a tile of another voice (multi-voice batches): then it is loaded again, see the kernel;
 //  - a tile's input arrives by 1-D bulk copies, one per (channel, item segment) of the 16-byte-aligned superset of the
 //    segment, into a ring of NSX fp32 staging slots of KCA channels.  The producer warp (lane c: channel c of the slot)
 //    runs up to NSX slots ahead, across tiles, so the next tile's loads are in flight under this tile's MMAs and stores;
@@ -284,7 +296,7 @@ struct StreamCfg {
     static constexpr int FIXED = BRES + NSA * Cfg::ASLOT + 256;  // (+ the mbarriers)
     static constexpr int NSX = (227 * 1024 - 1024 - FIXED) / XSLOT < 4 ? (227 * 1024 - 1024 - FIXED) / XSLOT : 4;
     static constexpr int NT = Cfg::NCONV + 128 * Cfg::NMW + 32;
-    static constexpr int SMEM_BYTES = BRES + NSA * Cfg::ASLOT + NSX * XSLOT + (1 + 2 * NSA + 2 * NSX) * 8;
+    static constexpr int SMEM_BYTES = BRES + NSA * Cfg::ASLOT + NSX * XSLOT + (2 + 2 * NSA + 2 * NSX) * 8;
     static_assert(NSX >= 2 && SMEM_BYTES + 1024 <= 227 * 1024, "shared memory budget");
     static_assert(XPITCH % 4 == 0 && Cfg::KCA == 32, "staging slot: 16-byte channel rows, one channel per producer lane");
 };
@@ -295,15 +307,17 @@ struct XSeg {
     int i0, n, item, u0, dst;
 };
 // The staged segments of the tile at virtual row r0 (A row i = virtual row r0 - 1 + i); producer and converter both call
-// it.  Rows below `covered` outside every segment are zero rows (row -1, an item's zero row); rows from `covered` on
-// (only with items shorter than 64 positions) are not staged.
+// it.  Rows below `covered` outside every segment are zero rows (row -1, an item's zero row, a gap row before the first
+// tile of a voice); rows from `covered` on (with items shorter than 64 positions, or a gap at the tile's end) are not
+// staged.
 template <class SC>
 __device__ __forceinline__ void tile_segments(const RunTable &rows, int r0, XSeg (&seg)[SC::MAXSEG], int &covered) {
     int i = r0 == 0 ? 1 : 0, dst = 0;
 #pragma unroll
     for (int k = 0; k < SC::MAXSEG; ++k) {
         RunPos p = rows.find(r0 - 1 + i);
-        if (i < SC::AR && p.item >= 0 && p.unit == p.len) p = rows.find(r0 - 1 + ++i);  // skip an item's zero row
+        // skip an item's zero row, or the gap row before r0 (r0 itself always belongs to an item: see set_units)
+        if (i < SC::AR && (p.item >= 0 ? p.unit == p.len : i == 0)) p = rows.find(r0 - 1 + ++i);
         const int n = (i < SC::AR && p.item >= 0) ? min(p.len - p.unit, SC::AR - i) : 0;
         seg[k] = {i, n, p.item, p.unit, dst};
         dst += (n + 6) & ~3;
@@ -352,22 +366,36 @@ __device__ __forceinline__ void convt_stream_store(const float *acc, const float
 
 template <class Cfg>
 __global__ void __launch_bounds__(StreamCfg<Cfg>::NT, 1)
-convt_stream_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed,
-                       const __grid_constant__ RunTable rows, int ntiles, int *__restrict__ status) {
+convt_stream_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const __grid_constant__ RunTable rows, int ntiles,
+                       int *__restrict__ status) {
     using SC = StreamCfg<Cfg>;
     constexpr int CIN = Cfg::CIN, N = Cfg::N, NG = Cfg::NG, KCA = Cfg::KCA, NCONV = Cfg::NCONV, NMW = Cfg::NMW;
     constexpr int ROWS = Cfg::ROWS, APITCH = Cfg::APITCH, ASLOT = Cfg::ASLOT, BSLOT = Cfg::BSLOT, NCHUNK = Cfg::NCHUNK;
     constexpr int AR = SC::AR, XPITCH = SC::XPITCH, XSLOT = SC::XSLOT, NSA = SC::NSA, NSX = SC::NSX, MAXSEG = SC::MAXSEG;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *bres = smem, *aring = smem + SC::BRES, *xring = aring + NSA * ASLOT;
-    uint64_t *fullW = reinterpret_cast<uint64_t *>(xring + NSX * XSLOT);
-    uint64_t *fullA = fullW + 1, *emptyA = fullA + NSA, *fullX = emptyA + NSA, *emptyX = fullX + NSX;
+    uint64_t *fullW = reinterpret_cast<uint64_t *>(xring + NSX * XSLOT), *emptyW = fullW + 1;
+    uint64_t *fullA = emptyW + 1, *emptyA = fullA + NSA, *fullX = emptyA + NSA, *emptyX = fullX + NSX;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int Lin = rows.stride;  // input positions between items
+    // Resident B per voice.  set_units keeps every tile within one voice, so tile r0's weights are rows.blob_at(r0).  Load
+    // k of B (k = 0, 1, ...: one per voice change along this CTA's walk, the first before the first tile) completes phase k
+    // of fullW; the MMA warpgroups wait for it (parity k & 1) before the first MMA of a tile of that voice.  B is
+    // overwritten only by the producer's lane 0, and only after emptyW has completed phase k - 1: each MMA warpgroup's
+    // thread 0 arrives there after wgmma_wait<0> of the last tile before the voice change, so every MMA that read the
+    // old B has completed.  The producer has issued the staging loads of every earlier tile by then, so the wait cannot
+    // close a cycle; it only holds back the new voice's staging loads until the old voice's MMAs are done.
+    auto voice = [&](int tile) { return rows.blob_at(tile * ROWS); };
+    auto load_b = [&](const float *vb) {
+        const uint8_t *src = reinterpret_cast<const uint8_t *>(vb) + tc_region_start() + tc_up_offset(Cfg::STAGE);
+        mbar_arrive_expect_tx(fullW, SC::BRES);
+        for (int i = 0; i < NCHUNK; ++i) bulk_g2s(bres + i * BSLOT, src + (size_t)i * BSLOT, BSLOT, fullW);
+    };
 
     if (tid == 0) {
         mbar_init(fullW, 1);
+        mbar_init(emptyW, NMW);
         for (int s = 0; s < NSA; ++s) { mbar_init(&fullA[s], NCONV); mbar_init(&emptyA[s], NMW); }
         for (int s = 0; s < NSX; ++s) { mbar_init(&fullX[s], 1); mbar_init(&emptyX[s], NCONV); }
         fence_mbar_init();
@@ -376,17 +404,23 @@ convt_stream_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const
 
     if (warp == (NCONV + 128 * NMW) / 32) {
         // ================= producer warp: resident B (lane 0), then the input tiles (lane c: channel c of a slot) =========
-        if (lane == 0) {
-            const uint8_t *src = reinterpret_cast<const uint8_t *>(packed) + tc_region_start() + tc_up_offset(Cfg::STAGE);
-            mbar_arrive_expect_tx(fullW, SC::BRES);
-            for (int i = 0; i < NCHUNK; ++i) bulk_g2s(bres + i * BSLOT, src + (size_t)i * BSLOT, BSLOT, fullW);
-        }
+        const float *wb = voice(blockIdx.x);  // the voice whose B is resident (or on its way)
+        int nw = 0;                           // loads of B so far, minus one
+        if (lane == 0) load_b(wb);
         pdl_wait();  // x: the previous kernel's output
         int sx = 0, phx = 0;
         bool ok = true;
 #pragma unroll 1
         for (int tile = blockIdx.x; tile < ntiles && ok; tile += gridDim.x) {
             const int r0 = tile * ROWS;
+            if (voice(tile) != wb) {
+                wb = voice(tile);
+                ok = __shfl_sync(0xffffffffu, lane == 0 ? mbar_wait(emptyW, nw & 1) : false, 0);
+                if (!ok) break;
+                if (lane == 0) load_b(wb);
+                ++nw;
+                __syncwarp();
+            }
             XSeg seg[MAXSEG];
             int covered;
             tile_segments<SC>(rows, r0, seg, covered);
@@ -420,16 +454,27 @@ convt_stream_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const
         const int mw = warp / 4 - NCONV / 128, t = tid & 127;
         const uint64_t adesc_t = desc_template(APITCH, 128), bdesc_t = desc_template(N * 16, 128);
         const uint32_t aring_addr = smem_u32(aring) + mw * 64 * 16, bres_addr = smem_u32(bres);
-        float bj[NG / 8][2];  // bias of this thread's channels 8k + 2q + e
+        float bj[NG / 8][2];  // bias of this thread's channels 8k + 2q + e, of the resident voice
+        auto load_bias = [&](const float *vb) {
 #pragma unroll
-        for (int k = 0; k < NG / 8; ++k)
+            for (int k = 0; k < NG / 8; ++k)
 #pragma unroll
-            for (int e = 0; e < 2; ++e) bj[k][e] = __ldg(packed + bias_offset(1 + Cfg::STAGE) + 8 * k + 2 * (t & 3) + e);
+                for (int e = 0; e < 2; ++e) bj[k][e] = __ldg(vb + bias_offset(1 + Cfg::STAGE) + 8 * k + 2 * (t & 3) + e);
+        };
+        const float *wb = voice(blockIdx.x);
+        int nw = 0;
+        load_bias(wb);
         float acc[N / 2];
         int sa = 0, pha = 0;
         bool ok = mbar_wait(fullW, 0);  // a timed-out wait only raises the status word: control flow stays uniform
 #pragma unroll 1
         for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+            if (voice(tile) != wb) {  // B of this voice: load nw + 1
+                wb = voice(tile);
+                ++nw;
+                load_bias(wb);
+                ok &= mbar_wait(fullW, nw & 1);
+            }
             int psa = -1;
 #pragma unroll 1
             for (int ca = 0; ca < CIN / KCA; ++ca) {
@@ -459,7 +504,9 @@ convt_stream_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const
             wgmma_wait<0>();
             acc_fence<N / 2>(acc);
             if (t == 0) mbar_arrive(&emptyA[psa]);
-            if (tile + (int)gridDim.x >= ntiles) pdl_trigger();  // last tile's MMAs done: the next kernel may be scheduled
+            const int next = tile + (int)gridDim.x;
+            if (t == 0 && next < ntiles && voice(next) != wb) mbar_arrive(emptyW);  // every MMA on this B has completed
+            if (next >= ntiles) pdl_trigger();  // last tile's MMAs done: the next kernel may be scheduled
             pdl_wait();
             convt_stream_store<Cfg>(acc, bj, y, mw, t, tile * ROWS, rows);
         }
@@ -522,7 +569,7 @@ convt_stream_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const
 }
 
 template <class Cfg>
-static int launch_convt_stream(const float *x, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s) {
+static int launch_convt_stream(const float *x, float *y, const RunTable &batch, int *status, cudaStream_t s) {
     using SC = StreamCfg<Cfg>;
     static bool configured = false;
     if (!configured) {
@@ -534,11 +581,10 @@ static int launch_convt_stream(const float *x, float *y, const float *packed, co
     int dev = 0, sms = 0;
     MG_CUDA_TRY(cudaGetDevice(&dev));
     MG_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const RunTable rows = convt_rows(batch);
+    const RunTable rows = convt_rows(batch, Cfg::ROWS);
     const int ntiles = (rows.first[rows.n] + Cfg::ROWS - 1) / Cfg::ROWS;
     const unsigned grid = (unsigned)(ntiles < sms ? ntiles : sms);
-    MG_CUDA_TRY(launch_ex(convt_stream_tc_kernel<Cfg>, dim3(grid), dim3(SC::NT), SC::SMEM_BYTES, s, true, 1, x, y, packed, rows, ntiles,
-                          status));
+    MG_CUDA_TRY(launch_ex(convt_stream_tc_kernel<Cfg>, dim3(grid), dim3(SC::NT), SC::SMEM_BYTES, s, true, 1, x, y, rows, ntiles, status));
     return MG_OK;
 }
 
@@ -559,8 +605,8 @@ static const char *stream_cfg_name() {
 // also parks the tile's 64 row lookups in shared memory for the epilogue, which runs once per channel group.
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NCONV + 128 + 32, 1)
-convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const float *__restrict__ packed,
-                         const __grid_constant__ RunTable rows, int *__restrict__ status) {
+convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, const __grid_constant__ RunTable rows,
+                         int *__restrict__ status) {
     constexpr int CIN = Cfg::CIN, NG = Cfg::NG, N = Cfg::N, NCG = Cfg::NCG;
     constexpr int ROWS = 64, APITCH = Cfg::APITCH, BSLOT = Cfg::BSLOT, NCHUNK = Cfg::NCHUNK;
     constexpr int KPT = CIN / 8;                    // k-panels of the resident A
@@ -589,7 +635,7 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
     if (warp == NCONV / 32 + 4) {
         // ================= TMA producer: B slots of every channel group, in consumption order =================
         if (lane == 0) {
-            const uint8_t *src = reinterpret_cast<const uint8_t *>(packed) + tc_region_start() + tc_up_offset(Cfg::STAGE);
+            const uint8_t *src = reinterpret_cast<const uint8_t *>(tile_blob(rows, r0)) + tc_region_start() + tc_up_offset(Cfg::STAGE);
             int s = 0, ph = 0;
             bool ok = true;
             for (int i = 0; i < NCG * NCHUNK && ok; ++i) {  // blob order is [cg][chunk]: exactly this loop
@@ -635,7 +681,7 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
             if (t == 0) { mbar_arrive(&emptyB[psb]); psb = -1; }
             if (cg == NCG - 1) pdl_trigger();  // last channel group's MMAs done: the next kernel may be scheduled
             if (cg == 0) pdl_wait();
-            convt_store<Cfg>(acc, y, packed + bias_offset(1 + Cfg::STAGE) + cg * NG, 0, t, cg, Cfg::S * Lin,
+            convt_store<Cfg>(acc, y, tile_blob(rows, r0) + bias_offset(1 + Cfg::STAGE) + cg * NG, 0, t, cg, Cfg::S * Lin,
                              [&](int m) { return ok ? srow[m] : RunPos{-1, 0, 0}; });  // (after fullA[0]: srow is complete)
         }
         if (!ok && t == 0) atomicExch(status, 33);
@@ -670,33 +716,32 @@ convt_resident_tc_kernel(const float *__restrict__ x, float *__restrict__ y, con
 }
 
 template <class Cfg>
-static int launch_convt_resident(const float *x, float *y, const float *packed, const RunTable &batch, int *status, cudaStream_t s) {
+static int launch_convt_resident(const float *x, float *y, const RunTable &batch, int *status, cudaStream_t s) {
     constexpr int smem = 2 * (Cfg::CIN / 8) * Cfg::APITCH + 4 * Cfg::BSLOT + (Cfg::CIN / 64 + 2 * 4) * 8 + 64 * sizeof(RunPos);
     static bool configured = false;
     if (!configured) {
         MG_CUDA_TRY(cudaFuncSetAttribute(convt_resident_tc_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         configured = true;
     }
-    const RunTable rows = convt_rows(batch);
+    const RunTable rows = convt_rows(batch, 64);
     MG_CUDA_TRY(launch_ex(convt_resident_tc_kernel<Cfg>, dim3((unsigned)((rows.first[rows.n] + 63) / 64)), dim3(Cfg::NCONV + 128 + 32),
-                          smem, s, true, 1, x, y, packed, rows, status));
+                          smem, s, true, 1, x, y, rows, status));
     return MG_OK;
 }
 
 // x [B][Cin][Lin] -> y [B][Cout][S*Lin], fp32 NCL, (Cin, Cout, S) of generator stage `stage`; Lin = batch.stride, item i's
 // first len_i input positions (and S len_i output positions) are its own.  precision MG_GEN_PRECISION_BF16: stages 0 and 1
 // run their single-pass variants; stages 2 and 3 keep the streaming kernel's three passes (it is bound by memory).
-int launch_convt_tc(const float *x, float *y, const float *packed, int stage, const RunTable &batch, int *status, cudaStream_t s,
-                    int precision) {
+int launch_convt_tc(const float *x, float *y, int stage, const RunTable &batch, int *status, cudaStream_t s, int precision) {
     if (precision != MG_GEN_PRECISION_FP32 && precision != MG_GEN_PRECISION_BF16)
         return set_error(MG_ERR_INVALID_ARGUMENT, "launch_convt_tc: precision %d", precision);
-    if (precision == MG_GEN_PRECISION_BF16 && stage == 0) return launch_convt<Bf16<UpCfg<0>>>(x, y, packed, batch, status, s);
-    if (precision == MG_GEN_PRECISION_BF16 && stage == 1) return launch_convt_resident<Bf16<UpCfg<1>>>(x, y, packed, batch, status, s);
+    if (precision == MG_GEN_PRECISION_BF16 && stage == 0) return launch_convt<Bf16<UpCfg<0>>>(x, y, batch, status, s);
+    if (precision == MG_GEN_PRECISION_BF16 && stage == 1) return launch_convt_resident<Bf16<UpCfg<1>>>(x, y, batch, status, s);
     switch (stage) {
-        case 0: return launch_convt<UpCfg<0>>(x, y, packed, batch, status, s);
-        case 1: return launch_convt_resident<UpCfg<1>>(x, y, packed, batch, status, s);
-        case 2: return launch_convt_stream<UpCfg<2>>(x, y, packed, batch, status, s);
-        case 3: return launch_convt_stream<UpCfg<3>>(x, y, packed, batch, status, s);
+        case 0: return launch_convt<UpCfg<0>>(x, y, batch, status, s);
+        case 1: return launch_convt_resident<UpCfg<1>>(x, y, batch, status, s);
+        case 2: return launch_convt_stream<UpCfg<2>>(x, y, batch, status, s);
+        case 3: return launch_convt_stream<UpCfg<3>>(x, y, batch, status, s);
     }
     return set_error(MG_ERR_INVALID_ARGUMENT, "launch_convt_tc: stage %d", stage);
 }

@@ -60,6 +60,10 @@ def lib():
         L.mg_gen_forward_precision.restype = ctypes.c_int
         L.mg_gen_forward_precision.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                                ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+        L.mg_gen_forward_voices.restype = ctypes.c_int
+        L.mg_gen_forward_voices.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                            ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                            ctypes.c_size_t, ctypes.c_void_p]
         L.mg_gen_forward_timed.restype = ctypes.c_int
         L.mg_gen_forward_timed.argtypes = L.mg_gen_forward.argtypes + [ctypes.POINTER(ctypes.c_float)]
         L.mg_gen_check_status.restype = ctypes.c_int
@@ -220,6 +224,24 @@ def _lengths(lengths, B, T_max):
     if bad:
         raise EngineError("lengths must lie in [1, T_max = %d] (got %d)" % (T_max, bad[0]))
     return (ctypes.c_int * B)(*lengths)
+
+
+def _voice_ids(voice, B, n_voices):
+    """Per-item voice ids of a multi-voice batch as a C int array: a list, a tuple or a CPU integer tensor of B values in
+    [0, n_voices).  A CUDA tensor is refused: reading it would synchronise the stream."""
+    if hasattr(voice, "device") and hasattr(voice, "is_floating_point"):
+        if voice.device.type != "cpu":
+            raise EngineError("voice must be a list, a tuple or a CPU tensor (reading a CUDA tensor would synchronise)")
+        if voice.is_floating_point() or voice.dim() != 1:
+            raise EngineError("voice must be a 1-D integer tensor")
+        voice = voice.tolist()
+    voice = [int(v) for v in voice]
+    if len(voice) != B:
+        raise EngineError("voice has %d entries for a batch of %d" % (len(voice), B))
+    bad = [v for v in voice if not 0 <= v < n_voices]
+    if bad:
+        raise EngineError("voice ids must lie in [0, n_voices = %d) (got %d)" % (n_voices, bad[0]))
+    return (ctypes.c_int * B)(*voice)
 
 
 PRECISIONS = {"fp32": 0, "bf16": 1}  # MG_GEN_PRECISION_FP32 / _BF16, include/melgan_b200.h
@@ -512,6 +534,43 @@ class GeneratorDevice(_PackedBlob):
             else:
                 check(lib().mg_gen_forward_precision(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens, code,
                                                      ws.data_ptr(), ws.numel() * 4, stream))
+            off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4
+            sc.arm(ws.view(torch.int32)[off:off + 1])
+        return out
+
+    def forward_voices(self, voices, mel, voice, lengths=None, out=None, precision="fp32"):
+        """Many voices in one forward (inference): item i of mel [B, 80, T_max] runs on the weights of voices[voice[i]] (a
+        sequence of GeneratorDevice on this device, this one among them or not) -> audio [B, 1, 256 T_max], each item bit
+        for bit its own forward on its own voice (at the same precision; 0 past 256 lengths[i] samples).  voice: B ids in
+        [0, len(voices)), and lengths as in forward_ragged (None: every item T_max frames), each a list, a tuple or a CPU
+        integer tensor.  Items sorted by voice run fastest (contract at mg_gen_forward_voices, include/melgan_b200.h).
+        Uses this module's scratch of the current stream.  Asynchronous, like forward."""
+        torch = self.torch
+        code = _precision(precision)
+        if mel.dim() != 3 or mel.shape[1] != 80:
+            raise EngineError("mel must be [B, 80, T_max], got %s" % (tuple(mel.shape),))
+        if mel.device != self.device or mel.dtype != torch.float32:
+            raise EngineError("mel must be an fp32 tensor on %s" % (self.device,))
+        voices = list(voices)
+        if not voices:
+            raise EngineError("forward_voices needs at least one voice")
+        for v in voices:
+            if not isinstance(v, GeneratorDevice) or v.device != self.device:
+                raise EngineError("every voice must be a GeneratorDevice on %s" % (self.device,))
+        mel = mel.contiguous()
+        B, _, T = mel.shape
+        lens = None if lengths is None else _lengths(lengths, B, T)
+        ids = _voice_ids(voice, B, len(voices))
+        if out is None:
+            out = torch.empty((B, 1, 256 * T), dtype=torch.float32, device=self.device)
+        sc = self._scratch.current()
+        sc.check()
+        ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream().cuda_stream
+            blobs = _ptr_array([v.packed.data_ptr() for v in voices])  # (each read orders this stream after its pack)
+            check(lib().mg_gen_forward_voices(blobs, len(voices), ids, mel.data_ptr(), out.data_ptr(), B,
+                                              T, lens, code, ws.data_ptr(), ws.numel() * 4, stream))
             off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4
             sc.arm(ws.view(torch.int32)[off:off + 1])
         return out

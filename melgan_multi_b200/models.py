@@ -227,6 +227,29 @@ class Generator(nn.Module):
         return _GeneratorFunction.apply(self, x, *flat)
 
 
+def generate_voices(generators, mel, voice, lengths=None, precision="fp32"):
+    """Vocodes a batch that mixes voices in one forward (inference only: no autograd graph is built).  generators: a
+    sequence of Generator modules (a vocoder fine-tuned per speaker, say) on mel's CUDA device, each packed lazily as
+    generate packs it.  mel [B, 80, T_max] fp32; voice: B ids in [0, len(generators)) as a list, a tuple or a CPU integer
+    tensor; lengths as in Generator.generate (None: every item T_max frames).  Item i of the audio [B, 1, 256 T_max] is
+    bit for bit generators[voice[i]].generate(mel[i:i+1, :, :lengths[i]], precision=precision), then 0.  Items need not be
+    sorted by voice, but sorted ones run fastest."""
+    _engine._precision(precision)
+    if not mel.is_cuda:
+        raise _engine.EngineError("melgan_multi_b200.generate_voices needs a CUDA tensor (no CPU fallback)")
+    generators = list(generators)
+    if not generators:
+        raise _engine.EngineError("generate_voices needs at least one generator")
+    with torch.no_grad():
+        devs = []
+        for g in generators:
+            dev = g._ensure_packed()
+            if dev.device != mel.device:
+                raise _engine.EngineError("generate_voices: a generator is on %s, mel on %s" % (dev.device, mel.device))
+            devs.append(dev)
+        return devs[0].forward_voices(devs, mel.detach().float(), voice, lengths, precision=precision)
+
+
 class Discriminator(nn.Module):
     """One discriminator (reference models.py:74-103).  Inside ``MultiScaleDiscriminator`` (its only caller in the
     reference, models.py:109-113) the three of them run as one fused pipeline on the stacked real + generated batch;
