@@ -27,6 +27,7 @@ import threading
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch._utils import _unflatten_dense_tensors
 from torch.nn import AvgPool1d, Conv1d, ConvTranspose1d
 from torch.nn.utils import weight_norm
 
@@ -75,12 +76,30 @@ def _layer_modules(gen):
     return mods
 
 
+def _owned_copies(tensors):
+    """Copies of tensors (None stays None) carved out of one new allocation and filled by one multi-tensor copy."""
+    src = [t for t in tensors if t is not None]
+    if not src:
+        return list(tensors)
+    flat = torch.empty(sum(t.numel() for t in src), dtype=src[0].dtype, device=src[0].device)
+    dst = _unflatten_dense_tensors(flat, src)  # src-shaped views of flat, made in one call (per-tensor views cost the host)
+    torch._foreach_copy_(dst, src)
+    it = iter(dst)
+    return [next(it) if t is not None else None for t in tensors]
+
+
 class _GeneratorFunction(torch.autograd.Function):
     """Forward on the fused sm_90a kernels; backward by recomputation through stock PyTorch ops (open row: native
     backward).  The recomputation -- 30 convs forward, their backward, weight-norm: ~600 launches that cost the host more
     than the GPU -- is captured ONCE per input shape as a pair of CUDA graphs (torch.cuda.make_graphed_callables) and
     replayed, so the step is no longer bound by eager launch overhead (MG_GEN_BWD_GRAPH=0: eager).
-    Inputs: mel, then 30 x (weight_v, weight_g, bias)."""
+    Inputs: mel, then 30 x (weight_v, weight_g, bias).
+
+    The gradients it returns belong to the caller on both paths.  A graphed backward writes them into static buffers of
+    the graph that its next replay overwrites, so they are copied out (one flat allocation, one multi-tensor copy) before
+    they are handed on: .grad accumulation across backward() calls, zero_grad(set_to_none=False), two calls in one loss
+    and a mel.grad kept across later steps all see their own values.  The graph buffers are per module, so one module's
+    backward must not run on two streams at once."""
 
     @staticmethod
     def forward(ctx, gen, mel, *params):
@@ -94,15 +113,18 @@ class _GeneratorFunction(torch.autograd.Function):
         gen = ctx.gen
         mel, *params = ctx.saved_tensors
         need_mel = ctx.needs_input_grad[1]
+        graphed = ctx.graphed is not None and need_mel == ctx.graphed[1]
         with torch.enable_grad():
             mel_ = mel.detach().requires_grad_(need_mel)
             leaves = [p.detach().requires_grad_(True) for p in params]
-            if ctx.graphed is not None and need_mel == ctx.graphed[1]:
+            if graphed:
                 y = ctx.graphed[0](mel_, *leaves)
             else:
                 y = gen._torch_forward(mel_, leaves)
             wanted = ([mel_] if need_mel else []) + leaves
             grads = torch.autograd.grad(y, wanted, grad_out.contiguous(), allow_unused=True)
+        if graphed:
+            grads = _owned_copies(grads)
         grads = list(grads)
         gmel = grads.pop(0) if need_mel else None
         return (None, gmel, *grads)
@@ -175,13 +197,16 @@ class Generator(nn.Module):
         return _engine.GeneratorStream(self._ensure_packed, vs[0].device, max_sessions, max_push_frames, precision)
 
     def _graphed_recompute(self, mel, params):
-        """(graphed stock-op forward+backward, mel_requires_grad) for this input shape, or None.  Cached per shape / dtype
-        policy; the graphs own static copies of nothing but activations -- parameters are call arguments."""
+        """(graphed stock-op forward+backward, mel_requires_grad) for this input shape, or None.  Cached per shape and per
+        setting that picks the recompute's algorithms (cuDNN precision, benchmark and determinism, torch's deterministic
+        mode: a graph replays the algorithms chosen at its capture); the graphs own static copies of nothing but
+        activations and gradients -- parameters are call arguments."""
         import os
         if os.environ.get("MG_GEN_BWD_GRAPH", "1") == "0" or torch.cuda.is_current_stream_capturing():
             return None
         need_mel = bool(mel.requires_grad)
-        key = (tuple(mel.shape), mel.device, need_mel, torch.backends.cudnn.conv.fp32_precision, torch.backends.cudnn.benchmark)
+        key = (tuple(mel.shape), mel.device, need_mel, torch.backends.cudnn.conv.fp32_precision, torch.backends.cudnn.benchmark,
+               torch.backends.cudnn.deterministic, torch.are_deterministic_algorithms_enabled())
         cache = self.__dict__.setdefault("_bwd_graphs", {})
         if key not in cache:
             if len(cache) >= 4:  # shapes keep changing (e.g. whole-utterance validation): stay eager for new ones
