@@ -171,12 +171,30 @@ void mg_gen_stream_destroy(mg_gen_stream *s);
 int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, const int *frames, const int *flags, int n, float *audio,
                        int *out_samples, void *stream);
 int mg_gen_stream_check_status(mg_gen_stream *s, void *stream);
+/* Many voices in one stream step: slot i runs on the weights of packed[voice[i]], in the same launches as one voice.
+ *   packed: HOST array of n_voices >= 1 blobs of mg_gen_pack (16-byte aligned, none NULL; each read anew every step)
+ *   voice:  HOST array of n ids in [0, n_voices) (NULL: every slot uses voice 0)
+ *   everything else as for mg_gen_stream_step (same handle, precision, state and mg_gen_stream_state_bytes).
+ * A slot's voice binds on the step that opens its utterance (its first frames after create, MG_GEN_STREAM_END or
+ * MG_GEN_STREAM_RESET).  While the utterance is open every step must pass the same id for the slot, or set
+ * MG_GEN_STREAM_RESET on it; a slot with no open utterance accepts any id.  n_voices may change between steps as long as
+ * the ids passed stay in range.  The concatenation of a session's outputs is bit-identical to mg_gen_forward_precision of
+ * its whole mel on packed[its voice] at the handle's precision, for any push schedule.  Each kernel's items are planned
+ * by ascending voice, slot order within a voice, so each voice is one run and (as in mg_gen_forward_voices) the conv_pre
+ * and ConvT grids start a new tile at each change of voice.  Refused with MG_ERR_INVALID_ARGUMENT before any CUDA call:
+ * n_voices < 1, a NULL or misaligned blob, an id out of range, a changed id on an open slot without RESET, and
+ * everything mg_gen_stream_step refuses.  mg_gen_stream_step(s, packed, ...) is this call with (&packed, 1, NULL). */
+int mg_gen_stream_step_voices(mg_gen_stream *s, const void *const *packed, int n_voices, const int *voice, const float *mel,
+                              const int *frames, const int *flags, int n, float *audio, int *out_samples, void *stream);
 /* Planning without a device: advances the handle's counters exactly as mg_gen_stream_step would and reports out_samples,
  * the items each of the 8 chain kernels would run (kernel_items[8], may be NULL) and the bytes the window-assembly and
  * audio copies would read and write (copy_bytes, may be NULL).  No CUDA call.  A handle advanced this way refuses later
- * real steps. */
+ * real steps.  mg_gen_stream_dry_step_voices does the same for mg_gen_stream_step_voices (voices bound and refused as
+ * there; no blob is needed); mg_gen_stream_dry_step is its case (1, NULL). */
 int mg_gen_stream_dry_step(mg_gen_stream *s, const int *frames, const int *flags, int n, int *out_samples, int *kernel_items,
                            long long *copy_bytes);
+int mg_gen_stream_dry_step_voices(mg_gen_stream *s, int n_voices, const int *voice, const int *frames, const int *flags, int n,
+                                  int *out_samples, int *kernel_items, long long *copy_bytes);
 
 /* Same as mg_gen_forward, but brackets each of the mg_gen_forward_launches() kernels with CUDA
  * events on `stream`, waits for the last one and returns the per-kernel device times in

@@ -20,6 +20,12 @@
 // positions, and derives every window, offset and count from them: a step never reads the device.  One window-assembly
 // launch per boundary builds the windows of the kernel that follows it in the padded [item][C][stride] layout the kernel
 // reads, and stores each session's next tail; the same kernel copies the newly final audio to the caller.
+//
+// Voices (mg_gen_stream_step_voices): each slot runs on the blob of the voice its utterance was opened with.  The planner
+// walks the sessions by ascending voice, slot order within a voice, so every kernel's items come in voice runs and its
+// RunTable::voices starts a new tile at each change of voice, as in mg_gen_forward_voices.  Tails, mel rows and audio
+// rows stay indexed by slot: only the item numbering follows the walk.  With one voice the walk is slot order.
+#include <algorithm>
 #include <new>
 #include <string.h>
 
@@ -164,8 +170,10 @@ struct Plan {
     AsmTable asm_[kKernels + 1];       // boundary b = 0..7: the windows of kernel b and the tails; [8]: audio to the caller
     long long asm_elems[kKernels + 1];  // the largest job of each launch (floats)
     int items[kKernels], lens[kKernels][MG_GEN_RAGGED_MAX_B], stride[kKernels];
+    int voice[kKernels][MG_GEN_RAGGED_MAX_B];  // each item's voice
     long long F[MG_GEN_RAGGED_MAX_B][9];  // the counters after the step
     unsigned char par[MG_GEN_RAGGED_MAX_B][kKernels];
+    int bound[MG_GEN_RAGGED_MAX_B];  // each slot's voice after the step (-1: no utterance open)
     long long bytes;  // bytes the window-assembly and audio copies read plus write
 };
 
@@ -199,6 +207,7 @@ struct mg_gen_stream {
     StateLayout L;
     long long F[MG_GEN_RAGGED_MAX_B][9];  // per slot: final positions at every boundary (all 0: no utterance open)
     unsigned char par[MG_GEN_RAGGED_MAX_B][kKernels];  // which half of the tail store holds the slot's current tail
+    int voice[MG_GEN_RAGGED_MAX_B];  // per slot: the voice its open utterance is bound to (-1: none open)
     bool status_written, dry;
     Plan plan;
 };
@@ -215,12 +224,23 @@ int check_chain(const char *fn) {
     return MG_OK;
 }
 
-// Argument checks of a step (no CUDA call), then the plan.  On success p holds the launches and the new counters.
-int plan_step(const char *fn, const mg_gen_stream *s, const int *frames, const int *flags, int n, int *out_samples, Plan &p) {
+// Argument checks of a step (no CUDA call), then the plan.  On success p holds the launches, the new counters and the
+// slots' voices.  voice: n ids in [0, n_voices) (NULL: all 0); an open slot keeps its voice unless this step resets it.
+int plan_step(const char *fn, const mg_gen_stream *s, int n_voices, const int *voice, const int *frames, const int *flags, int n,
+              int *out_samples, Plan &p) {
     if (!s || !frames || !out_samples) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
     if (n < 0 || n > s->S) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n = %d is outside [0, max_sessions = %d]", fn, n, s->S);
+    if (n_voices < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, n_voices);
     for (int i = 0; i < n; ++i) {
         const int fl = flags ? flags[i] : 0;
+        const int v = voice ? voice[i] : 0;
+        if (v < 0 || v >= n_voices)
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: voice[%d] = %d is outside [0, n_voices = %d)", fn, i, v, n_voices);
+        if (!(fl & MG_GEN_STREAM_RESET) && s->F[i][0] > 0 && v != s->voice[i])
+            return set_error(MG_ERR_INVALID_ARGUMENT,
+                             "%s: voice[%d] = %d, but slot %d's open utterance is bound to voice %d (a slot changes voice only "
+                             "with MG_GEN_STREAM_RESET or after MG_GEN_STREAM_END)",
+                             fn, i, v, i, s->voice[i]);
         if (frames[i] < 0 || frames[i] > s->P)
             return set_error(MG_ERR_INVALID_ARGUMENT, "%s: frames[%d] = %d is outside [0, max_push_frames = %d]", fn, i, frames[i], s->P);
         if (fl & ~(MG_GEN_STREAM_END | MG_GEN_STREAM_RESET))
@@ -235,8 +255,14 @@ int plan_step(const char *fn, const mg_gen_stream *s, const int *frames, const i
     for (int k = 0; k < kKernels; ++k) { p.items[k] = 0; p.stride[k] = 0; }
     memcpy(p.F, s->F, sizeof(p.F));
     memcpy(p.par, s->par, sizeof(p.par));
-    for (int i = 0; i < n; ++i) {
-        const int fl = flags ? flags[i] : 0;
+    memcpy(p.bound, s->voice, sizeof(p.bound));
+    // the walk: by ascending voice, slot order within a voice (stable), so each kernel's items come in voice runs
+    int order[MG_GEN_RAGGED_MAX_B];
+    for (int i = 0; i < n; ++i) order[i] = i;
+    if (voice) std::stable_sort(order, order + n, [voice](int a, int b) { return voice[a] < voice[b]; });
+    for (int q = 0; q < n; ++q) {
+        const int i = order[q];
+        const int fl = flags ? flags[i] : 0, v = voice ? voice[i] : 0;
         const bool end = fl & MG_GEN_STREAM_END;
         long long F[9], Fn[9];
         for (int b = 0; b <= kKernels; ++b) F[b] = (fl & MG_GEN_STREAM_RESET) ? 0 : s->F[i][b];
@@ -267,6 +293,7 @@ int plan_step(const char *fn, const mg_gen_stream *s, const int *frames, const i
                 if (runs) {
                     item = p.items[k]++;
                     p.lens[k][item] = len;
+                    p.voice[k][item] = v;
                     if (len > p.stride[k]) p.stride[k] = len;
                 }
                 j.dst_item = item;
@@ -286,6 +313,7 @@ int plan_step(const char *fn, const mg_gen_stream *s, const int *frames, const i
             p.bytes += 8ll * out_samples[i];
         }
         for (int b = 0; b <= kKernels; ++b) p.F[i][b] = end ? 0 : Fn[b];
+        p.bound[i] = p.F[i][0] > 0 ? v : -1;  // bound by the step that opens the utterance, free once it ends
     }
     for (int k = 0; k < kKernels; ++k) p.stride[k] = round16(p.stride[k]);
     return MG_OK;
@@ -330,25 +358,34 @@ int mg_gen_stream_create(mg_gen_stream **out, int max_sessions, int max_push_fra
     s->state = (char *)state;
     s->state_bytes = state_bytes;
     s->L = state_layout(max_sessions, max_push_frames);
+    for (int i = 0; i < MG_GEN_RAGGED_MAX_B; ++i) s->voice[i] = -1;
     *out = s;
     return MG_OK;
 }
 
 void mg_gen_stream_destroy(mg_gen_stream *s) { delete s; }
 
-int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, const int *frames, const int *flags, int n, float *audio,
-                       int *out_samples, void *stream) {
-    const char *fn = "mg_gen_stream_step";
+}  // extern "C"
+
+namespace {
+
+// mg_gen_stream_step_voices, and mg_gen_stream_step as its one-voice case (&packed, 1, NULL)
+int step_voices(const char *fn, mg_gen_stream *s, const void *const *packed, int n_voices, const int *voice, const float *mel,
+                const int *frames, const int *flags, int n, float *audio, int *out_samples, void *stream) {
     if (!s || !packed || !audio) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
     if (s->dry) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: this handle was advanced by mg_gen_stream_dry_step", fn);
-    if ((uintptr_t)packed % 16) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed must be 16-byte aligned", fn);
+    if (n_voices < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, n_voices);
+    for (int v = 0; v < n_voices; ++v) {
+        if (!packed[v]) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] is NULL", fn, v);
+        if ((uintptr_t)packed[v] % 16) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] must be 16-byte aligned", fn, v);
+    }
     int rc = check_chain(fn);
     if (rc) return rc;
     bool any = false;
     for (int i = 0; frames && i < n && i < s->S; ++i) any |= frames[i] > 0;
     if (any && !mel) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null mel with frames to push", fn);
     Plan &p = s->plan;
-    if ((rc = plan_step(fn, s, frames, flags, n, out_samples, p))) return rc;
+    if ((rc = plan_step(fn, s, n_voices, voice, frames, flags, n, out_samples, p))) return rc;
 
     cudaStream_t st = (cudaStream_t)stream;
     const StateLayout &L = s->L;
@@ -358,7 +395,7 @@ int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, c
         MG_CUDA_TRY(cudaMemsetAsync(status, 0, sizeof(int), st));
         s->status_written = true;
     }
-    const float *w = (const float *)packed;
+    const float *const *blobs = reinterpret_cast<const float *const *>(packed);
     const float *prev = nullptr;  // the previous kernel's output windows
     long long prev_item = 0;
     int prev_row = 0;
@@ -384,8 +421,8 @@ int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, c
         c.dst_row = stride;
         if ((rc = launch_window(c, p.asm_[k], p.asm_elems[k], st))) return rc;
         if (p.items[k] == 0) continue;  // (no later kernel has items either: nothing was made final here)
-        if ((rc = launch_chain_kernel(k, win, out, RunTable::ragged(p.lens[k], p.items[k], stride, w), status, st, s->precision)))
-            return rc;
+        const RunTable t = RunTable::voices(p.lens[k], p.items[k], stride, blobs, p.voice[k]);
+        if ((rc = launch_chain_kernel(k, win, out, t, status, st, s->precision))) return rc;
         prev = out;
         prev_row = kRatio[k] * stride;
         prev_item = (long long)kC[k + 1] * prev_row;
@@ -400,20 +437,48 @@ int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, c
     if ((rc = launch_window(c, p.asm_[kKernels], p.asm_elems[kKernels], st))) return rc;
     memcpy(s->F, p.F, sizeof(p.F));
     memcpy(s->par, p.par, sizeof(p.par));
+    memcpy(s->voice, p.bound, sizeof(p.bound));
     return MG_OK;
 }
 
-int mg_gen_stream_dry_step(mg_gen_stream *s, const int *frames, const int *flags, int n, int *out_samples, int *kernel_items,
-                           long long *copy_bytes) {
-    if (!s) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_stream_dry_step: null argument");
-    int rc = plan_step("mg_gen_stream_dry_step", s, frames, flags, n, out_samples, s->plan);
+int dry_step_voices(const char *fn, mg_gen_stream *s, int n_voices, const int *voice, const int *frames, const int *flags, int n,
+                    int *out_samples, int *kernel_items, long long *copy_bytes) {
+    if (!s) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
+    int rc = plan_step(fn, s, n_voices, voice, frames, flags, n, out_samples, s->plan);
     if (rc) return rc;
     s->dry = true;
     for (int k = 0; kernel_items && k < kKernels; ++k) kernel_items[k] = s->plan.items[k];
     if (copy_bytes) *copy_bytes = s->plan.bytes;
     memcpy(s->F, s->plan.F, sizeof(s->F));
     memcpy(s->par, s->plan.par, sizeof(s->par));
+    memcpy(s->voice, s->plan.bound, sizeof(s->voice));
     return MG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mg_gen_stream_step_voices(mg_gen_stream *s, const void *const *packed, int n_voices, const int *voice, const float *mel,
+                              const int *frames, const int *flags, int n, float *audio, int *out_samples, void *stream) {
+    return step_voices("mg_gen_stream_step_voices", s, packed, n_voices, voice, mel, frames, flags, n, audio, out_samples, stream);
+}
+
+int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, const int *frames, const int *flags, int n, float *audio,
+                       int *out_samples, void *stream) {
+    if (!packed) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_stream_step: null argument");
+    return step_voices("mg_gen_stream_step", s, &packed, 1, nullptr, mel, frames, flags, n, audio, out_samples, stream);
+}
+
+int mg_gen_stream_dry_step_voices(mg_gen_stream *s, int n_voices, const int *voice, const int *frames, const int *flags, int n,
+                                  int *out_samples, int *kernel_items, long long *copy_bytes) {
+    return dry_step_voices("mg_gen_stream_dry_step_voices", s, n_voices, voice, frames, flags, n, out_samples, kernel_items,
+                           copy_bytes);
+}
+
+int mg_gen_stream_dry_step(mg_gen_stream *s, const int *frames, const int *flags, int n, int *out_samples, int *kernel_items,
+                           long long *copy_bytes) {
+    return dry_step_voices("mg_gen_stream_dry_step", s, 1, nullptr, frames, flags, n, out_samples, kernel_items, copy_bytes);
 }
 
 int mg_gen_stream_check_status(mg_gen_stream *s, void *stream) {

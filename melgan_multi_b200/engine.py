@@ -195,6 +195,12 @@ def lib():
         L.mg_gen_stream_check_status.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
         L.mg_gen_stream_dry_step.restype = ctypes.c_int
         L.mg_gen_stream_dry_step.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int] + [ctypes.c_void_p] * 3
+        L.mg_gen_stream_step_voices.restype = ctypes.c_int
+        L.mg_gen_stream_step_voices.argtypes = ([ctypes.c_void_p] * 2 + [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int]
+                                                + [ctypes.c_void_p] * 3)
+        L.mg_gen_stream_dry_step_voices.restype = ctypes.c_int
+        L.mg_gen_stream_dry_step_voices.argtypes = ([ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int]
+                                                    + [ctypes.c_void_p] * 3)
         _lib = L
     return _lib
 
@@ -747,8 +753,10 @@ class GeneratorStream:
     concatenation equals Generator.generate of the whole mel bit for bit.
 
     packed_fn: a callable returning the GeneratorDevice whose packed weights a step reads (Generator._ensure_packed, so
-    weights changed between steps are re-packed).  state: optional caller-provided uint8 CUDA tensor of at least
-    mg_gen_stream_state_bytes bytes (the stream never lets a byte it has not written reach an output).
+    weights changed between steps are re-packed), or a list of them, one per voice (models.stream_voices): slot i then
+    runs on the weights of voice[i] (mg_gen_stream_step_voices; an open utterance keeps the voice it was opened with until
+    it ends or is reset).  state: optional caller-provided uint8 CUDA tensor of at least mg_gen_stream_state_bytes bytes
+    (the stream never lets a byte it has not written reach an output).
 
     One thread drives a handle at a time, and all steps of one handle must be enqueued on one CUDA stream (or otherwise
     ordered), as for mg_gen_stream_step: the state and the mel staging buffer that ``step`` copies each chunk into are
@@ -782,12 +790,18 @@ class GeneratorStream:
                                          state.numel() * state.element_size()))
         self._mel = torch.zeros((self.max_sessions, 80, self.max_push_frames), dtype=torch.float32, device=self.device)
 
-    def step_packed(self, mel, frames, flags=None, audio=None):
+    def step_packed(self, mel, frames, flags=None, audio=None, voice=None):
         """The C step on a packed buffer: mel [n, 80, max_push_frames] fp32 CUDA (slot i's frames first), frames / flags: n
-        ints.  Returns (audio [n, max_out], per-slot sample counts as a list of ints)."""
+        ints, voice: None (every slot on the first voice) or n voice ids as for ``step``.  Returns (audio [n, max_out],
+        per-slot sample counts as a list of ints)."""
         torch = self.torch
         n = len(frames)
-        dev = self._packed_fn()
+        devs = self._packed_fn()
+        devs = list(devs) if isinstance(devs, (list, tuple)) else [devs]
+        for d in devs:
+            if d.device != self.device:
+                raise EngineError("stream: a voice's weights are on %s, the stream on %s" % (d.device, self.device))
+        ids = None if voice is None else _voice_ids(voice, n, len(devs))
         if audio is None:
             audio = torch.empty((n, self.max_out), dtype=torch.float32, device=self.device)
         fr = (ctypes.c_int * max(n, 1))(*[int(v) for v in frames])
@@ -795,15 +809,18 @@ class GeneratorStream:
         cnt = (ctypes.c_int * max(n, 1))()
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            check(lib().mg_gen_stream_step(self._h, dev.packed.data_ptr(), mel.data_ptr() if mel is not None else None, fr, fl, n,
-                                           audio.data_ptr(), cnt, stream))
+            blobs = _ptr_array([d.packed.data_ptr() for d in devs])  # (each read orders this stream after its pack)
+            check(lib().mg_gen_stream_step_voices(self._h, blobs, len(devs), ids, mel.data_ptr() if mel is not None else None,
+                                                  fr, fl, n, audio.data_ptr(), cnt, stream))
         return audio, [cnt[i] for i in range(n)]
 
-    def step(self, chunks, end=None, reset=None):
+    def step(self, chunks, end=None, reset=None, voice=None):
         """chunks: one entry per slot 0 .. n-1, each a [80, n_i] fp32 CUDA tensor (0 <= n_i <= max_push_frames) or None;
         end / reset: None or n booleans (end: the utterance ends after this chunk; reset: drop the slot's unfinished
-        utterance first).  Returns n [1, m_i] CUDA tensors of newly final audio, owned by the caller.  Asynchronous on the
-        current stream: the lengths are known on return, the values once the stream gets there."""
+        utterance first); voice: None (every slot on the first voice) or n voice ids (a list, a tuple or a CPU integer
+        tensor) -- a slot's id may change only on a step that resets it or once its utterance has ended.  Returns n [1, m_i]
+        CUDA tensors of newly final audio, owned by the caller.  Asynchronous on the current stream: the lengths are known on
+        return, the values once the stream gets there."""
         n = len(chunks)
         if n > self.max_sessions:
             raise EngineError("stream: %d chunks for %d sessions" % (n, self.max_sessions))
@@ -821,7 +838,7 @@ class GeneratorStream:
                 self._mel[i, :, :c.shape[1]].copy_(c)
         flags = [(STREAM_END if end is not None and end[i] else 0) | (STREAM_RESET if reset is not None and reset[i] else 0)
                  for i in range(n)]
-        audio, counts = self.step_packed(self._mel, frames, flags)
+        audio, counts = self.step_packed(self._mel, frames, flags, voice=voice)
         return [audio[i:i + 1, :m] for i, m in enumerate(counts)]
 
     def check_status(self):

@@ -275,6 +275,32 @@ def generate_voices(generators, mel, voice, lengths=None, precision="fp32"):
         return devs[0].forward_voices(devs, mel.detach().float(), voice, lengths, precision=precision)
 
 
+def stream_voices(generators, max_sessions=1, max_push_frames=32, precision="fp32"):
+    """A streaming vocoder whose live sessions run on several voices in one step (inference only): generators is a
+    sequence of Generator modules on one CUDA device, each re-packed lazily at every step as Generator.stream does.  The
+    returned engine.GeneratorStream's step(chunks, end=None, reset=None, voice=None) takes one voice id per slot (None:
+    every slot on generators[0]); a slot keeps the voice its utterance was opened with until the utterance ends or the
+    slot is reset.  The concatenation of a session's outputs equals generators[v].generate() of its whole mel bit for bit."""
+    _engine._precision(precision)
+    generators = list(generators)
+    if not generators:
+        raise _engine.EngineError("stream_voices needs at least one generator")
+    devices = set()
+    for g in generators:
+        vs, _, _ = g._param_triplets()
+        if vs[0].device.type != "cuda":
+            raise _engine.EngineError("melgan_multi_b200.stream_voices needs every generator on CUDA (no CPU fallback)")
+        devices.add(vs[0].device)
+    if len(devices) > 1:
+        raise _engine.EngineError("stream_voices: the generators are on %s; they must share one device"
+                                  % ", ".join(sorted(map(str, devices))))
+
+    def packed():
+        return [g._ensure_packed() for g in generators]
+    packed()
+    return _engine.GeneratorStream(packed, devices.pop(), max_sessions, max_push_frames, precision)
+
+
 class Discriminator(nn.Module):
     """One discriminator (reference models.py:74-103).  Inside ``MultiScaleDiscriminator`` (its only caller in the
     reference, models.py:109-113) the three of them run as one fused pipeline on the stacked real + generated batch;
