@@ -132,6 +132,25 @@ int mg_gen_forward_precision(const void *packed, const float *mel, float *audio,
 int mg_gen_forward_voices(const void *const *packed, int n_voices, const int *voice, const float *mel, float *audio, int B,
                           int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream);
 
+/* 16-bit PCM audio straight from the last kernel: int16 samples instead of fp32, for servers that send WAV / raw LPCM.
+ * For the fp32 audio a that the matching float call returns at the same precision, every sample is
+ *     pcm16(a) = 0                                      if a is NaN
+ *              = clamp(rint(32768 a), -32768, 32767)    otherwise (rint rounds half to even)
+ * 32768 (the reference's MAX_WAV_VALUE) times a is exact in fp32, so pcm16 depends on the fp32 sample alone; tanh returns
+ * exactly +-1.0 for large arguments, so full scale saturates to 32767 / -32768 instead of wrapping.  The int16 audio is
+ * bit-identical to pcm16 of the float call's audio on every path below, at both precisions, and 0 past 256 L_i samples.
+ *
+ * mg_gen_forward_pcm16: one entry point for uniform, ragged, precision and voices forwards.  audio [B][1][256 T_max] int16
+ * device memory; everything else as for mg_gen_forward_voices, except that voice may be NULL (every item on packed[0]).
+ * The matching float call is mg_gen_forward_voices when voice is given, else mg_gen_forward_precision on packed[0] (same
+ * lengths, same limits: a ragged batch then has at most MG_GEN_RAGGED_MAX_B items).  Workspace, batch slices,
+ * mg_gen_check_status and mg_gen_stage_output work as after mg_gen_forward_voices.  Refused with MG_ERR_INVALID_ARGUMENT
+ * (MG_ERR_WORKSPACE_TOO_SMALL for a short workspace) before any CUDA call: everything the matching float call refuses,
+ * n_voices < 1 or a NULL or misaligned blob among packed[0 .. n_voices), and any chain other than the default one
+ * (mg_gen_set_pipeline, MG_GEN_TAIL, MG_GEN_FUSE_UP) at either precision.  Asynchronous on `stream`, no allocation. */
+int mg_gen_forward_pcm16(const void *const *packed, int n_voices, const int *voice, const float *mel, int16_t *audio, int B,
+                         int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream);
+
 /* Streaming vocoder: many live sessions, mel frames pushed a few at a time, each audio sample emitted once it is final.
  * A handle serves up to max_sessions (<= MG_GEN_RAGGED_MAX_B) slots at one precision.  Each mg_gen_stream_step gives slot i
  * (i < n) a push of frames[i] in [0, max_push_frames] new mel frames and flags[i] (flags NULL: all 0):
@@ -186,6 +205,13 @@ int mg_gen_stream_check_status(mg_gen_stream *s, void *stream);
  * everything mg_gen_stream_step refuses.  mg_gen_stream_step(s, packed, ...) is this call with (&packed, 1, NULL). */
 int mg_gen_stream_step_voices(mg_gen_stream *s, const void *const *packed, int n_voices, const int *voice, const float *mel,
                               const int *frames, const int *flags, int n, float *audio, int *out_samples, void *stream);
+/* mg_gen_stream_step_voices with int16 audio [n][mg_gen_stream_max_out(max_push_frames)]: slot i's newly final samples are
+ * pcm16 (see mg_gen_forward_pcm16) of what the float step would write, so an utterance's concatenated output is pcm16 of
+ * mg_gen_forward_precision of its whole mel.  The format is chosen per step: float and int16 steps may alternate on one
+ * handle, which does not change (same state, same mg_gen_stream_state_bytes).  Refused as mg_gen_stream_step_voices;
+ * mg_gen_stream_dry_step* and their copy_bytes describe the float step. */
+int mg_gen_stream_step_pcm16(mg_gen_stream *s, const void *const *packed, int n_voices, const int *voice, const float *mel,
+                             const int *frames, const int *flags, int n, int16_t *audio, int *out_samples, void *stream);
 /* Planning without a device: advances the handle's counters exactly as mg_gen_stream_step would and reports out_samples,
  * the items each of the 8 chain kernels would run (kernel_items[8], may be NULL) and the bytes the window-assembly and
  * audio copies would read and write (copy_bytes, may be NULL).  No CUDA call.  A handle advanced this way refuses later
@@ -374,6 +400,12 @@ int mg_gen_engine_forward_ragged(mg_gen_engine *e, const float *mel_host, float 
  * mg_gen_forward_precision). */
 int mg_gen_engine_forward_precision(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max,
                                     const int *lengths, int precision);
+/* mg_gen_engine_forward_precision with int16 audio_host [B][1][256 T_max]: pcm16 of its audio (contract at
+ * mg_gen_forward_pcm16).  The int16 samples are staged in pinned memory and downloaded per batch slice, half the bytes of
+ * the float call.  Refused with MG_ERR_INVALID_ARGUMENT before any CUDA call: everything the float call refuses, and any
+ * chain other than the default one. */
+int mg_gen_engine_forward_pcm16(mg_gen_engine *e, const float *mel_host, int16_t *audio_host, int B, int T_max,
+                                const int *lengths, int precision);
 /* Device time of the last forward in milliseconds (CUDA events on the engine's stream around the sliced
  * upload -> kernels -> download sequence). */
 int mg_gen_engine_last_kernel_ms(mg_gen_engine *e, float *ms);

@@ -15,13 +15,13 @@ static int *status_ptr(void *workspace, int B, int T) {
 }
 
 // batch: mel lengths (stride T); mel_host / audio_host: optional pinned host buffers (the engine entry point); the copies
-// ride on the batch slices' streams
-static int run_generator(const float *mel, float *audio, const RunTable &batch, float *ws, cudaStream_t s,
-                         cudaEvent_t *ev, const float *mel_host = nullptr, float *audio_host = nullptr,
-                         int precision = MG_GEN_PRECISION_FP32) {
+// ride on the batch slices' streams; pcm16: audio and audio_host hold int16 samples
+static int run_generator(const float *mel, void *audio, const RunTable &batch, float *ws, cudaStream_t s,
+                         cudaEvent_t *ev, const float *mel_host = nullptr, void *audio_host = nullptr,
+                         int precision = MG_GEN_PRECISION_FP32, bool pcm16 = false) {
     int *st = status_ptr(ws, batch.items(), batch.stride);
     MG_CUDA_TRY(cudaMemsetAsync(st, 0, sizeof(int), s));
-    return launch_generator_tc(mel, audio, batch, ws, st, s, ev, mel_host, audio_host, precision);
+    return launch_generator_tc(mel, audio, batch, ws, st, s, ev, mel_host, audio_host, precision, pcm16);
 }
 
 // a known precision, and bf16 only on the default chain (the only one with single-pass kernels)
@@ -108,7 +108,7 @@ size_t mg_gen_workspace_bytes(int B, int T) {
     return ws_offset(6, (size_t)B, (size_t)T) * sizeof(float) + 256;  // + pipeline status word
 }
 
-static int check_forward(const char *fn, const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
+static int check_forward(const char *fn, const void *packed, const float *mel, const void *audio, int B, int T, void *workspace,
                          size_t workspace_bytes) {
     if (!packed || !mel || !audio || !workspace) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
     if (workspace_bytes < mg_gen_workspace_bytes(B, T))
@@ -148,16 +148,22 @@ int mg_gen_forward_precision(const void *packed, const float *mel, float *audio,
                          (float *)workspace, (cudaStream_t)stream, nullptr, nullptr, nullptr, precision);
 }
 
-int mg_gen_forward_voices(const void *const *packed, int n_voices, const int *voice, const float *mel, float *audio, int B,
-                          int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream) {
-    const char *fn = "mg_gen_forward_voices";
-    int rc = check_precision(fn, precision);
-    if (rc) return rc;
+static int check_default_chain(const char *fn) {
     if (!generator_tc_default_chain())
         return set_error(MG_ERR_INVALID_ARGUMENT,
                          "%s: runs the default chain only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected another "
                          "(tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
                          fn, generator_tc_tail(), generator_tc_fused_up());
+    return MG_OK;
+}
+
+// mg_gen_forward_voices' checks (no CUDA call), then its batch table in t
+static int check_voices(const char *fn, const void *const *packed, int n_voices, const int *voice, const float *mel,
+                        const void *audio, int B, int T_max, const int *lengths, int precision, void *workspace,
+                        size_t workspace_bytes, RunTable &t) {
+    int rc = check_precision(fn, precision);
+    if (!rc) rc = check_default_chain(fn);
+    if (rc) return rc;
     if (n_voices < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, n_voices);
     if (!packed || !voice) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null packed or voice array", fn);
     for (int v = 0; v < n_voices; ++v) {
@@ -179,8 +185,44 @@ int mg_gen_forward_voices(const void *const *packed, int n_voices, const int *vo
         return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %d runs of equal length and voice exceed MG_GEN_RAGGED_MAX_B = %d", fn, runs,
                          MG_GEN_RAGGED_MAX_B);
     if ((rc = check_forward(fn, packed[0], mel, audio, B, T_max, workspace, workspace_bytes))) return rc;
-    return run_generator(mel, audio, RunTable::voices(lengths, B, T_max, blobs, voice), (float *)workspace, (cudaStream_t)stream,
-                         nullptr, nullptr, nullptr, precision);
+    t = RunTable::voices(lengths, B, T_max, blobs, voice);
+    return MG_OK;
+}
+
+int mg_gen_forward_voices(const void *const *packed, int n_voices, const int *voice, const float *mel, float *audio, int B,
+                          int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream) {
+    RunTable t;
+    int rc = check_voices("mg_gen_forward_voices", packed, n_voices, voice, mel, audio, B, T_max, lengths, precision, workspace,
+                          workspace_bytes, t);
+    if (rc) return rc;
+    return run_generator(mel, audio, t, (float *)workspace, (cudaStream_t)stream, nullptr, nullptr, nullptr, precision);
+}
+
+int mg_gen_forward_pcm16(const void *const *packed, int n_voices, const int *voice, const float *mel, int16_t *audio, int B,
+                         int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream) {
+    const char *fn = "mg_gen_forward_pcm16";
+    RunTable t;
+    int rc;
+    if (voice) {  // mg_gen_forward_voices' rules
+        rc = check_voices(fn, packed, n_voices, voice, mel, audio, B, T_max, lengths, precision, workspace, workspace_bytes, t);
+    } else {  // every item on voice 0: mg_gen_forward_precision's rules, on the default chain
+        rc = check_precision(fn, precision);
+        if (!rc) rc = check_default_chain(fn);
+        if (!rc && n_voices < 1) rc = set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, n_voices);
+        if (!rc && !packed) rc = set_error(MG_ERR_INVALID_ARGUMENT, "%s: null packed array", fn);
+        for (int v = 0; !rc && v < n_voices; ++v) {
+            if (!packed[v]) rc = set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] is NULL", fn, v);
+            else if ((uintptr_t)packed[v] % 16) rc = set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] must be 16-byte aligned", fn, v);
+        }
+        if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
+        if (!rc) rc = check_forward(fn, packed[0], mel, audio, B, T_max, workspace, workspace_bytes);
+        if (!rc) {
+            const float *w = (const float *)packed[0];
+            t = lengths ? RunTable::ragged(lengths, B, T_max, w) : RunTable::uniform(B, T_max, w);
+        }
+    }
+    if (rc) return rc;
+    return run_generator(mel, audio, t, (float *)workspace, (cudaStream_t)stream, nullptr, nullptr, nullptr, precision, true);
 }
 
 int mg_gen_forward_timed(const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
@@ -624,7 +666,7 @@ struct mg_gen_engine {
     float *packed = nullptr;
     float *raw = nullptr;  // device staging for raw v/g/bias
     float *mel = nullptr, *audio = nullptr, *ws = nullptr;
-    float *pin_in = nullptr, *pin_out = nullptr;
+    float *pin_in = nullptr, *pin_out = nullptr;  // (audio and pin_out hold int16 samples after a pcm16 forward)
     int *pin_status = nullptr;
     size_t cap_frames = 0;  // B*T capacity
     bool loaded = false;
@@ -684,19 +726,21 @@ int mg_gen_engine_load_state(mg_gen_engine *e, const float *const *v, const floa
     return MG_OK;
 }
 
-static int engine_check(const char *fn, mg_gen_engine *e, const float *mel_host, float *audio_host) {
+static int engine_check(const char *fn, mg_gen_engine *e, const float *mel_host, const void *audio_host) {
     if (!e || !mel_host || !audio_host) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
     if (!e->loaded) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: no weights loaded", fn);
     return MG_OK;
 }
 
-static int engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, const RunTable &batch,
-                          int precision = MG_GEN_PRECISION_FP32) {
+// pcm16: audio_host receives int16 samples; the device audio and the pinned staging are then read as int16, so the
+// download moves half the bytes
+static int engine_forward(mg_gen_engine *e, const float *mel_host, void *audio_host, const RunTable &batch,
+                          int precision = MG_GEN_PRECISION_FP32, bool pcm16 = false) {
     const int B = batch.items(), T = batch.stride;
     const size_t frames = (size_t)B * T;
     int rc = engine_reserve(e, frames);
     if (rc) return rc;
-    const size_t nin = frames * kMelBins * sizeof(float), nout = frames * 256 * sizeof(float);
+    const size_t nin = frames * kMelBins * sizeof(float), nout = frames * 256 * (pcm16 ? sizeof(int16_t) : sizeof(float));
     cudaPointerAttributes at;
     const bool in_pinned = cudaPointerGetAttributes(&at, mel_host) == cudaSuccess && at.type == cudaMemoryTypeHost;
     const bool out_pinned = cudaPointerGetAttributes(&at, audio_host) == cudaSuccess && at.type == cudaMemoryTypeHost;
@@ -706,8 +750,8 @@ static int engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_
     if (!e->pin_status) MG_CUDA_TRY(cudaMallocHost(&e->pin_status, sizeof(int)));
     MG_CUDA_TRY(cudaEventRecord(e->ev0, e->stream));
     // upload, kernels and download are enqueued per batch slice (launch_generator_tc); one synchronisation at the end
-    rc = run_generator(e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : e->pin_out,
-                       precision);
+    rc = run_generator(e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : (void *)e->pin_out,
+                       precision, pcm16);
     if (rc) return rc;
     MG_CUDA_TRY(cudaEventRecord(e->ev1, e->stream));
     *e->pin_status = 0;
@@ -742,6 +786,19 @@ int mg_gen_engine_forward_precision(mg_gen_engine *e, const float *mel_host, flo
     return engine_forward(e, mel_host, audio_host, lengths ? RunTable::ragged(lengths, B, T_max, e->packed)
                                                          : RunTable::uniform(B, T_max, e->packed),
                           precision);
+}
+
+int mg_gen_engine_forward_pcm16(mg_gen_engine *e, const float *mel_host, int16_t *audio_host, int B, int T_max, const int *lengths,
+                                int precision) {
+    const char *fn = "mg_gen_engine_forward_pcm16";
+    int rc = check_precision(fn, precision);
+    if (!rc) rc = check_default_chain(fn);
+    if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
+    if (!rc) rc = engine_check(fn, e, mel_host, audio_host);
+    if (rc) return rc;
+    return engine_forward(e, mel_host, audio_host, lengths ? RunTable::ragged(lengths, B, T_max, e->packed)
+                                                         : RunTable::uniform(B, T_max, e->packed),
+                          precision, true);
 }
 
 int mg_gen_engine_last_kernel_ms(mg_gen_engine *e, float *ms) {

@@ -27,6 +27,21 @@ int set_error(int code, const char *fmt, ...);
 
 __device__ __forceinline__ float lrelu(float x) { return fmaxf(x, x * kSlope); }
 
+// 16-bit PCM of an audio sample (mg_gen_forward_pcm16, include/melgan_b200.h): 0 for NaN, else
+// clamp(rint(32768 a), -32768, 32767) with rint rounding half to even.  32768 a is exact in fp32, so the result depends on
+// the fp32 sample alone; tanh can return exactly +-1.0f, which is why the clamp is needed on the positive side.
+__device__ __forceinline__ int16_t pcm16(float a) {
+    const float s = fminf(fmaxf(rintf(32768.f * a), -32768.f), 32767.f);
+    return a != a ? (int16_t)0 : (int16_t)__float2int_rz(s);
+}
+// the sample type an audio store writes: the fp32 sample itself, or its pcm16
+template <class T>
+__device__ __forceinline__ T audio_sample(float a);
+template <>
+__device__ __forceinline__ float audio_sample<float>(float a) { return a; }
+template <>
+__device__ __forceinline__ int16_t audio_sample<int16_t>(float a) { return pcm16(a); }
+
 __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gmem_src) {
     uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(gmem_src));
@@ -195,9 +210,10 @@ const char *generator_tc_kernel_config(int i, int T);
 const char *resblock_config_name(int stage, int L);
 int generator_tc_slices(int B, long long frames);  // batch slices (concurrent kernel chains) one forward is cut into
 // batch: the items' mel lengths, stride T_max (the layout of mel, audio and every workspace buffer), each run's weights
-int launch_generator_tc(const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
-                        cudaStream_t s, cudaEvent_t *ev = nullptr, const float *mel_host = nullptr, float *audio_host = nullptr,
-                        int precision = MG_GEN_PRECISION_FP32);
+// pcm16: audio (and audio_host) hold int16 samples, pcm16 of the fp32 audio, written by the last kernel (default chain only)
+int launch_generator_tc(const float *mel, void *audio, const RunTable &batch, float *ws, int *status,
+                        cudaStream_t s, cudaEvent_t *ev = nullptr, const float *mel_host = nullptr, void *audio_host = nullptr,
+                        int precision = MG_GEN_PRECISION_FP32, bool pcm16 = false);
 int launch_gen_pre_tc(const float *mel, float *y, const RunTable &batch, int *status, cudaStream_t s);
 int launch_disc_post1_tc(const float *x, float *y, const uint8_t *wtc, const float *bias, int Bt, int L, int *status,
                          cudaStream_t s);
@@ -250,5 +266,7 @@ int launch_chain_kernel(int k, const float *x, float *y, const RunTable &t, int 
                         int precision);
 int launch_resblock_tc(const float *x, float *y, int stage, const RunTable &batch, int *status, cudaStream_t s,
                        long long *trace = nullptr, int precision = MG_GEN_PRECISION_FP32);
+// stage code 14 (the default chain's last kernel) storing pcm16 of its audio, at either precision
+int launch_resblock_tc_pcm16(const float *x, int16_t *y, const RunTable &batch, int *status, cudaStream_t s, int precision);
 
 }  // namespace mg

@@ -91,9 +91,11 @@ const char *generator_tc_kernel_config(int i, int T) {
 // Tensor-core pipeline of one contiguous slice of the batch (mel lengths, stride T_max, each run's weights).  a0: conv_pre output; a[0]:
 // ResBlock-0 output (unfused chains); a[1], a[2], u: three buffers of 8192 T_max floats per item that the stages rotate
 // through (a kernel never writes its input).  Every kernel gets the batch at its own scale.  precision goes to the ConvT
-// and ResBlock kernels (conv_pre always runs its three passes).
-static int generator_tc_chain(const float *mel, float *audio, const RunTable &batch, float *a0,
-                              float *const *a, float *u, int *status, cudaStream_t s, cudaEvent_t *ev, int precision) {
+// and ResBlock kernels (conv_pre always runs its three passes).  pcm16: audio is int16, written by the last kernel's
+// Pcm16 form (the default chain's up3+res3+post only).
+static int generator_tc_chain(const float *mel, void *audio, const RunTable &batch, float *a0,
+                              float *const *a, float *u, int *status, cudaStream_t s, cudaEvent_t *ev, int precision,
+                              bool pcm16) {
     ChainStep st[12];
     const int n = build_chain(st);
     int rc;
@@ -120,8 +122,14 @@ static int generator_tc_chain(const float *mel, float *audio, const RunTable &ba
             if (k.arg < 0) return set_error(MG_ERR_INVALID_ARGUMENT, "generator pipeline: MG_GEN_FUSE_UP=2 cannot be combined with a tail-fused up3");
             const bool last = k.arg == 4 || k.arg == 14;
             const bool front = k.arg >= 12 && k.arg <= 14, tailf = k.arg >= 20;
-            float *out = last ? audio : (k.arg <= 2 && cur != a[k.arg]) ? a[k.arg] : other(cur, nullptr);
             const int Lk = front ? 2 * len : len;  // the ResBlock's own length
+            if (last && pcm16) {
+                if (k.arg != 14) return set_error(MG_ERR_INVALID_ARGUMENT, "generator pipeline: int16 audio needs the default chain");
+                if ((rc = launch_resblock_tc_pcm16(cur, static_cast<int16_t *>(audio), batch.scaled(Lk), status, s, precision)))
+                    return rc;
+                continue;  // (the last kernel)
+            }
+            float *out = last ? static_cast<float *>(audio) : (k.arg <= 2 && cur != a[k.arg]) ? a[k.arg] : other(cur, nullptr);
             if ((rc = launch_resblock_tc(cur, out, k.arg, batch.scaled(Lk), status, s, nullptr, precision))) return rc;
             cur = out;
             len = tailf ? Lk * stage_stride(k.arg - 20 + 1) : Lk;
@@ -173,9 +181,10 @@ int generator_tc_slices(int B, long long frames) {
 // mel_host / audio_host (both or neither; pinned): the host-buffer entry point's copies, cut the same way -- each slice's
 // stream uploads its items' valid mel prefixes before its chain and downloads its audio rows (valid prefix and zero tail)
 // after it, so all but the last download overlap the other chains' kernels.  precision: MG_GEN_PRECISION_*; the caller
-// has checked that a bf16 forward runs the default chain.
-int launch_generator_tc(const float *mel, float *audio, const RunTable &batch, float *ws, int *status,
-                        cudaStream_t s, cudaEvent_t *ev, const float *mel_host, float *audio_host, int precision) {
+// has checked that a bf16 forward runs the default chain.  pcm16: audio and audio_host hold int16 samples (the caller has
+// checked the chain), so every audio offset and size counts 2-byte elements.
+int launch_generator_tc(const float *mel, void *audio, const RunTable &batch, float *ws, int *status,
+                        cudaStream_t s, cudaEvent_t *ev, const float *mel_host, void *audio_host, int precision, bool pcm16) {
     const int B = batch.items(), T = batch.stride;
     long long frames = 0;
     for (int r = 0; r < batch.n; ++r) frames += (long long)(batch.item0[r + 1] - batch.item0[r]) * batch.len[r];
@@ -197,7 +206,7 @@ int launch_generator_tc(const float *mel, float *audio, const RunTable &batch, f
     float *base[6];
     for (int i = 0; i < 6; ++i) base[i] = ws + ws_offset(i, B, T);
     const size_t per_item[6] = {(size_t)512 * T, (size_t)256 * 8 * T, (size_t)128 * 64 * T, (size_t)64 * 128 * T, 0, (size_t)8192 * T};
-    const size_t mel_item = (size_t)kMelBins * T, audio_item = (size_t)256 * T;
+    const size_t mel_item = (size_t)kMelBins * T, audio_item = (size_t)256 * T * (pcm16 ? sizeof(int16_t) : sizeof(float));  // (bytes)
     // one pool per (host thread, device): streams and events belong to the device that was current when they were created
     static thread_local SliceStreams pools[kMaxDevices];
     int dev = 0;
@@ -229,11 +238,12 @@ int launch_generator_tc(const float *mel, float *audio, const RunTable &batch, f
                                                   rows, cudaMemcpyHostToDevice, q));
             }
             float *a[3] = {base[1] + b0 * per_item[1], base[2] + b0 * per_item[2], base[3] + b0 * per_item[3]};
-            int r = generator_tc_chain(mel + b0 * mel_item, audio + b0 * audio_item, part, base[0] + b0 * per_item[0], a,
-                                       base[5] + b0 * per_item[5], status, q, ev, precision);
+            char *audio_b = static_cast<char *>(audio) + b0 * audio_item;
+            int r = generator_tc_chain(mel + b0 * mel_item, audio_b, part, base[0] + b0 * per_item[0], a,
+                                       base[5] + b0 * per_item[5], status, q, ev, precision, pcm16);
             if (r) return r;
             if (audio_host)
-                MG_CUDA_TRY(cudaMemcpyAsync(audio_host + b0 * audio_item, audio + b0 * audio_item, nb * audio_item * sizeof(float),
+                MG_CUDA_TRY(cudaMemcpyAsync(static_cast<char *>(audio_host) + b0 * audio_item, audio_b, nb * audio_item,
                                             cudaMemcpyDeviceToHost, q));
             return MG_OK;
         };

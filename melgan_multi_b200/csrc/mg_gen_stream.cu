@@ -117,6 +117,19 @@ __global__ void __launch_bounds__(256) stream_window_kernel(const float *__restr
     }
 }
 
+// The audio copy of an int16 step (mg_gen_stream_step_pcm16): the last window-assembly launch's jobs (no tail, no
+// kept positions, dst_row unused: one channel), storing pcm16 of each newly final sample into the caller's int16 row.
+__global__ void __launch_bounds__(256) stream_audio_pcm16_kernel(const float *__restrict__ src, long long src_item_stride,
+                                                                 int16_t *__restrict__ dst, long long dst_item_stride,
+                                                                 const __grid_constant__ AsmTable t) {
+    tc::pdl_wait();
+    tc::pdl_trigger();
+    const AsmJob j = t.job[blockIdx.y];
+    const float *s = src + (size_t)j.src_item * src_item_stride + j.src_off;
+    int16_t *d = dst + (size_t)j.dst_item * dst_item_stride;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < j.nnew; p += gridDim.x * blockDim.x) d[p] = pcm16(s[p]);
+}
+
 struct Copy {
     const float *tail_in = nullptr;
     float *tail_out = nullptr;
@@ -135,6 +148,16 @@ int launch_window(const Copy &c, const AsmTable &t, long long max_elems, cudaStr
     bx = bx < 1 ? 1 : bx > 64 ? 64 : bx;
     MG_CUDA_TRY(launch_ex(stream_window_kernel, dim3((unsigned)bx, (unsigned)t.n), dim3(256), 0, s, true, 1, c.tail_in, c.tail_out,
                           c.tail_cap, c.src, c.src_item_stride, c.src_row, c.dst, c.dst_item_stride, c.dst_row, c.C, t));
+    return MG_OK;
+}
+
+int launch_audio_pcm16(const float *src, long long src_item_stride, int16_t *dst, long long dst_item_stride, const AsmTable &t,
+                       long long max_elems, cudaStream_t s) {
+    if (t.n == 0) return MG_OK;
+    long long bx = (max_elems + 1023) / 1024;
+    bx = bx < 1 ? 1 : bx > 64 ? 64 : bx;
+    MG_CUDA_TRY(launch_ex(stream_audio_pcm16_kernel, dim3((unsigned)bx, (unsigned)t.n), dim3(256), 0, s, true, 1, src,
+                          src_item_stride, dst, dst_item_stride, t));
     return MG_OK;
 }
 
@@ -369,9 +392,10 @@ void mg_gen_stream_destroy(mg_gen_stream *s) { delete s; }
 
 namespace {
 
-// mg_gen_stream_step_voices, and mg_gen_stream_step as its one-voice case (&packed, 1, NULL)
+// mg_gen_stream_step_voices, and mg_gen_stream_step as its one-voice case (&packed, 1, NULL); pcm16: audio holds int16
+// samples (mg_gen_stream_step_pcm16), written by the int16 form of the last copy -- the chain and the state are the same
 int step_voices(const char *fn, mg_gen_stream *s, const void *const *packed, int n_voices, const int *voice, const float *mel,
-                const int *frames, const int *flags, int n, float *audio, int *out_samples, void *stream) {
+                const int *frames, const int *flags, int n, void *audio, int *out_samples, void *stream, bool pcm16 = false) {
     if (!s || !packed || !audio) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
     if (s->dry) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: this handle was advanced by mg_gen_stream_dry_step", fn);
     if (n_voices < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, n_voices);
@@ -427,14 +451,20 @@ int step_voices(const char *fn, mg_gen_stream *s, const void *const *packed, int
         prev_row = kRatio[k] * stride;
         prev_item = (long long)kC[k + 1] * prev_row;
     }
-    Copy c;  // the newly final audio of every session to its row of the caller's buffer
-    c.src = prev;
-    c.src_item_stride = prev_item;
-    c.src_row = prev_row;
-    c.dst = audio;
-    c.dst_item_stride = mg_gen_stream_max_out(s->P);
-    c.dst_row = 0;
-    if ((rc = launch_window(c, p.asm_[kKernels], p.asm_elems[kKernels], st))) return rc;
+    if (pcm16) {  // the newly final audio of every session, as pcm16, to its row of the caller's int16 buffer
+        if ((rc = launch_audio_pcm16(prev, prev_item, static_cast<int16_t *>(audio), mg_gen_stream_max_out(s->P), p.asm_[kKernels],
+                                     p.asm_elems[kKernels], st)))
+            return rc;
+    } else {
+        Copy c;  // the newly final audio of every session to its row of the caller's buffer
+        c.src = prev;
+        c.src_item_stride = prev_item;
+        c.src_row = prev_row;
+        c.dst = static_cast<float *>(audio);
+        c.dst_item_stride = mg_gen_stream_max_out(s->P);
+        c.dst_row = 0;
+        if ((rc = launch_window(c, p.asm_[kKernels], p.asm_elems[kKernels], st))) return rc;
+    }
     memcpy(s->F, p.F, sizeof(p.F));
     memcpy(s->par, p.par, sizeof(p.par));
     memcpy(s->voice, p.bound, sizeof(p.bound));
@@ -462,6 +492,12 @@ extern "C" {
 int mg_gen_stream_step_voices(mg_gen_stream *s, const void *const *packed, int n_voices, const int *voice, const float *mel,
                               const int *frames, const int *flags, int n, float *audio, int *out_samples, void *stream) {
     return step_voices("mg_gen_stream_step_voices", s, packed, n_voices, voice, mel, frames, flags, n, audio, out_samples, stream);
+}
+
+int mg_gen_stream_step_pcm16(mg_gen_stream *s, const void *const *packed, int n_voices, const int *voice, const float *mel,
+                             const int *frames, const int *flags, int n, int16_t *audio, int *out_samples, void *stream) {
+    return step_voices("mg_gen_stream_step_pcm16", s, packed, n_voices, voice, mel, frames, flags, n, audio, out_samples, stream,
+                       true);
 }
 
 int mg_gen_stream_step(mg_gen_stream *s, const void *packed, const float *mel, const int *frames, const int *flags, int n, float *audio,

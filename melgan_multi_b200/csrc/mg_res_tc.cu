@@ -43,6 +43,7 @@
 // product -- in the convs and the front ConvT's taps --, X and the front ConvT operand written as hi only, the weight
 // ring filled with the hi half of each chunk (C <= 64: the whole stacked chunk, of which only the hi rows are read) and the cluster halo exchange sending the hi k-panels only.  The fp32 parts
 // (residual stream, biases, conv_post epilogue) are unchanged.
+// Pcm16<Cfg> (Up3Rb3Post and Bf16<Up3Rb3Post>): the audio is stored as 16-bit PCM, pcm16(tanhf(acc)), see below.
 #include <stdlib.h>
 #include <string.h>
 
@@ -61,6 +62,7 @@ struct RbCfg {
     static constexpr bool POST = POST_;  // fuse LeakyReLU -> conv_post -> tanh into the final epilogue (last stage)
     static constexpr bool UPF = UPF_;
     static constexpr bool ONEPASS = false;  // Bf16<RbCfg<..>>: one bf16 pass per product (mg_tc.cuh)
+    using Out = float;                      // element type of y; Pcm16<Cfg>: int16 audio
     static constexpr int P = 64 * NRB;
     static constexpr int NWG = NRB / RPW * NCP;  // consumer warpgroups
     static constexpr int NCONS = 128 * NWG;
@@ -108,6 +110,15 @@ struct RbCfg {
     static_assert(NRB % RPW == 0 && C % NCP == 0 && NCW % 32 == 0, "warpgroup split");
 };
 
+// 16-bit PCM output of a conv_post configuration (mg_gen_forward_pcm16): the same kernel, whose epilogue stores
+// pcm16(tanhf(acc)) (mg_common.cuh) as int16 instead of tanhf(acc); everything before the store is unchanged, so the
+// samples are pcm16 of the float kernel's bit for bit.  A distinct type, so the instantiation has a symbol of its own.
+template <class Cfg>
+struct Pcm16 : Cfg {
+    using Out = int16_t;
+    static_assert(Cfg::POST, "int16 output is the audio of a conv_post configuration");
+};
+
 template <int RPW, int R>
 __device__ __forceinline__ void acc_fence2(float (&a)[RPW][R]) {
 #pragma unroll
@@ -116,7 +127,7 @@ __device__ __forceinline__ void acc_fence2(float (&a)[RPW][R]) {
 
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NT, 1)
-resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, int stage, const __grid_constant__ RunTable clusters,
+resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y_, int stage, const __grid_constant__ RunTable clusters,
                    int *__restrict__ status, long long *__restrict__ trace) {
     constexpr int C = Cfg::C, P = Cfg::P, SLACK = Cfg::SLACK, HALO = Cfg::HALO, HL = Cfg::HL;
     constexpr int XPITCH = Cfg::XPITCH, XBYTES = Cfg::XBYTES, KC = Cfg::KC, CHUNK = Cfg::CHUNK, NSTAGE = Cfg::NSTAGE;
@@ -140,6 +151,10 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, int stage
     // bytes of a ResBlock / front-ConvT weight chunk brought in (single pass: the hi half where it is contiguous)
     constexpr uint32_t WBYTES = ONE && !STK ? Cfg::HALF : CHUNK;
     static_assert(!ONE || Cfg::UPT == 0, "the single-pass variant has no tail ConvT");
+    // y is declared float * for every configuration, so that the float instantiations keep their signature and symbol;
+    // Pcm16<Cfg> stores int16 audio through it
+    typename Cfg::Out *__restrict__ y = reinterpret_cast<typename Cfg::Out *>(y_);
+    static_assert(Cfg::POST || sizeof(typename Cfg::Out) == sizeof(float), "int16 output is for the conv_post epilogue only");
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *Xh = smem, *Xl = smem + XBYTES, *ring = smem + 2 * XBYTES;
     float *pend = reinterpret_cast<float *>(ring + NSTAGE * CHUNK);  // sum of the c2 biases folded so far
@@ -659,11 +674,11 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, int stage
                     const int pp = p + k - 3;  // outside the tile only where it is outside the sequence too (zero padding)
                     if (pp >= 0 && pp < P) acc += Q[k * P + pp];
                 }
-                y[(size_t)b * Ls + tp] = tanhf(acc);
+                y[(size_t)b * Ls + tp] = audio_sample<typename Cfg::Out>(tanhf(acc));
             }
         }
         if (oc + P >= L)  // the item's last CTA: the audio past the item's end reads 0 (ragged batches)
-            for (int p = L + tid; p < Ls; p += NCONS) y[(size_t)b * Ls + p] = 0.f;
+            for (int p = L + tid; p < Ls; p += NCONS) y[(size_t)b * Ls + p] = 0;
         MG_TR(25);
     } else if constexpr (Cfg::UPT != 0) {
         // ---- tail ConvT: D[s, phi*TNG + co] (+)= X[s - tap, :] * Wstack_tap^T over the C channels of X = split(lrelu(x_out))
@@ -789,7 +804,7 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y, int stage
 }
 
 template <class Cfg>
-static int launch_resblock(const float *x, float *y, int stage, const RunTable &batch, int *status,
+static int launch_resblock(const float *x, typename Cfg::Out *y, int stage, const RunTable &batch, int *status,
                            long long *trace, cudaStream_t s) {
     static bool configured = false;
     if (!configured) {
@@ -816,8 +831,8 @@ static int launch_resblock(const float *x, float *y, int stage, const RunTable &
         const long long v = n;
         MG_CUDA_TRY(cudaMemcpy(trace + 127, &v, sizeof(v), cudaMemcpyHostToDevice));
     }
-    MG_CUDA_TRY(launch_ex(resblock_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, CS, x, y, stage, clusters,
-                          status, trace));
+    MG_CUDA_TRY(launch_ex(resblock_tc_kernel<Cfg>, grid, dim3(Cfg::NT), Cfg::SMEM_BYTES, s, true, CS, x, reinterpret_cast<float *>(y),
+                          stage, clusters, status, trace));
     return MG_OK;
 }
 
@@ -880,6 +895,14 @@ int launch_resblock_tc(const float *x, float *y, int stage, const RunTable &batc
         case 22: return launch_resblock<Rb2Up3>(x, y, 2, batch, status, trace, s);
     }
     return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc: stage %d", stage);
+}
+
+// the default chain's last kernel (stage code 14) with int16 audio y [B][1][L]: pcm16 of what launch_resblock_tc(.., 14, ..)
+// stores at the same precision
+int launch_resblock_tc_pcm16(const float *x, int16_t *y, const RunTable &batch, int *status, cudaStream_t s, int precision) {
+    if (precision == MG_GEN_PRECISION_FP32) return launch_resblock<Pcm16<Up3Rb3Post>>(x, y, 3, batch, status, nullptr, s);
+    if (precision == MG_GEN_PRECISION_BF16) return launch_resblock<Pcm16<Bf16<Up3Rb3Post>>>(x, y, 3, batch, status, nullptr, s);
+    return set_error(MG_ERR_INVALID_ARGUMENT, "launch_resblock_tc_pcm16: precision %d", precision);
 }
 
 // the configuration launch_resblock_tc runs for a stage code (evidence files record it)

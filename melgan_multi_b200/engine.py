@@ -198,6 +198,12 @@ def lib():
         L.mg_gen_stream_step_voices.restype = ctypes.c_int
         L.mg_gen_stream_step_voices.argtypes = ([ctypes.c_void_p] * 2 + [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int]
                                                 + [ctypes.c_void_p] * 3)
+        L.mg_gen_forward_pcm16.restype = ctypes.c_int
+        L.mg_gen_forward_pcm16.argtypes = L.mg_gen_forward_voices.argtypes
+        L.mg_gen_stream_step_pcm16.restype = ctypes.c_int
+        L.mg_gen_stream_step_pcm16.argtypes = L.mg_gen_stream_step_voices.argtypes
+        L.mg_gen_engine_forward_pcm16.restype = ctypes.c_int
+        L.mg_gen_engine_forward_pcm16.argtypes = L.mg_gen_engine_forward_precision.argtypes
         L.mg_gen_stream_dry_step_voices.restype = ctypes.c_int
         L.mg_gen_stream_dry_step_voices.argtypes = ([ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int]
                                                     + [ctypes.c_void_p] * 3)
@@ -259,6 +265,45 @@ def _precision(precision):
     if not isinstance(precision, str) or precision not in PRECISIONS:
         raise EngineError("precision must be one of %s (got %r)" % (", ".join(map(repr, PRECISIONS)), precision))
     return PRECISIONS[precision]
+
+
+def _pcm16(dtype):
+    """Whether an inference call returns 16-bit PCM: dtype torch.float32 (fp32 audio in [-1, 1]) or torch.int16 (pcm16 of
+    that audio: 0 for NaN, else clamp(rint(32768 a), -32768, 32767), contract at mg_gen_forward_pcm16 in
+    include/melgan_b200.h)."""
+    import torch
+    if dtype is torch.float32:
+        return False
+    if dtype is torch.int16:
+        return True
+    raise EngineError("dtype must be torch.float32 or torch.int16 (got %r)" % (dtype,))
+
+
+def _pcm16_np(dtype):
+    """_pcm16 for the host-buffer path: np.float32 or np.int16 (or their np.dtype)."""
+    try:
+        dt = np.dtype(dtype)
+    except TypeError:
+        dt = None
+    if dt == np.float32 and not isinstance(dtype, str):
+        return False
+    if dt == np.int16 and not isinstance(dtype, str):
+        return True
+    raise EngineError("dtype must be np.float32 or np.int16 (got %r)" % (dtype,))
+
+
+def _audio_out(torch, out, shape, pcm, device):
+    """The caller's out= for audio of `shape` (None: a new tensor of the call's dtype).  An int16 out needs dtype=torch.int16
+    and the reverse, on the call's device, contiguous and of the audio's shape."""
+    dt = torch.int16 if pcm else torch.float32
+    if out is None:
+        return torch.empty(shape, dtype=dt, device=device)
+    if pcm or out.dtype == torch.int16:
+        if out.dtype != dt:
+            raise EngineError("out is %s but dtype is %s" % (out.dtype, dt))
+        if out.device != device or tuple(out.shape) != tuple(shape) or not out.is_contiguous():
+            raise EngineError("out must be a contiguous %s tensor of shape %s on %s" % (dt, tuple(shape), device))
+    return out
 
 
 class _StatusWatch:
@@ -486,25 +531,30 @@ class GeneratorDevice(_PackedBlob):
         """The current stream's workspace, grown to mg_gen_workspace_bytes(B, T)."""
         return self._scratch.current().buffer("ws", lib().mg_gen_workspace_bytes(B, T))
 
-    def forward(self, mel, out=None, precision="fp32"):
+    def forward(self, mel, out=None, precision="fp32", dtype=None):
         """mel [B, 80, T] -> audio [B, 1, 256 T].  precision "fp32" (the default) or "bf16" (one bf16 pass per tensor-core
-        product: inference only, contract at mg_gen_forward_precision in include/melgan_b200.h)."""
+        product: inference only, contract at mg_gen_forward_precision in include/melgan_b200.h).  dtype torch.float32 (the
+        default) or torch.int16: 16-bit PCM written by the last kernel, pcm16 of the float audio bit for bit (contract at
+        mg_gen_forward_pcm16); out= must then be int16."""
         torch = self.torch
         code = _precision(precision)
+        pcm = _pcm16(torch.float32 if dtype is None else dtype)
         if mel.dim() != 3 or mel.shape[1] != 80:
             raise EngineError("mel must be [B, 80, T], got %s" % (tuple(mel.shape),))
         if mel.device != self.device or mel.dtype != torch.float32:
             raise EngineError("mel must be an fp32 tensor on %s" % (self.device,))
         mel = mel.contiguous()
         B, _, T = mel.shape
-        if out is None:
-            out = torch.empty((B, 1, 256 * T), dtype=torch.float32, device=self.device)
+        out = _audio_out(torch, out, (B, 1, 256 * T), pcm, self.device)
         sc = self._scratch.current()
         sc.check()  # the previous forward's status word on this stream, if its copy has landed
         ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            if code == 0:
+            if pcm:
+                check(lib().mg_gen_forward_pcm16(_ptr_array([self.packed.data_ptr()]), 1, None, mel.data_ptr(), out.data_ptr(),
+                                                 B, T, None, code, ws.data_ptr(), ws.numel() * 4, stream))
+            elif code == 0:
                 check(lib().mg_gen_forward(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T,
                                            ws.data_ptr(), ws.numel() * 4, stream))
             else:
@@ -514,12 +564,14 @@ class GeneratorDevice(_PackedBlob):
             sc.arm(ws.view(torch.int32)[off:off + 1])
         return out
 
-    def forward_ragged(self, mel, lengths, out=None, precision="fp32"):
+    def forward_ragged(self, mel, lengths, out=None, precision="fp32", dtype=None):
         """Ragged batch (inference): mel [B, 80, T_max] with item i's frames [0, lengths[i]) valid (the rest is never read)
         -> audio [B, 1, 256 T_max]; item i's first 256 lengths[i] samples equal its own forward (at the same precision) bit
-        for bit, the rest are 0.  lengths: a list, a tuple or a CPU integer tensor.  Asynchronous, like forward."""
+        for bit, the rest are 0.  lengths: a list, a tuple or a CPU integer tensor.  dtype as for forward.  Asynchronous,
+        like forward."""
         torch = self.torch
         code = _precision(precision)
+        pcm = _pcm16(torch.float32 if dtype is None else dtype)
         if mel.dim() != 3 or mel.shape[1] != 80:
             raise EngineError("mel must be [B, 80, T_max], got %s" % (tuple(mel.shape),))
         if mel.device != self.device or mel.dtype != torch.float32:
@@ -527,14 +579,16 @@ class GeneratorDevice(_PackedBlob):
         mel = mel.contiguous()
         B, _, T = mel.shape
         lens = _lengths(lengths, B, T)
-        if out is None:
-            out = torch.empty((B, 1, 256 * T), dtype=torch.float32, device=self.device)
+        out = _audio_out(torch, out, (B, 1, 256 * T), pcm, self.device)
         sc = self._scratch.current()
         sc.check()
         ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
-            if code == 0:
+            if pcm:
+                check(lib().mg_gen_forward_pcm16(_ptr_array([self.packed.data_ptr()]), 1, None, mel.data_ptr(), out.data_ptr(),
+                                                 B, T, lens, code, ws.data_ptr(), ws.numel() * 4, stream))
+            elif code == 0:
                 check(lib().mg_gen_forward_ragged(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens,
                                                   ws.data_ptr(), ws.numel() * 4, stream))
             else:
@@ -544,15 +598,16 @@ class GeneratorDevice(_PackedBlob):
             sc.arm(ws.view(torch.int32)[off:off + 1])
         return out
 
-    def forward_voices(self, voices, mel, voice, lengths=None, out=None, precision="fp32"):
+    def forward_voices(self, voices, mel, voice, lengths=None, out=None, precision="fp32", dtype=None):
         """Many voices in one forward (inference): item i of mel [B, 80, T_max] runs on the weights of voices[voice[i]] (a
         sequence of GeneratorDevice on this device, this one among them or not) -> audio [B, 1, 256 T_max], each item bit
         for bit its own forward on its own voice (at the same precision; 0 past 256 lengths[i] samples).  voice: B ids in
         [0, len(voices)), and lengths as in forward_ragged (None: every item T_max frames), each a list, a tuple or a CPU
         integer tensor.  Items sorted by voice run fastest (contract at mg_gen_forward_voices, include/melgan_b200.h).
-        Uses this module's scratch of the current stream.  Asynchronous, like forward."""
+        dtype as for forward.  Uses this module's scratch of the current stream.  Asynchronous, like forward."""
         torch = self.torch
         code = _precision(precision)
+        pcm = _pcm16(torch.float32 if dtype is None else dtype)
         if mel.dim() != 3 or mel.shape[1] != 80:
             raise EngineError("mel must be [B, 80, T_max], got %s" % (tuple(mel.shape),))
         if mel.device != self.device or mel.dtype != torch.float32:
@@ -567,16 +622,15 @@ class GeneratorDevice(_PackedBlob):
         B, _, T = mel.shape
         lens = None if lengths is None else _lengths(lengths, B, T)
         ids = _voice_ids(voice, B, len(voices))
-        if out is None:
-            out = torch.empty((B, 1, 256 * T), dtype=torch.float32, device=self.device)
+        out = _audio_out(torch, out, (B, 1, 256 * T), pcm, self.device)
         sc = self._scratch.current()
         sc.check()
         ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
             blobs = _ptr_array([v.packed.data_ptr() for v in voices])  # (each read orders this stream after its pack)
-            check(lib().mg_gen_forward_voices(blobs, len(voices), ids, mel.data_ptr(), out.data_ptr(), B,
-                                              T, lens, code, ws.data_ptr(), ws.numel() * 4, stream))
+            fn = lib().mg_gen_forward_pcm16 if pcm else lib().mg_gen_forward_voices
+            check(fn(blobs, len(voices), ids, mel.data_ptr(), out.data_ptr(), B, T, lens, code, ws.data_ptr(), ws.numel() * 4, stream))
             off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4
             sc.arm(ws.view(torch.int32)[off:off + 1])
         return out
@@ -756,16 +810,19 @@ class GeneratorStream:
     weights changed between steps are re-packed), or a list of them, one per voice (models.stream_voices): slot i then
     runs on the weights of voice[i] (mg_gen_stream_step_voices; an open utterance keeps the voice it was opened with until
     it ends or is reset).  state: optional caller-provided uint8 CUDA tensor of at least mg_gen_stream_state_bytes bytes
-    (the stream never lets a byte it has not written reach an output).
+    (the stream never lets a byte it has not written reach an output).  dtype: the handle's audio format, torch.float32
+    (the default) or torch.int16 (16-bit PCM, pcm16 of the float samples bit for bit: mg_gen_stream_step_pcm16).
 
     One thread drives a handle at a time, and all steps of one handle must be enqueued on one CUDA stream (or otherwise
     ordered), as for mg_gen_stream_step: the state and the mel staging buffer that ``step`` copies each chunk into are
     the handle's own, and the next step overwrites them in stream order.  Distinct handles of one generator may step
     concurrently on distinct streams or threads."""
 
-    def __init__(self, packed_fn, device, max_sessions=1, max_push_frames=32, precision="fp32", state=None):
+    def __init__(self, packed_fn, device, max_sessions=1, max_push_frames=32, precision="fp32", state=None, dtype=None):
         import torch
         self.torch = torch
+        self.dtype = torch.float32 if dtype is None else dtype
+        _pcm16(self.dtype)
         self._packed_fn = packed_fn
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -793,7 +850,8 @@ class GeneratorStream:
     def step_packed(self, mel, frames, flags=None, audio=None, voice=None):
         """The C step on a packed buffer: mel [n, 80, max_push_frames] fp32 CUDA (slot i's frames first), frames / flags: n
         ints, voice: None (every slot on the first voice) or n voice ids as for ``step``.  Returns (audio [n, max_out],
-        per-slot sample counts as a list of ints)."""
+        per-slot sample counts as a list of ints).  audio: None (a new tensor of the handle's dtype) or a contiguous fp32 or
+        int16 CUDA tensor [n, max_out], whose dtype picks this step's format (float and int16 steps may alternate)."""
         torch = self.torch
         n = len(frames)
         devs = self._packed_fn()
@@ -803,15 +861,20 @@ class GeneratorStream:
                 raise EngineError("stream: a voice's weights are on %s, the stream on %s" % (d.device, self.device))
         ids = None if voice is None else _voice_ids(voice, n, len(devs))
         if audio is None:
-            audio = torch.empty((n, self.max_out), dtype=torch.float32, device=self.device)
+            audio = torch.empty((n, self.max_out), dtype=self.dtype, device=self.device)
+        pcm = audio.dtype == torch.int16
+        if pcm and (audio.device != self.device or audio.dim() != 2 or audio.shape[0] < n or audio.shape[1] != self.max_out
+                    or not audio.is_contiguous()):
+            raise EngineError("stream: int16 audio must be a contiguous [%d, %d] tensor on %s" % (n, self.max_out, self.device))
         fr = (ctypes.c_int * max(n, 1))(*[int(v) for v in frames])
         fl = (ctypes.c_int * max(n, 1))(*[int(v) for v in flags]) if flags is not None else None
         cnt = (ctypes.c_int * max(n, 1))()
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream().cuda_stream
             blobs = _ptr_array([d.packed.data_ptr() for d in devs])  # (each read orders this stream after its pack)
-            check(lib().mg_gen_stream_step_voices(self._h, blobs, len(devs), ids, mel.data_ptr() if mel is not None else None,
-                                                  fr, fl, n, audio.data_ptr(), cnt, stream))
+            fn = lib().mg_gen_stream_step_pcm16 if pcm else lib().mg_gen_stream_step_voices
+            check(fn(self._h, blobs, len(devs), ids, mel.data_ptr() if mel is not None else None, fr, fl, n, audio.data_ptr(), cnt,
+                     stream))
         return audio, [cnt[i] for i in range(n)]
 
     def step(self, chunks, end=None, reset=None, voice=None):
@@ -819,7 +882,7 @@ class GeneratorStream:
         end / reset: None or n booleans (end: the utterance ends after this chunk; reset: drop the slot's unfinished
         utterance first); voice: None (every slot on the first voice) or n voice ids (a list, a tuple or a CPU integer
         tensor) -- a slot's id may change only on a step that resets it or once its utterance has ended.  Returns n [1, m_i]
-        CUDA tensors of newly final audio, owned by the caller.  Asynchronous on the current stream: the lengths are known on
+        CUDA tensors of newly final audio in the handle's dtype, owned by the caller.  Asynchronous on the current stream: the lengths are known on
         return, the values once the stream gets there."""
         n = len(chunks)
         if n > self.max_sessions:
@@ -1183,33 +1246,48 @@ class GeneratorHost:
                 lst.append(a.ctypes.data)
         check(lib().mg_gen_engine_load_state(self._h, _ptr_array(vs), _ptr_array(gs), _ptr_array(bs)))
 
-    def forward(self, mel, out=None, precision="fp32"):
-        """mel [B, 80, T] -> audio [B, 1, 256 T]; precision as for GeneratorDevice.forward."""
+    def forward(self, mel, out=None, precision="fp32", dtype=np.float32):
+        """mel [B, 80, T] -> audio [B, 1, 256 T]; precision as for GeneratorDevice.forward.  dtype np.float32 (the default)
+        or np.int16: 16-bit PCM, pcm16 of the float audio bit for bit (mg_gen_engine_forward_pcm16)."""
         code = _precision(precision)
+        pcm = _pcm16_np(dtype)
         mel = np.ascontiguousarray(mel, dtype=np.float32)
         B, C, T = mel.shape
         if C != 80:
             raise EngineError("mel must be [B, 80, T]")
-        if out is None:
-            out = np.empty((B, 1, 256 * T), np.float32)
-        if code == 0:
+        out = self._out(out, (B, 1, 256 * T), pcm)
+        if pcm:
+            check(lib().mg_gen_engine_forward_pcm16(self._h, mel.ctypes.data, out.ctypes.data, B, T, None, code))
+        elif code == 0:
             check(lib().mg_gen_engine_forward(self._h, mel.ctypes.data, out.ctypes.data, B, T))
         else:
             check(lib().mg_gen_engine_forward_precision(self._h, mel.ctypes.data, out.ctypes.data, B, T, None, code))
         return out
 
-    def forward_ragged(self, mel, lengths, out=None, precision="fp32"):
+    @staticmethod
+    def _out(out, shape, pcm):
+        dt = np.int16 if pcm else np.float32
+        if out is None:
+            return np.empty(shape, dt)
+        if pcm or out.dtype == np.int16:
+            if out.dtype != dt or tuple(out.shape) != tuple(shape) or not out.flags.c_contiguous:
+                raise EngineError("out must be a C-contiguous %s array of shape %s" % (np.dtype(dt).name, tuple(shape)))
+        return out
+
+    def forward_ragged(self, mel, lengths, out=None, precision="fp32", dtype=np.float32):
         """Ragged batch from host memory (mg_gen_engine_forward_ragged): mel [B, 80, T_max], lengths and precision as for
-        GeneratorDevice.forward_ragged -> audio [B, 1, 256 T_max]."""
+        GeneratorDevice.forward_ragged, dtype as for forward -> audio [B, 1, 256 T_max]."""
         code = _precision(precision)
+        pcm = _pcm16_np(dtype)
         mel = np.ascontiguousarray(mel, dtype=np.float32)
         if mel.ndim != 3 or mel.shape[1] != 80:
             raise EngineError("mel must be [B, 80, T_max]")
         B, _, T = mel.shape
         lens = _lengths(lengths, B, T)
-        if out is None:
-            out = np.empty((B, 1, 256 * T), np.float32)
-        if code == 0:
+        out = self._out(out, (B, 1, 256 * T), pcm)
+        if pcm:
+            check(lib().mg_gen_engine_forward_pcm16(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens, code))
+        elif code == 0:
             check(lib().mg_gen_engine_forward_ragged(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens))
         else:
             check(lib().mg_gen_engine_forward_precision(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens, code))

@@ -169,32 +169,37 @@ class Generator(nn.Module):
     def _engine_forward(self, mel):
         return self._ensure_packed().forward(mel)
 
-    def generate(self, x, lengths=None, precision="fp32"):
+    def generate(self, x, lengths=None, precision="fp32", dtype=torch.float32):
         """Vocodes a batch in one forward (inference only: no autograd graph is built).  x [B, 80, T_max] fp32 CUDA.
         lengths None: every item has T_max frames.  Otherwise B mel lengths in [1, T_max] as a list, a tuple or a CPU integer
         tensor; the frames past each length are never read, and the audio [B, 1, 256 T_max] of item i starts with exactly
         the 256 lengths[i] samples of generate(x[i:i+1, :, :lengths[i]], precision=precision) and is 0 after them.
         precision "fp32" computes what self(x) computes; "bf16" runs one bf16 pass per tensor-core product (faster, audio
-        about 1e-3 from float64 in relative L2: the contract is at mg_gen_forward_precision, include/melgan_b200.h)."""
+        about 1e-3 from float64 in relative L2: the contract is at mg_gen_forward_precision, include/melgan_b200.h).
+        dtype torch.float32 returns audio in [-1, 1]; torch.int16 returns 16-bit PCM written by the last kernel, bit for bit
+        pcm16 of the float audio: 0 for NaN, else clamp(rint(32768 a), -32768, 32767) (mg_gen_forward_pcm16)."""
         _engine._precision(precision)
+        _engine._pcm16(dtype)
         if not x.is_cuda:
             raise _engine.EngineError("melgan_multi_b200.Generator.generate needs a CUDA tensor (no CPU fallback)")
         with torch.no_grad():
             dev = self._ensure_packed()
             if lengths is None:
-                return dev.forward(x.detach().float(), precision=precision)
-            return dev.forward_ragged(x.detach().float(), lengths, precision=precision)
+                return dev.forward(x.detach().float(), precision=precision, dtype=dtype)
+            return dev.forward_ragged(x.detach().float(), lengths, precision=precision, dtype=dtype)
 
-    def stream(self, max_sessions=1, max_push_frames=32, precision="fp32"):
+    def stream(self, max_sessions=1, max_push_frames=32, precision="fp32", dtype=torch.float32):
         """A streaming vocoder over this generator's weights (inference only): up to max_sessions live mel streams, each
         step pushing at most max_push_frames new frames per session and returning the audio samples that became final
         (engine.GeneratorStream; the concatenation of a session's outputs equals generate() of its whole mel bit for bit).
-        Weights changed between steps are re-packed, as in generate."""
+        Weights changed between steps are re-packed, as in generate.  dtype: the format of every step's audio, as in
+        generate (torch.int16: pcm16 of the float samples)."""
+        _engine._pcm16(dtype)
         vs, _, _ = self._param_triplets()
         if vs[0].device.type != "cuda":
             raise _engine.EngineError("melgan_multi_b200.Generator.stream needs the module on CUDA (no CPU fallback)")
         self._ensure_packed()
-        return _engine.GeneratorStream(self._ensure_packed, vs[0].device, max_sessions, max_push_frames, precision)
+        return _engine.GeneratorStream(self._ensure_packed, vs[0].device, max_sessions, max_push_frames, precision, dtype=dtype)
 
     def _graphed_recompute(self, mel, params):
         """(graphed stock-op forward+backward, mel_requires_grad) for this input shape, or None.  Cached per shape and per
@@ -252,14 +257,15 @@ class Generator(nn.Module):
         return _GeneratorFunction.apply(self, x, *flat)
 
 
-def generate_voices(generators, mel, voice, lengths=None, precision="fp32"):
+def generate_voices(generators, mel, voice, lengths=None, precision="fp32", dtype=torch.float32):
     """Vocodes a batch that mixes voices in one forward (inference only: no autograd graph is built).  generators: a
     sequence of Generator modules (a vocoder fine-tuned per speaker, say) on mel's CUDA device, each packed lazily as
     generate packs it.  mel [B, 80, T_max] fp32; voice: B ids in [0, len(generators)) as a list, a tuple or a CPU integer
     tensor; lengths as in Generator.generate (None: every item T_max frames).  Item i of the audio [B, 1, 256 T_max] is
     bit for bit generators[voice[i]].generate(mel[i:i+1, :, :lengths[i]], precision=precision), then 0.  Items need not be
-    sorted by voice, but sorted ones run fastest."""
+    sorted by voice, but sorted ones run fastest.  dtype as in Generator.generate (torch.int16: 16-bit PCM)."""
     _engine._precision(precision)
+    _engine._pcm16(dtype)
     if not mel.is_cuda:
         raise _engine.EngineError("melgan_multi_b200.generate_voices needs a CUDA tensor (no CPU fallback)")
     generators = list(generators)
@@ -272,16 +278,18 @@ def generate_voices(generators, mel, voice, lengths=None, precision="fp32"):
             if dev.device != mel.device:
                 raise _engine.EngineError("generate_voices: a generator is on %s, mel on %s" % (dev.device, mel.device))
             devs.append(dev)
-        return devs[0].forward_voices(devs, mel.detach().float(), voice, lengths, precision=precision)
+        return devs[0].forward_voices(devs, mel.detach().float(), voice, lengths, precision=precision, dtype=dtype)
 
 
-def stream_voices(generators, max_sessions=1, max_push_frames=32, precision="fp32"):
+def stream_voices(generators, max_sessions=1, max_push_frames=32, precision="fp32", dtype=torch.float32):
     """A streaming vocoder whose live sessions run on several voices in one step (inference only): generators is a
     sequence of Generator modules on one CUDA device, each re-packed lazily at every step as Generator.stream does.  The
     returned engine.GeneratorStream's step(chunks, end=None, reset=None, voice=None) takes one voice id per slot (None:
     every slot on generators[0]); a slot keeps the voice its utterance was opened with until the utterance ends or the
-    slot is reset.  The concatenation of a session's outputs equals generators[v].generate() of its whole mel bit for bit."""
+    slot is reset.  The concatenation of a session's outputs equals generators[v].generate() of its whole mel bit for bit.
+    dtype as in Generator.stream."""
     _engine._precision(precision)
+    _engine._pcm16(dtype)
     generators = list(generators)
     if not generators:
         raise _engine.EngineError("stream_voices needs at least one generator")
@@ -298,7 +306,7 @@ def stream_voices(generators, max_sessions=1, max_push_frames=32, precision="fp3
     def packed():
         return [g._ensure_packed() for g in generators]
     packed()
-    return _engine.GeneratorStream(packed, devices.pop(), max_sessions, max_push_frames, precision)
+    return _engine.GeneratorStream(packed, devices.pop(), max_sessions, max_push_frames, precision, dtype=dtype)
 
 
 class Discriminator(nn.Module):
