@@ -28,15 +28,75 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 from torch._utils import _unflatten_dense_tensors
+from torch.multiprocessing.reductions import StorageWeakRef
 from torch.nn import AvgPool1d, Conv1d, ConvTranspose1d
 from torch.nn.utils import weight_norm
+from torch.optim.optimizer import register_optimizer_step_post_hook
 
 from . import engine as _engine
+from .optim import _bump_versions
 from .synth import DISCRIMINATOR_LAYERS, GENERATOR_LAYERS
 
 # Makes a module's lazy (re-)pack one step when host threads call it at once: the first caller packs (engine
 # _PackedBlob orders every later read of the blob after that pack), the others see the weights already packed.
 _PACK_LOCK = threading.Lock()
+
+
+class _PackKey:
+    """What a module's packed blob was folded from: every parameter's (data_ptr, _version), and a weak reference to each
+    parameter's storage.  (data_ptr, _version) alone can recur: ``p.data = t`` keeps p's version counter, and the
+    caching allocator may put t where a storage freed since the pack used to be (two ``vector_to_parameters`` calls in a
+    row, ``.cpu()``, a new ``.data``, ``.cuda()``).  The freed storage's weak reference has expired then, so the key no
+    longer matches.  A weak reference keeps no memory: a freed storage's bytes go back to the allocator as before."""
+
+    def __init__(self, ts):
+        self.key = tuple((t.data_ptr(), t._version) for t in ts)
+        self.refs = [StorageWeakRef(t.untyped_storage()) for t in ts]
+
+    def matches(self, ts):
+        return self.key == tuple((t.data_ptr(), t._version) for t in ts) and not any(r.expired() for r in self.refs)
+
+
+class _Repack:
+    """The modules that fold their weight-norm parameters into a packed blob, keyed on every parameter (_PackKey).  The
+    key sees in-place ops under no_grad, optimizer steps (the fused ones through _bump_after_fused_step) and
+    ``load_state_dict``, and new storage (``p.data = t``, ``load_state_dict(assign=True)``, ``vector_to_parameters``,
+    ``.to()``).  It cannot see an in-place write through ``p.data``, nor a write the host never issues, such as a
+    replayed CUDA graph of an optimizer step.  Nor does it see ``torch._foreach_lerp_`` with a scalar weight, which
+    ``swa_utils.AveragedModel``'s EMA update runs: on CUDA that op leaves the version counters as they were
+    (torch 2.11)."""
+
+    def _pack_if_changed(self, dev, vs, gs, bs):
+        """dev.pack(vs, gs, bs) unless the blob was last folded from exactly these parameter values (call under
+        _PACK_LOCK)."""
+        ts = vs + gs + bs
+        if self._packed_key is None or not self._packed_key.matches(ts):
+            dev.pack(vs, gs, bs)
+            self._packed_key = _PackKey(ts)
+
+    def repack(self):
+        """Makes the next call of this module, and of every module inside it, fold the parameters' current values.
+        A stream or a ``generate_voices`` call built on it picks them up at its next step or call.  It does not reach
+        a module that contains this one: call repack() on the module you will call, or on the outermost one."""
+        with _PACK_LOCK:
+            for m in self.modules():
+                if isinstance(m, _Repack):
+                    m._packed_key = None
+
+
+@torch.compiler.disable  # in a compiled step, traced, the bump would be dropped
+def _bump_after_fused_step(optimizer, args, kwargs):
+    """torch.optim's fused steps (``Adam(fused=True)`` and the other ``fused`` optimizers) write the parameters without
+    bumping their version counters, unlike the for-loop and foreach forms.  Bumping them here lets the modules' packed
+    folds see the step, as autograd's saved-tensor checks then do too.  The hook is process-wide because an optimizer
+    step does not say which modules its parameters belong to; for any other parameter the bump only does what the
+    for-loop and foreach steps already do."""
+    ps = [p for g in optimizer.param_groups if g.get("fused") for p in g["params"] if p.grad is not None]
+    if ps:
+        _bump_versions(ps)
+
+
+register_optimizer_step_post_hook(_bump_after_fused_step)
 
 _RES_DILATIONS = (1, 3, 9)
 
@@ -130,8 +190,13 @@ class _GeneratorFunction(torch.autograd.Function):
         return (None, gmel, *grads)
 
 
-class Generator(nn.Module):
-    """mel [B, 80, T] fp32 CUDA -> audio [B, 1, 256*T] (reference models.py:43-71)."""
+class Generator(_Repack, nn.Module):
+    """mel [B, 80, T] fp32 CUDA -> audio [B, 1, 256*T] (reference models.py:43-71).
+
+    The weights are folded and packed at the first call and again whenever a parameter's _version or data_ptr changed:
+    optimizer steps, in-place ops under no_grad, load_state_dict and p.data = t are seen.  In-place writes through
+    p.data and replayed CUDA graphs (an optimizer step captured with capturable=True) are not, nor is an EMA update of
+    swa_utils.AveragedModel on CUDA (_Repack): call repack() after them."""
 
     def __init__(self):
         super().__init__()
@@ -142,7 +207,7 @@ class Generator(nn.Module):
         self.resblocks = nn.ModuleList([ResBlock(c, c) for c in (256, 128, 64, 32)])
         self.conv_post = _wn_conv(32, 1, 7, padding=3)
         self._dev = None          # engine.GeneratorDevice, created lazily on the parameters' device
-        self._packed_key = None   # (data_ptr, _version) of every parameter at the last pack
+        self._packed_key = None   # _PackKey of the parameters at the last pack
 
     # -- parameter plumbing -----------------------------------------------------------------
     def _param_triplets(self):
@@ -160,10 +225,7 @@ class Generator(nn.Module):
             if self._dev is None or self._dev.device != dev:
                 self._dev = _engine.GeneratorDevice(dev)
                 self._packed_key = None
-            key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
-            if key != self._packed_key:
-                self._dev.pack(vs, gs, bs)
-                self._packed_key = key
+            self._pack_if_changed(self._dev, vs, gs, bs)
             return self._dev
 
     def _engine_forward(self, mel):
@@ -192,7 +254,8 @@ class Generator(nn.Module):
         """A streaming vocoder over this generator's weights (inference only): up to max_sessions live mel streams, each
         step pushing at most max_push_frames new frames per session and returning the audio samples that became final
         (engine.GeneratorStream; the concatenation of a session's outputs equals generate() of its whole mel bit for bit).
-        Weights changed between steps are re-packed, as in generate.  dtype: the format of every step's audio, as in
+        Weights changed between steps are re-packed at the next step, as in generate (after the writes the class
+        docstring names, once repack() was called).  dtype: the format of every step's audio, as in
         generate (torch.int16: pcm16 of the float samples)."""
         _engine._pcm16(dtype)
         vs, _, _ = self._param_triplets()
@@ -309,11 +372,16 @@ def stream_voices(generators, max_sessions=1, max_push_frames=32, precision="fp3
     return _engine.GeneratorStream(packed, devices.pop(), max_sessions, max_push_frames, precision, dtype=dtype)
 
 
-class Discriminator(nn.Module):
+class Discriminator(_Repack, nn.Module):
     """One discriminator (reference models.py:74-103).  Inside ``MultiScaleDiscriminator`` (its only caller in the
     reference, models.py:109-113) the three of them run as one fused pipeline on the stacked real + generated batch;
     called on its own, ``forward(x)`` runs the same sm_90a kernels on this module's weights and returns
-    ``(flattened logits, [7 feature maps])`` like the reference's.  CUDA only, no stock-op fallback."""
+    ``(flattened logits, [7 feature maps])`` like the reference's.  CUDA only, no stock-op fallback.
+
+    Called on its own it packs its own blob, apart from the enclosing MultiScaleDiscriminator's, and re-packs it as
+    Generator does: a change of a parameter's _version or data_ptr is seen, whichever module it was made through;
+    after an in-place write through p.data, a replayed CUDA graph or an AveragedModel EMA update call repack() (the
+    enclosing module's repack() covers this one too, but this one's does not reach the enclosing module)."""
 
     def __init__(self):
         super().__init__()
@@ -342,10 +410,7 @@ class Discriminator(nn.Module):
             if getattr(self, "_dev", None) is None or self._dev.device != dev:
                 self._dev = _engine.DiscriminatorDevice(dev, ndisc=1)
                 self._packed_key = None
-            key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
-            if key != self._packed_key:
-                self._dev.pack(vs, gs, bs)
-                self._packed_key = key
+            self._pack_if_changed(self._dev, vs, gs, bs)
         return self._dev.forward(x)
 
     def forward(self, x):
@@ -415,10 +480,14 @@ class _MSDFunction(torch.autograd.Function):
         return (None, None, None, gy, *out)
 
 
-class MultiScaleDiscriminator(nn.Module):
+class MultiScaleDiscriminator(_Repack, nn.Module):
     """Reference models.py:106-135: three Discriminators on y, pool(y), pool(pool(y)); returns
     (y_d_rs, y_d_gs, fmap_rs, fmap_gs).  On CUDA the whole stack runs in the hand-written kernels of
-    libmelgan_b200.so with y and y_hat stacked into one batch (the reference calls each discriminator twice)."""
+    libmelgan_b200.so with y and y_hat stacked into one batch (the reference calls each discriminator twice).
+
+    The forward and its backward read weights packed at the first call and re-packed whenever a parameter's _version
+    or data_ptr changed, as in Generator.  After an in-place write through p.data, a replayed CUDA graph or an
+    AveragedModel EMA update call repack(), which also re-packs the three Discriminators for their stand-alone calls."""
 
     def __init__(self):
         super().__init__()
@@ -438,10 +507,7 @@ class MultiScaleDiscriminator(nn.Module):
             if self._dev is None or self._dev.device != dev:
                 self._dev = _engine.DiscriminatorDevice(dev)
                 self._packed_key = None
-            key = tuple((t.data_ptr(), t._version) for t in vs + gs + bs)
-            if key != self._packed_key:
-                self._dev.pack(vs, gs, bs)
-                self._packed_key = key
+            self._pack_if_changed(self._dev, vs, gs, bs)
         return self._dev.forward(y2)
 
     # -- stock-PyTorch restatement on folded weights, used ONLY to differentiate (backward) -----------------

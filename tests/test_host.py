@@ -154,6 +154,59 @@ def test_discriminators_refuse_cpu_tensors():
         d.discriminators[0](torch.zeros(1, 1, 64))
 
 
+@pytest.mark.parametrize("make", [lambda ps: torch.optim.Adam(ps, fused=True), lambda ps: torch.optim.AdamW(ps, fused=True),
+                                  lambda ps: torch.optim.SGD(ps, lr=0.1, fused=True)], ids=["Adam", "AdamW", "SGD"])
+def test_fused_optimizer_steps_bump_the_versions_the_packed_weights_are_keyed_on(make):
+    """torch's fused optimizer steps leave the parameters' version counters as they were; once models is imported,
+    a step bumps those of every parameter it updated, as the for-loop and foreach steps do."""
+    from melgan_multi_b200 import models  # noqa: F401 (registers the step hook)
+    p, idle = torch.nn.Parameter(torch.randn(5)), torch.nn.Parameter(torch.randn(3))
+    p.grad = torch.randn(5)
+    opt = make([p, idle])
+    v0 = p._version
+    opt.step()
+    assert p._version > v0 and idle._version == 0
+
+
+def test_compiled_fused_optimizer_step_bumps_the_versions():
+    from melgan_multi_b200 import models  # noqa: F401 (registers the step hook)
+    p = torch.nn.Parameter(torch.randn(5))
+    p.grad = torch.randn(5)
+    opt = torch.optim.Adam([p], fused=True)
+    step = torch.compile(lambda: opt.step())
+    w0, v0 = p.detach().clone(), p._version
+    step()
+    assert not torch.equal(p.detach(), w0) and p._version > v0
+
+
+def test_pack_key_sees_a_new_storage_at_the_packed_address():
+    """p.data = t keeps p's version counter, and the caching allocator may hand t the address of the storage the last
+    pack read once that storage is freed: (data_ptr, _version) then recurs, but the freed storage's weak reference has
+    expired."""
+    from melgan_multi_b200 import models
+    ps = [torch.nn.Parameter(torch.randn(4)) for _ in range(3)]
+    key = models._PackKey(ps)
+    assert key.matches(ps)
+    ps[1].data = torch.randn(4)  # the packed storage of ps[1] is freed here
+    assert not key.matches(ps)
+    key.key = tuple((t.data_ptr(), t._version) for t in ps)  # as if the new storage had landed at the packed address
+    assert not key.matches(ps)
+    assert models._PackKey(ps).matches(ps)
+
+
+def test_repack_reaches_every_packed_module_inside():
+    from melgan_multi_b200 import models
+    msd = models.MultiScaleDiscriminator()
+    for m in [msd] + list(msd.discriminators):
+        m._packed_key = ("stale",)
+    msd.repack()
+    assert all(m._packed_key is None for m in [msd] + list(msd.discriminators))
+    d = msd.discriminators[1]
+    d._packed_key = msd._packed_key = ("stale",)
+    d.repack()
+    assert d._packed_key is None and msd._packed_key == ("stale",)
+
+
 def test_simt_test_library_is_separate_from_the_product():
     """The first-generation fp32 SIMT generator is test infrastructure: it lives in its own library, and the product
     library neither exports nor contains it."""
