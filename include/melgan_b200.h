@@ -368,11 +368,29 @@ int mg_disc_tc_element(size_t offset, int *copy, int *co, int *ci, int *tap);
  *   mg_mel_spectrogram: audio [B][L] device fp32 in [-1, 1] -> mel [B][n_mels][T] device fp32, T = mg_mel_frames(L)
  *     (= L / 256 when L is a multiple of 256).  Asynchronous on `stream`.  One CTA per item and pair of frames, all on
  *     grid.x: any B works as long as B * ceil(T / 2) <= 2^31 - 1; beyond that MG_ERR_INVALID_ARGUMENT, before any launch.
+ *   mg_mel_spectrogram_backward: the gradient of a loss with respect to the audio, grad_audio = d loss / d audio [B][L]
+ *     device fp32, given grad_mel = d loss / d mel [B][n_mels][T] device fp32, for
+ *       mel = log(clamp(M . |rfft(w . frame_t(pad(audio)))|, min=1e-5))
+ *     (pad: 384 zeros each side; frame_t: padded samples [256 t, 256 t + 1024); w: periodic Hann; M: the tables' filter
+ *     bank), under torch autograd's conventions: the gradient passes where the band's sum s >= 1e-5 and is 0 below it;
+ *     a bin with |X| = 0 contributes 0; the rfft's adjoint runs over bins 0..512 as the forward has them (interior bins
+ *     not doubled); gradients on padding are dropped; samples no frame reaches (the trailing L mod 256 past the last
+ *     frame) get exactly 0.  Every element of grad_audio is written; it may be uninitialised.  The magnitudes and s are
+ *     recomputed with the forward's arithmetic.  Deterministic: no floating-point atomics, each item bit-identical to its
+ *     own B = 1 call.  Asynchronous on `stream`, no host synchronisation (capturable in a CUDA graph).
+ *     workspace: caller-owned device memory, 16-byte aligned, of at least mg_mel_backward_workspace_bytes(B, L) =
+ *     B * mg_mel_frames(L) * 1024 * 4 bytes (0 when B, L or the launch limit are invalid); it holds the per-frame
+ *     gradients for one call, so concurrent calls need their own.  Same limit as the forward (B * ceil(T / 2) <= 2^31 - 1).
+ *     NULL pointers, B < 1, T < 1, misaligned tables or workspace are refused with MG_ERR_INVALID_ARGUMENT, a short
+ *     workspace with MG_ERR_WORKSPACE_TOO_SMALL, before any launch.
  */
 size_t mg_mel_tables_bytes(void);
 int mg_mel_tables_build(int sampling_rate, int n_mels, float fmin, float fmax, int norm, void *tables_host);
 int mg_mel_frames(int L);
 int mg_mel_spectrogram(const void *tables, const float *audio, float *mel, int B, int L, void *stream);
+size_t mg_mel_backward_workspace_bytes(int B, int L);
+int mg_mel_spectrogram_backward(const void *tables, const float *audio, const float *grad_mel, float *grad_audio, int B, int L,
+                                void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
  * Host-buffer engine.   The call a non-PyTorch host makes: owns its device buffers, takes and

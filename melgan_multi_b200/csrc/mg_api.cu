@@ -658,6 +658,18 @@ int mg_mel_spectrogram(const void *tables, const float *audio, float *mel, int B
     return launch_mel(tables, audio, mel, B, L, (cudaStream_t)stream);
 }
 
+size_t mg_mel_backward_workspace_bytes(int B, int L) { return mel_backward_workspace_bytes(B, L); }
+
+int mg_mel_spectrogram_backward(const void *tables, const float *audio, const float *grad_mel, float *grad_audio, int B, int L,
+                                void *workspace, size_t workspace_bytes, void *stream) {
+    const char *fn = "mg_mel_spectrogram_backward";
+    if (!tables || !audio || !grad_mel || !grad_audio || !workspace || B < 1 || L < 1)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: bad argument", fn);
+    if ((uintptr_t)tables % 16) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: tables must be 16-byte aligned", fn);
+    if ((uintptr_t)workspace % 16) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: workspace must be 16-byte aligned", fn);
+    return launch_mel_backward(tables, audio, grad_mel, grad_audio, B, L, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 /* ------------------------------- host-buffer engine ------------------------------------- */
 
 struct mg_gen_engine {

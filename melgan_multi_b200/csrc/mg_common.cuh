@@ -254,6 +254,9 @@ size_t mel_tables_bytes();
 int mel_tables_build(int sr, int n_mels, float fmin, float fmax, int norm, MelTables *t);
 int mel_frames(int L);
 int launch_mel(const void *tables, const float *audio, float *mel, int B, int L, cudaStream_t s);
+size_t mel_backward_workspace_bytes(int B, int L);
+int launch_mel_backward(const void *tables, const float *audio, const float *grad_mel, float *grad_audio, int B, int L,
+                        void *workspace, size_t workspace_bytes, cudaStream_t s);
 int launch_msd_forward(const void *packed, const float *y, int Bt, int L, float *const *fmaps, int *status, cudaStream_t s);
 // batch: lengths and stride of the kernel's input (ConvT) / of the ResBlock itself (the output length for codes 12..14)
 // precision: MG_GEN_PRECISION_FP32 (3-pass split bf16) or MG_GEN_PRECISION_BF16 (one pass; only the default chain's kernels)

@@ -83,21 +83,13 @@ int mel_tables_build(int sr, int n_mels, float fmin, float fmax, int norm, MelTa
 
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 
-__global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ tab, const float *__restrict__ audio,
-                                                  float *__restrict__ mel, int L, int T) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    MelTables *st = reinterpret_cast<MelTables *>(smem_raw);
-    float2 *buf = reinterpret_cast<float2 *>(smem_raw + ((sizeof(MelTables) + 15) / 16) * 16);  // [2 frames][2 buffers][512]
-    float *mag = reinterpret_cast<float *>(buf + 2 * 2 * 512);                                     // [2 frames][513 (+3)]
-    const int tid = threadIdx.x, fr = tid >> 7, lt = tid & 127;
-    const int pairs = (T + 1) >> 1;  // grid.x = items x frame pairs: a batch is not limited by grid.y's 65535
-    const int b = (int)blockIdx.x / pairs, t = 2 * ((int)blockIdx.x - b * pairs) + fr;
-    for (int i = tid; i < (int)(sizeof(MelTables) / 4); i += 256) reinterpret_cast<uint32_t *>(st)[i] = reinterpret_cast<const uint32_t *>(tab)[i];
-    __syncthreads();
-    const bool live = t < T;
-    float2 *A = buf + fr * 1024, *Bf = A + 512;
+// Frame t of item xb (128 threads, lt = 0..127, of a 256-thread CTA that calls this together: it holds __syncthreads):
+// windowed 512-point complex Stockham FFT in A / Bf, split into the 513 bins of the real transform; mg[k] = |X[k]|, and
+// X[k] itself when Xk is given.  The forward and the backward both run it, so the backward differentiates the very
+// magnitudes the forward summed.
+__device__ __forceinline__ void mel_frame_bins(const MelTables *st, const float *xb, int L, int t, bool live, int lt, float2 *A,
+                                               float2 *Bf, float *mg, float2 *Xk) {
     // windowed frame, even samples -> real part, odd -> imaginary; sample index in the UNPADDED signal: t*hop - 384 + n
-    const float *xb = audio + (size_t)b * L;
     for (int n = lt; n < 512; n += 128) {
         const int i0 = t * kMelHop - kMelPad + 2 * n;
         const float x0 = (live && i0 >= 0 && i0 < L) ? __ldg(xb + i0) : 0.f;
@@ -122,7 +114,6 @@ __global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ 
         float2 *tmp = in; in = out; out = tmp;
     }
     // Z = in: bins of the real transform, X[k] = E[k] + e^{-2 pi i k / 1024} O[k], E = (Z[k] + conj Z[512-k]) / 2, O = (Z[k] - conj Z[512-k]) / 2i
-    float *mg = mag + fr * 516;
     for (int k = lt; k <= 512; k += 128) {
         const float2 zk = in[k & 511], zc = in[(512 - k) & 511];
         const float2 E = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y - zc.y));
@@ -130,14 +121,151 @@ __global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ 
         const float2 w = k < 512 ? st->tw[k] : make_float2(-1.f, 0.f);
         const float2 X = make_float2(E.x + w.x * O.x - w.y * O.y, E.y + w.x * O.y + w.y * O.x);
         mg[k] = sqrtf(X.x * X.x + X.y * X.y);  // power = 1 (meldataset.py:50)
+        if (Xk) Xk[k] = X;
     }
     __syncthreads();
-    if (live && lt < st->n_mels) {
-        const int ks = st->kstart[lt], kc = st->kcount[lt];
-        const float *w = st->weights + st->woff[lt];
-        float s = 0.f;
-        for (int i = 0; i < kc; ++i) s = fmaf(w[i], mg[ks + i], s);
-        mel[((size_t)b * st->n_mels + lt) * T + t] = logf(fmaxf(s, 1e-5f));  // meldataset.py:19-25: log(clip(x, 1e-5) * 1)
+}
+
+// mel band m before the log: the fma dot product of its sparse filter run with the magnitudes
+__device__ __forceinline__ float mel_band_sum(const MelTables *st, const float *mg, int m) {
+    const int ks = st->kstart[m], kc = st->kcount[m];
+    const float *w = st->weights + st->woff[m];
+    float s = 0.f;
+    for (int i = 0; i < kc; ++i) s = fmaf(w[i], mg[ks + i], s);
+    return s;
+}
+
+__global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ tab, const float *__restrict__ audio,
+                                                  float *__restrict__ mel, int L, int T) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    MelTables *st = reinterpret_cast<MelTables *>(smem_raw);
+    float2 *buf = reinterpret_cast<float2 *>(smem_raw + ((sizeof(MelTables) + 15) / 16) * 16);  // [2 frames][2 buffers][512]
+    float *mag = reinterpret_cast<float *>(buf + 2 * 2 * 512);                                     // [2 frames][513 (+3)]
+    const int tid = threadIdx.x, fr = tid >> 7, lt = tid & 127;
+    const int pairs = (T + 1) >> 1;  // grid.x = items x frame pairs: a batch is not limited by grid.y's 65535
+    const int b = (int)blockIdx.x / pairs, t = 2 * ((int)blockIdx.x - b * pairs) + fr;
+    for (int i = tid; i < (int)(sizeof(MelTables) / 4); i += 256) reinterpret_cast<uint32_t *>(st)[i] = reinterpret_cast<const uint32_t *>(tab)[i];
+    __syncthreads();
+    const bool live = t < T;
+    float2 *A = buf + fr * 1024;
+    float *mg = mag + fr * 516;
+    mel_frame_bins(st, audio + (size_t)b * L, L, t, live, lt, A, A + 512, mg, nullptr);
+    if (live && lt < st->n_mels)
+        mel[((size_t)b * st->n_mels + lt) * T + t] = logf(fmaxf(mel_band_sum(st, mg, lt), 1e-5f));  // meldataset.py:19-25: log(clip(x, 1e-5) * 1)
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Backward: grad_audio = d loss / d audio given grad_mel = d loss / d mel, torch autograd's conventions (clamp(min=)
+// passes where s >= 1e-5, |0| has gradient 0, the rfft adjoint over bins 0..512 as the forward has them, padding dropped).
+//
+// mel_backward_frame_kernel, same CTA geometry as mel_kernel, per frame:
+//   recompute X and s with the forward's arithmetic  ->  gs_m = g_m / s_m (0 below the clip)  ->  dmag = M^T gs (filters
+//   of one parity never share a bin -- each triangle ends where the next-but-one starts -- so two passes, even then odd,
+//   accumulate without atomics)  ->  G[k] = dmag_k X_k / |X_k|  ->  adjoint of the even/odd split into dZ[0..511]  ->
+//   512-point inverse Stockham FFT (conjugate twiddles, unnormalised)  ->  times the window  ->  dframe[b][t][1024].
+// mel_backward_ola_kernel: grad_audio[b][i] = sum over the <= 4 frames covering padded sample i + 384, ascending t.
+//
+// Adjoint of the split, with a_k = (1 - i W^k) / 2, b_k = (1 + i W^k) / 2 (W^k = tw[k], W^512 = -1), X[k] = a_k Z[k & 511] +
+// b_k conj Z[(512 - k) & 511]:  dZ[j] = P(j) + Q((512 - j) & 511), P(k) = conj(a_k) G[k], Q(k) = b_k conj G[k]; dZ[0] also
+// takes P(512) + Q(512), the Nyquist bin's share.
+// ---------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float2 split_adjoint(const float2 G, const float2 w) {  // conj(a) G, w = W^k
+    return make_float2(0.5f * (G.x + w.y * G.x - w.x * G.y), 0.5f * (G.y + w.x * G.x + w.y * G.y));
+}
+__device__ __forceinline__ float2 split_adjoint_conj(const float2 G, const float2 w) {  // b conj(G)
+    return make_float2(0.5f * (G.x - w.y * G.x + w.x * G.y), 0.5f * (-G.y + w.x * G.x + w.y * G.y));
+}
+
+__global__ void __launch_bounds__(256) mel_backward_frame_kernel(const MelTables *__restrict__ tab, const float *__restrict__ audio,
+                                                                 const float *__restrict__ grad_mel, float *__restrict__ dframe,
+                                                                 int L, int T) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    MelTables *st = reinterpret_cast<MelTables *>(smem_raw);
+    float2 *buf = reinterpret_cast<float2 *>(smem_raw + ((sizeof(MelTables) + 15) / 16) * 16);  // [2 frames][2 buffers][512]
+    float2 *Xall = buf + 2 * 2 * 512;                                                             // [2 frames][513 (+3)]
+    float *mag = reinterpret_cast<float *>(Xall + 2 * 516);                                       // [2 frames][513 (+3)]
+    float *dmag = mag + 2 * 516;                                                                  // [2 frames][513 (+3)]
+    const int tid = threadIdx.x, fr = tid >> 7, lt = tid & 127;
+    const int pairs = (T + 1) >> 1;
+    const int b = (int)blockIdx.x / pairs, t = 2 * ((int)blockIdx.x - b * pairs) + fr;
+    for (int i = tid; i < (int)(sizeof(MelTables) / 4); i += 256) reinterpret_cast<uint32_t *>(st)[i] = reinterpret_cast<const uint32_t *>(tab)[i];
+    __syncthreads();
+    const bool live = t < T;
+    float2 *A = buf + fr * 1024, *Xk = Xall + fr * 516;
+    float *mg = mag + fr * 516, *dm = dmag + fr * 516;
+    mel_frame_bins(st, audio + (size_t)b * L, L, t, live, lt, A, A + 512, mg, Xk);
+    const int n_mels = st->n_mels;
+    float gs = 0.f;
+    if (live && lt < n_mels) {
+        const float s = mel_band_sum(st, mg, lt);
+        gs = s >= 1e-5f ? __ldg(grad_mel + ((size_t)b * n_mels + lt) * T + t) / s : 0.f;  // log' = 1 / s; clamp(min=)' = [s >= min]
+    }
+    for (int k = lt; k <= 512; k += 128) dm[k] = 0.f;
+    __syncthreads();
+#pragma unroll 1
+    for (int parity = 0; parity < 2; ++parity) {
+        if (lt < n_mels && (lt & 1) == parity) {
+            const int ks = st->kstart[lt], kc = st->kcount[lt];
+            const float *w = st->weights + st->woff[lt];
+            for (int i = 0; i < kc; ++i) dm[ks + i] = fmaf(w[i], gs, dm[ks + i]);
+        }
+        __syncthreads();
+    }
+    for (int k = lt; k <= 512; k += 128) {  // abs' = X / |X|, and 0 at X = 0
+        const float m = mg[k], r = m > 0.f ? dm[k] / m : 0.f;
+        Xk[k] = make_float2(r * Xk[k].x, r * Xk[k].y);
+    }
+    __syncthreads();
+    float2 *in = A, *out = A + 512;
+    for (int j = lt; j < 512; j += 128) {
+        const int jc = (512 - j) & 511;
+        const float2 p = split_adjoint(Xk[j], st->tw[j]), q = split_adjoint_conj(Xk[jc], st->tw[jc]);
+        float2 d = make_float2(p.x + q.x, p.y + q.y);
+        if (j == 0) {  // the Nyquist bin reads Z[0] as well: P(512) + Q(512), W^512 = -1
+            const float2 p5 = split_adjoint(Xk[512], make_float2(-1.f, 0.f)), q5 = split_adjoint_conj(Xk[512], make_float2(-1.f, 0.f));
+            d = make_float2(d.x + (p5.x + q5.x), d.y + (p5.y + q5.y));
+        }
+        in[j] = d;
+    }
+    __syncthreads();
+    // inverse transform: the forward's Stockham passes with conjugate twiddles, e^{+2 pi i k / (2 ns)}, no 1/512
+#pragma unroll 1
+    for (int ns = 1; ns < 512; ns <<= 1) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int j = lt + 128 * r;
+            const int k = j & (ns - 1);
+            const float2 tw = st->tw[k * (512 / ns)];
+            const float2 v0 = in[j], v1 = cmul(in[j + 256], make_float2(tw.x, -tw.y));
+            const int j0 = ((j - k) << 1) + k;
+            out[j0] = make_float2(v0.x + v1.x, v0.y + v1.y);
+            out[j0 + ns] = make_float2(v0.x - v1.x, v0.y - v1.y);
+        }
+        __syncthreads();
+        float2 *tmp = in; in = out; out = tmp;
+    }
+    if (!live) return;
+    // dz[n] = d/dRe z[n] + i d/dIm z[n], z[n] = w[2n] x[2n] + i w[2n+1] x[2n+1]
+    float2 *df = reinterpret_cast<float2 *>(dframe + ((size_t)b * T + t) * kMelNfft);
+    for (int n = lt; n < 512; n += 128) df[n] = make_float2(st->win[2 * n] * in[n].x, st->win[2 * n + 1] * in[n].y);
+}
+
+// one CTA = 1024 consecutive samples of one item; each sample gathers the frames that read it, ascending t, so the sum is
+// the same bits in every run and for every batch layout.  Every sample in [0, L) is written (0 where no frame reaches).
+__global__ void __launch_bounds__(256) mel_backward_ola_kernel(const float *__restrict__ dframe, float *__restrict__ grad_audio,
+                                                               int L, int T) {
+    const int chunks = (L + 1023) >> 10;
+    const int b = (int)blockIdx.x / chunks, c = (int)blockIdx.x - b * chunks;
+    const float *db = dframe + (size_t)b * T * kMelNfft;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int i = (c << 10) + 256 * r + (int)threadIdx.x;
+        if (i >= L) break;
+        const int p = i + kMelPad;                     // index in the padded signal; frame t covers [256 t, 256 t + 1024)
+        const int t1 = min(p / kMelHop, T - 1), t0 = p >= kMelNfft ? (p - kMelNfft) / kMelHop + 1 : 0;
+        float acc = 0.f;
+        for (int t = t0; t <= t1; ++t) acc += __ldg(db + (size_t)t * kMelNfft + (p - t * kMelHop));
+        grad_audio[(size_t)b * L + i] = acc;
     }
 }
 
@@ -156,6 +284,37 @@ int launch_mel(const void *tables, const float *audio, float *mel, int B, int L,
         configured = true;
     }
     mel_kernel<<<(unsigned)ctas, 256, smem, s>>>(reinterpret_cast<const MelTables *>(tables), audio, mel, L, T);
+    MG_CUDA_TRY(cudaGetLastError());
+    return MG_OK;
+}
+
+size_t mel_backward_workspace_bytes(int B, int L) {
+    const int T = L < 1 ? 0 : mel_frames(L);
+    if (B < 1 || T < 1 || (long long)B * ((T + 1) / 2) > 0x7fffffffll) return 0;
+    return (size_t)B * T * kMelNfft * sizeof(float);
+}
+
+int launch_mel_backward(const void *tables, const float *audio, const float *grad_mel, float *grad_audio, int B, int L,
+                        void *workspace, size_t workspace_bytes, cudaStream_t s) {
+    const int T = mel_frames(L);
+    if (T < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_mel_spectrogram_backward: %d samples are fewer than one frame", L);
+    const long long ctas = (long long)B * ((T + 1) / 2);
+    if (ctas > 0x7fffffffll)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "mg_mel_spectrogram_backward: B=%d x %d frame pairs exceed 2^31 - 1 CTAs", B, (T + 1) / 2);
+    const size_t need = mel_backward_workspace_bytes(B, L);
+    if (workspace_bytes < need)
+        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "mg_mel_spectrogram_backward: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+    constexpr int smem = ((sizeof(MelTables) + 15) / 16) * 16 + 2 * 2 * 512 * 8 + 2 * 516 * 8 + 2 * 2 * 516 * 4;
+    static bool configured = false;
+    if (!configured) {
+        MG_CUDA_TRY(cudaFuncSetAttribute(mel_backward_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        configured = true;
+    }
+    float *dframe = reinterpret_cast<float *>(workspace);
+    mel_backward_frame_kernel<<<(unsigned)ctas, 256, smem, s>>>(reinterpret_cast<const MelTables *>(tables), audio, grad_mel, dframe, L, T);
+    MG_CUDA_TRY(cudaGetLastError());
+    // B * ceil(L / 1024) <= B * ceil(T / 2) CTAs: L < 256 (T + 1) gives L / 1024 < (T + 1) / 4
+    mel_backward_ola_kernel<<<(unsigned)((long long)B * ((L + 1023) / 1024)), 256, 0, s>>>(dframe, grad_audio, L, T);
     MG_CUDA_TRY(cudaGetLastError());
     return MG_OK;
 }
