@@ -24,35 +24,25 @@ static int run_generator(const float *mel, void *audio, const RunTable &batch, f
     return launch_generator_tc(mel, audio, batch, ws, st, s, ev, mel_host, audio_host, precision, pcm16);
 }
 
-// a known precision, and bf16 only on the default chain (the only one with single-pass kernels)
-static int check_precision(const char *fn, int precision) {
+int check_precision(const char *fn, int precision) {
     if (precision != MG_GEN_PRECISION_FP32 && precision != MG_GEN_PRECISION_BF16)
         return set_error(MG_ERR_INVALID_ARGUMENT, "%s: unknown precision %d (MG_GEN_PRECISION_FP32 = 0, MG_GEN_PRECISION_BF16 = 1)", fn,
                          precision);
-    if (precision == MG_GEN_PRECISION_BF16 && !generator_tc_default_chain())
+    return MG_OK;
+}
+
+int check_default_chain(const char *fn, const char *role) {
+    if (!generator_tc_default_chain())
         return set_error(MG_ERR_INVALID_ARGUMENT,
-                         "%s: bf16 runs on the default chain only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected "
-                         "another (tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
-                         fn, generator_tc_tail(), generator_tc_fused_up());
+                         "%s: %s only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected another (tail mask %d, "
+                         "front mask %d); mg_gen_set_pipeline(-1) restores the default",
+                         fn, role, generator_tc_tail(), generator_tc_fused_up());
     return MG_OK;
 }
 
 static int check_shape(const char *fn, int B, int T) {
     if (B < 1 || T < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: need B >= 1 and T >= 1 (got B=%d, T=%d)", fn, B, T);
     if ((long long)B * T > (1ll << 24)) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: B*T = %lld too large", fn, (long long)B * T);
-    return MG_OK;
-}
-
-// the ragged entry points' own arguments: B within the parameter tables' capacity, every length in [1, T_max]
-static int check_lengths(const char *fn, int B, int T_max, const int *lengths) {
-    int rc = check_shape(fn, B, T_max);
-    if (rc) return rc;
-    if (B > MG_GEN_RAGGED_MAX_B)
-        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: B = %d exceeds MG_GEN_RAGGED_MAX_B = %d", fn, B, MG_GEN_RAGGED_MAX_B);
-    if (!lengths) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null lengths", fn);
-    for (int i = 0; i < B; ++i)
-        if (lengths[i] < 1 || lengths[i] > T_max)
-            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: lengths[%d] = %d is outside [1, T_max = %d]", fn, i, lengths[i], T_max);
     return MG_OK;
 }
 
@@ -77,6 +67,183 @@ static int run_one_kernel(const char *fn, cudaStream_t stream, F launch) {
 }  // namespace mg
 
 using namespace mg;
+
+/* ------------------------------- host-buffer engine ------------------------------------- */
+
+struct mg_gen_engine {
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    float *packed = nullptr;
+    float *raw = nullptr;  // device staging for raw v/g/bias
+    float *mel = nullptr, *audio = nullptr, *ws = nullptr;
+    float *pin_in = nullptr, *pin_out = nullptr;  // (audio and pin_out hold int16 samples after a pcm16 forward)
+    int *pin_status = nullptr;
+    size_t cap_frames = 0;  // B*T capacity
+    bool loaded = false;
+    float last_ms = 0.f;
+};
+
+static void engine_free_io(mg_gen_engine *e) {
+    cudaFree(e->mel); cudaFree(e->audio); cudaFree(e->ws);
+    cudaFreeHost(e->pin_in); cudaFreeHost(e->pin_out);
+    e->mel = e->audio = e->ws = e->pin_in = e->pin_out = nullptr;
+    e->cap_frames = 0;
+}
+
+static int engine_reserve(mg_gen_engine *e, size_t frames) {
+    if (frames <= e->cap_frames) return MG_OK;
+    engine_free_io(e);
+    MG_CUDA_TRY(cudaMalloc(&e->mel, frames * kMelBins * sizeof(float)));
+    MG_CUDA_TRY(cudaMalloc(&e->audio, frames * 256 * sizeof(float)));
+    MG_CUDA_TRY(cudaMalloc(&e->ws, mg_gen_workspace_bytes(1, (int)frames)));
+    MG_CUDA_TRY(cudaMallocHost(&e->pin_in, frames * kMelBins * sizeof(float)));
+    MG_CUDA_TRY(cudaMallocHost(&e->pin_out, frames * 256 * sizeof(float)));
+    e->cap_frames = frames;
+    return MG_OK;
+}
+
+// pcm16: audio_host receives int16 samples; the device audio and the pinned staging are then read as int16, so the
+// download moves half the bytes
+static int engine_forward(mg_gen_engine *e, const float *mel_host, void *audio_host, const RunTable &batch,
+                          int precision = MG_GEN_PRECISION_FP32, bool pcm16 = false) {
+    const int B = batch.items(), T = batch.stride;
+    const size_t frames = (size_t)B * T;
+    int rc = engine_reserve(e, frames);
+    if (rc) return rc;
+    const size_t nin = frames * kMelBins * sizeof(float), nout = frames * 256 * (pcm16 ? sizeof(int16_t) : sizeof(float));
+    cudaPointerAttributes at;
+    const bool in_pinned = cudaPointerGetAttributes(&at, mel_host) == cudaSuccess && at.type == cudaMemoryTypeHost;
+    const bool out_pinned = cudaPointerGetAttributes(&at, audio_host) == cudaSuccess && at.type == cudaMemoryTypeHost;
+    cudaGetLastError();  // clear "invalid value" some drivers raise for pageable pointers
+    const float *src = mel_host;
+    if (!in_pinned) { memcpy(e->pin_in, mel_host, nin); src = e->pin_in; }
+    if (!e->pin_status) MG_CUDA_TRY(cudaMallocHost(&e->pin_status, sizeof(int)));
+    MG_CUDA_TRY(cudaEventRecord(e->ev0, e->stream));
+    // upload, kernels and download are enqueued per batch slice (launch_generator_tc); one synchronisation at the end
+    rc = run_generator(e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : (void *)e->pin_out,
+                       precision, pcm16);
+    if (rc) return rc;
+    MG_CUDA_TRY(cudaEventRecord(e->ev1, e->stream));
+    *e->pin_status = 0;
+    MG_CUDA_TRY(cudaMemcpyAsync(e->pin_status, status_ptr(e->ws, B, T), sizeof(int), cudaMemcpyDeviceToHost, e->stream));
+    MG_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    if (!out_pinned) memcpy(audio_host, e->pin_out, nout);
+    if (*e->pin_status)
+        return set_error(MG_ERR_CUDA, "mg_gen_engine_forward: tensor-core pipeline wait timed out (code %d)", *e->pin_status);
+    MG_CUDA_TRY(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
+    return MG_OK;
+}
+
+/* ------------------------------- generator forward -------------------------------------- */
+
+namespace mg {
+
+// What a forward entry point asks of the shared rules beyond those every one applies (ForwardCall::rules)
+enum : unsigned {
+    kBlobArray = 1,         // packed is the caller's array of n_voices blobs, each checked ("packed[i] is NULL")
+    kNeedVoice = 2,         // voice must not be NULL
+    kNeedLengths = 4,       // lengths must not be NULL
+    kDefaultChainOnly = 8,  // any other chain is refused at fp32 too (the multi-voice and int16 kernels exist only there)
+    kPcm16 = 16,            // audio holds int16 samples
+    kHost = 32,             // mel and audio are host buffers; engine holds the weights and the workspace
+};
+
+// One generator forward as an entry point received it.  The device-pointer entry points pass packed, ws, ws_bytes and
+// stream (a single-pointer one passes its pointer's address and n_voices = 1); the host-buffer ones pass engine.
+struct ForwardCall {
+    const char *fn;
+    unsigned rules;
+    const void *const *packed;
+    int n_voices;
+    const int *voice;
+    const float *mel;
+    void *audio;
+    int B, T;
+    const int *lengths;
+    int precision;
+    void *ws;
+    size_t ws_bytes;
+    void *stream;
+    mg_gen_engine *engine;
+};
+
+// The rules of every generator forward in the order they are checked; the first one broken is reported, before any CUDA
+// call:
+//   1. precision is MG_GEN_PRECISION_FP32 or MG_GEN_PRECISION_BF16;
+//   2. the chain is the default one, at bf16 or under kDefaultChainOnly;
+//   3. kBlobArray: n_voices >= 1, packed (and voice, kNeedVoice) not NULL, every blob non-NULL and 16-byte aligned;
+//   4. B >= 1, T >= 1, B*T <= 2^24;
+//   5. lengths not NULL (kNeedLengths); without voice ids a ragged batch has at most MG_GEN_RAGGED_MAX_B items; item by
+//      item, voice[i] in [0, n_voices) and lengths[i] in [1, T];
+//   6. with voice ids, at most MG_GEN_RAGGED_MAX_B runs of equal length and voice;
+//   7. device calls: packed, mel, audio and workspace not NULL, a workspace of mg_gen_workspace_bytes(B, T) bytes
+//      (else MG_ERR_WORKSPACE_TOO_SMALL), packed and workspace 16-byte aligned; host-buffer calls: engine, mel and audio
+//      not NULL, weights loaded.
+static int check_forward(const ForwardCall &c) {
+    const char *fn = c.fn;
+    const bool bf16 = c.precision == MG_GEN_PRECISION_BF16;
+    int rc = check_precision(fn, c.precision);
+    if (!rc && (bf16 || (c.rules & kDefaultChainOnly)))
+        rc = check_default_chain(fn, bf16 ? "bf16 runs on the default chain" : "runs the default chain");
+    if (rc) return rc;
+    if (c.rules & kBlobArray) {
+        if (c.n_voices < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, c.n_voices);
+        if (!c.packed || ((c.rules & kNeedVoice) && !c.voice))
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null packed%s array", fn, c.rules & kNeedVoice ? " or voice" : "");
+        for (int v = 0; v < c.n_voices; ++v) {
+            if (!c.packed[v]) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] is NULL", fn, v);
+            if ((uintptr_t)c.packed[v] % 16) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] must be 16-byte aligned", fn, v);
+        }
+    }
+    if ((rc = check_shape(fn, c.B, c.T))) return rc;
+    if ((c.rules & kNeedLengths) && !c.lengths) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null lengths", fn);
+    if (c.lengths && !c.voice && c.B > MG_GEN_RAGGED_MAX_B)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: B = %d exceeds MG_GEN_RAGGED_MAX_B = %d", fn, c.B, MG_GEN_RAGGED_MAX_B);
+    for (int i = 0; (c.voice || c.lengths) && i < c.B; ++i) {
+        if (c.voice && (c.voice[i] < 0 || c.voice[i] >= c.n_voices))
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: voice[%d] = %d is outside [0, n_voices = %d)", fn, i, c.voice[i],
+                             c.n_voices);
+        if (c.lengths && (c.lengths[i] < 1 || c.lengths[i] > c.T))
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: lengths[%d] = %d is outside [1, T_max = %d]", fn, i, c.lengths[i], c.T);
+    }
+    if (c.voice) {
+        int runs = 1;  // what RunTable::voices merges: neighbours of equal length and blob
+        for (int i = 1; i < c.B; ++i)
+            runs += (c.lengths && c.lengths[i] != c.lengths[i - 1]) || c.packed[c.voice[i]] != c.packed[c.voice[i - 1]];
+        if (runs > MG_GEN_RAGGED_MAX_B)
+            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %d runs of equal length and voice exceed MG_GEN_RAGGED_MAX_B = %d", fn,
+                             runs, MG_GEN_RAGGED_MAX_B);
+    }
+    if (c.rules & kHost) {
+        if (!c.engine || !c.mel || !c.audio) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
+        if (!c.engine->loaded) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: no weights loaded", fn);
+        return MG_OK;
+    }
+    if (!c.packed[0] || !c.mel || !c.audio || !c.ws) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
+    const size_t need = mg_gen_workspace_bytes(c.B, c.T);
+    if (c.ws_bytes < need) return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "%s: workspace %zu < %zu bytes", fn, c.ws_bytes, need);
+    if ((uintptr_t)c.packed[0] % 16 || (uintptr_t)c.ws % 16)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed/workspace must be 16-byte aligned", fn);
+    return MG_OK;
+}
+
+// the batch table of a call check_forward accepted
+static RunTable batch_table(const ForwardCall &c) {
+    const float *const *blobs = c.rules & kHost ? &c.engine->packed : reinterpret_cast<const float *const *>(c.packed);
+    if (c.voice) return RunTable::voices(c.lengths, c.B, c.T, blobs, c.voice);
+    return c.lengths ? RunTable::ragged(c.lengths, c.B, c.T, blobs[0]) : RunTable::uniform(c.B, c.T, blobs[0]);
+}
+
+static int forward(const ForwardCall &c) {
+    int rc = check_forward(c);
+    if (rc) return rc;
+    const RunTable t = batch_table(c);
+    const bool pcm16 = c.rules & kPcm16;
+    if (c.rules & kHost) return engine_forward(c.engine, c.mel, c.audio, t, c.precision, pcm16);
+    return run_generator(c.mel, c.audio, t, (float *)c.ws, (cudaStream_t)c.stream, nullptr, nullptr, nullptr, c.precision, pcm16);
+}
+
+}  // namespace mg
 
 extern "C" {
 
@@ -108,135 +275,46 @@ size_t mg_gen_workspace_bytes(int B, int T) {
     return ws_offset(6, (size_t)B, (size_t)T) * sizeof(float) + 256;  // + pipeline status word
 }
 
-static int check_forward(const char *fn, const void *packed, const float *mel, const void *audio, int B, int T, void *workspace,
-                         size_t workspace_bytes) {
-    if (!packed || !mel || !audio || !workspace) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
-    if (workspace_bytes < mg_gen_workspace_bytes(B, T))
-        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "%s: workspace %zu < %zu bytes", fn, workspace_bytes, mg_gen_workspace_bytes(B, T));
-    if ((uintptr_t)packed % 16 || (uintptr_t)workspace % 16)
-        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed/workspace must be 16-byte aligned", fn);
-    return MG_OK;
-}
-
 int mg_gen_forward(const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
                    size_t workspace_bytes, void *stream) {
-    int rc = check_shape("mg_gen_forward", B, T);
-    if (!rc) rc = check_forward("mg_gen_forward", packed, mel, audio, B, T, workspace, workspace_bytes);
-    if (rc) return rc;
-    return run_generator(mel, audio, RunTable::uniform(B, T, (const float *)packed), (float *)workspace, (cudaStream_t)stream,
-                         nullptr);
+    return forward({"mg_gen_forward", 0, &packed, 1, nullptr, mel, audio, B, T, nullptr, MG_GEN_PRECISION_FP32, workspace,
+                    workspace_bytes, stream});
 }
 
 int mg_gen_forward_ragged(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
                           void *workspace, size_t workspace_bytes, void *stream) {
-    int rc = check_lengths("mg_gen_forward_ragged", B, T_max, lengths);
-    if (!rc) rc = check_forward("mg_gen_forward_ragged", packed, mel, audio, B, T_max, workspace, workspace_bytes);
-    if (rc) return rc;
-    return run_generator(mel, audio, RunTable::ragged(lengths, B, T_max, (const float *)packed), (float *)workspace,
-                         (cudaStream_t)stream, nullptr);
+    return forward({"mg_gen_forward_ragged", kNeedLengths, &packed, 1, nullptr, mel, audio, B, T_max, lengths,
+                    MG_GEN_PRECISION_FP32, workspace, workspace_bytes, stream});
 }
 
 int mg_gen_forward_precision(const void *packed, const float *mel, float *audio, int B, int T_max, const int *lengths,
                              int precision, void *workspace, size_t workspace_bytes, void *stream) {
-    const char *fn = "mg_gen_forward_precision";
-    int rc = check_precision(fn, precision);
-    if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
-    if (!rc) rc = check_forward(fn, packed, mel, audio, B, T_max, workspace, workspace_bytes);
-    if (rc) return rc;
-    const float *w = (const float *)packed;
-    return run_generator(mel, audio, lengths ? RunTable::ragged(lengths, B, T_max, w) : RunTable::uniform(B, T_max, w),
-                         (float *)workspace, (cudaStream_t)stream, nullptr, nullptr, nullptr, precision);
-}
-
-static int check_default_chain(const char *fn) {
-    if (!generator_tc_default_chain())
-        return set_error(MG_ERR_INVALID_ARGUMENT,
-                         "%s: runs the default chain only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected another "
-                         "(tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
-                         fn, generator_tc_tail(), generator_tc_fused_up());
-    return MG_OK;
-}
-
-// mg_gen_forward_voices' checks (no CUDA call), then its batch table in t
-static int check_voices(const char *fn, const void *const *packed, int n_voices, const int *voice, const float *mel,
-                        const void *audio, int B, int T_max, const int *lengths, int precision, void *workspace,
-                        size_t workspace_bytes, RunTable &t) {
-    int rc = check_precision(fn, precision);
-    if (!rc) rc = check_default_chain(fn);
-    if (rc) return rc;
-    if (n_voices < 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, n_voices);
-    if (!packed || !voice) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null packed or voice array", fn);
-    for (int v = 0; v < n_voices; ++v) {
-        if (!packed[v]) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] is NULL", fn, v);
-        if ((uintptr_t)packed[v] % 16) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] must be 16-byte aligned", fn, v);
-    }
-    if ((rc = check_shape(fn, B, T_max))) return rc;
-    for (int i = 0; i < B; ++i) {
-        if (voice[i] < 0 || voice[i] >= n_voices)
-            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: voice[%d] = %d is outside [0, n_voices = %d)", fn, i, voice[i], n_voices);
-        if (lengths && (lengths[i] < 1 || lengths[i] > T_max))
-            return set_error(MG_ERR_INVALID_ARGUMENT, "%s: lengths[%d] = %d is outside [1, T_max = %d]", fn, i, lengths[i], T_max);
-    }
-    const float *const *blobs = reinterpret_cast<const float *const *>(packed);
-    int runs = 1;  // what RunTable::voices merges: neighbours of equal length and blob
-    for (int i = 1; i < B; ++i)
-        runs += (lengths && lengths[i] != lengths[i - 1]) || blobs[voice[i]] != blobs[voice[i - 1]];
-    if (runs > MG_GEN_RAGGED_MAX_B)
-        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %d runs of equal length and voice exceed MG_GEN_RAGGED_MAX_B = %d", fn, runs,
-                         MG_GEN_RAGGED_MAX_B);
-    if ((rc = check_forward(fn, packed[0], mel, audio, B, T_max, workspace, workspace_bytes))) return rc;
-    t = RunTable::voices(lengths, B, T_max, blobs, voice);
-    return MG_OK;
+    return forward({"mg_gen_forward_precision", 0, &packed, 1, nullptr, mel, audio, B, T_max, lengths, precision, workspace,
+                    workspace_bytes, stream});
 }
 
 int mg_gen_forward_voices(const void *const *packed, int n_voices, const int *voice, const float *mel, float *audio, int B,
                           int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream) {
-    RunTable t;
-    int rc = check_voices("mg_gen_forward_voices", packed, n_voices, voice, mel, audio, B, T_max, lengths, precision, workspace,
-                          workspace_bytes, t);
-    if (rc) return rc;
-    return run_generator(mel, audio, t, (float *)workspace, (cudaStream_t)stream, nullptr, nullptr, nullptr, precision);
+    return forward({"mg_gen_forward_voices", kBlobArray | kNeedVoice | kDefaultChainOnly, packed, n_voices, voice, mel, audio, B,
+                    T_max, lengths, precision, workspace, workspace_bytes, stream});
 }
 
 int mg_gen_forward_pcm16(const void *const *packed, int n_voices, const int *voice, const float *mel, int16_t *audio, int B,
                          int T_max, const int *lengths, int precision, void *workspace, size_t workspace_bytes, void *stream) {
-    const char *fn = "mg_gen_forward_pcm16";
-    RunTable t;
-    int rc;
-    if (voice) {  // mg_gen_forward_voices' rules
-        rc = check_voices(fn, packed, n_voices, voice, mel, audio, B, T_max, lengths, precision, workspace, workspace_bytes, t);
-    } else {  // every item on voice 0: mg_gen_forward_precision's rules, on the default chain
-        rc = check_precision(fn, precision);
-        if (!rc) rc = check_default_chain(fn);
-        if (!rc && n_voices < 1) rc = set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_voices = %d, need at least 1", fn, n_voices);
-        if (!rc && !packed) rc = set_error(MG_ERR_INVALID_ARGUMENT, "%s: null packed array", fn);
-        for (int v = 0; !rc && v < n_voices; ++v) {
-            if (!packed[v]) rc = set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] is NULL", fn, v);
-            else if ((uintptr_t)packed[v] % 16) rc = set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] must be 16-byte aligned", fn, v);
-        }
-        if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
-        if (!rc) rc = check_forward(fn, packed[0], mel, audio, B, T_max, workspace, workspace_bytes);
-        if (!rc) {
-            const float *w = (const float *)packed[0];
-            t = lengths ? RunTable::ragged(lengths, B, T_max, w) : RunTable::uniform(B, T_max, w);
-        }
-    }
-    if (rc) return rc;
-    return run_generator(mel, audio, t, (float *)workspace, (cudaStream_t)stream, nullptr, nullptr, nullptr, precision, true);
+    return forward({"mg_gen_forward_pcm16", kBlobArray | kDefaultChainOnly | kPcm16, packed, n_voices, voice, mel, audio, B,
+                    T_max, lengths, precision, workspace, workspace_bytes, stream});
 }
 
 int mg_gen_forward_timed(const void *packed, const float *mel, float *audio, int B, int T, void *workspace,
                          size_t workspace_bytes, void *stream, float *kernel_ms) {
-    int rc = check_shape("mg_gen_forward_timed", B, T);
+    const ForwardCall c{"mg_gen_forward_timed", 0, &packed, 1, nullptr, mel, audio, B, T, nullptr, MG_GEN_PRECISION_FP32,
+                        workspace, workspace_bytes, stream};
+    int rc = kernel_ms ? check_forward(c) : set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_forward_timed: null argument");
     if (rc) return rc;
-    if (!packed || !mel || !audio || !workspace || !kernel_ms)
-        return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_forward_timed: null argument");
-    if (workspace_bytes < mg_gen_workspace_bytes(B, T))
-        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "mg_gen_forward_timed: workspace too small");
     const int n = mg_gen_forward_launches();  // events: one before each launch + one after the last
     cudaEvent_t ev[17];  // at most 12 kernels
     for (int i = 0; i <= n; ++i) MG_CUDA_TRY(cudaEventCreate(&ev[i]));
-    rc = run_generator(mel, audio, RunTable::uniform(B, T, (const float *)packed), (float *)workspace, (cudaStream_t)stream, ev);
+    rc = run_generator(mel, audio, batch_table(c), (float *)workspace, (cudaStream_t)stream, ev);
     if (rc == MG_OK) {
         cudaError_t e = cudaEventSynchronize(ev[n]);
         if (e != cudaSuccess) rc = set_error(MG_ERR_CUDA, "mg_gen_forward_timed: %s", cudaGetErrorString(e));
@@ -510,14 +588,9 @@ int mg_gen_chain_kernel(const void *packed, int k, const float *x, float *y, int
     for (int i = 0; lengths && i < B; ++i)
         if (lengths[i] < 1 || lengths[i] > L_max)
             return set_error(MG_ERR_INVALID_ARGUMENT, "%s: lengths[%d] = %d is outside [1, L_max = %d]", fn, i, lengths[i], L_max);
-    if (precision != MG_GEN_PRECISION_FP32 && precision != MG_GEN_PRECISION_BF16)
-        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: unknown precision %d (MG_GEN_PRECISION_FP32 = 0, MG_GEN_PRECISION_BF16 = 1)", fn,
-                         precision);
-    if (!generator_tc_default_chain())
-        return set_error(MG_ERR_INVALID_ARGUMENT,
-                         "%s: runs the default chain's kernels only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected "
-                         "another (tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
-                         fn, generator_tc_tail(), generator_tc_fused_up());
+    int rc = check_precision(fn, precision);
+    if (!rc) rc = check_default_chain(fn, "runs the default chain's kernels");
+    if (rc) return rc;
     const float *w = (const float *)packed;
     const RunTable t = lengths ? RunTable::ragged(lengths, B, L_max, w) : RunTable::uniform(B, L_max, w);
     return run_one_kernel(fn, (cudaStream_t)stream, [&](int *st) {
@@ -672,38 +745,6 @@ int mg_mel_spectrogram_backward(const void *tables, const float *audio, const fl
 
 /* ------------------------------- host-buffer engine ------------------------------------- */
 
-struct mg_gen_engine {
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    float *packed = nullptr;
-    float *raw = nullptr;  // device staging for raw v/g/bias
-    float *mel = nullptr, *audio = nullptr, *ws = nullptr;
-    float *pin_in = nullptr, *pin_out = nullptr;  // (audio and pin_out hold int16 samples after a pcm16 forward)
-    int *pin_status = nullptr;
-    size_t cap_frames = 0;  // B*T capacity
-    bool loaded = false;
-    float last_ms = 0.f;
-};
-
-static void engine_free_io(mg_gen_engine *e) {
-    cudaFree(e->mel); cudaFree(e->audio); cudaFree(e->ws);
-    cudaFreeHost(e->pin_in); cudaFreeHost(e->pin_out);
-    e->mel = e->audio = e->ws = e->pin_in = e->pin_out = nullptr;
-    e->cap_frames = 0;
-}
-
-static int engine_reserve(mg_gen_engine *e, size_t frames) {
-    if (frames <= e->cap_frames) return MG_OK;
-    engine_free_io(e);
-    MG_CUDA_TRY(cudaMalloc(&e->mel, frames * kMelBins * sizeof(float)));
-    MG_CUDA_TRY(cudaMalloc(&e->audio, frames * 256 * sizeof(float)));
-    MG_CUDA_TRY(cudaMalloc(&e->ws, mg_gen_workspace_bytes(1, (int)frames)));
-    MG_CUDA_TRY(cudaMallocHost(&e->pin_in, frames * kMelBins * sizeof(float)));
-    MG_CUDA_TRY(cudaMallocHost(&e->pin_out, frames * 256 * sizeof(float)));
-    e->cap_frames = frames;
-    return MG_OK;
-}
-
 int mg_gen_engine_create(mg_gen_engine **out, int max_B, int max_T) {
     if (!out) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_gen_engine_create: null out");
     int rc = check_shape("mg_gen_engine_create", max_B, max_T);
@@ -738,79 +779,26 @@ int mg_gen_engine_load_state(mg_gen_engine *e, const float *const *v, const floa
     return MG_OK;
 }
 
-static int engine_check(const char *fn, mg_gen_engine *e, const float *mel_host, const void *audio_host) {
-    if (!e || !mel_host || !audio_host) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: null argument", fn);
-    if (!e->loaded) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: no weights loaded", fn);
-    return MG_OK;
-}
-
-// pcm16: audio_host receives int16 samples; the device audio and the pinned staging are then read as int16, so the
-// download moves half the bytes
-static int engine_forward(mg_gen_engine *e, const float *mel_host, void *audio_host, const RunTable &batch,
-                          int precision = MG_GEN_PRECISION_FP32, bool pcm16 = false) {
-    const int B = batch.items(), T = batch.stride;
-    const size_t frames = (size_t)B * T;
-    int rc = engine_reserve(e, frames);
-    if (rc) return rc;
-    const size_t nin = frames * kMelBins * sizeof(float), nout = frames * 256 * (pcm16 ? sizeof(int16_t) : sizeof(float));
-    cudaPointerAttributes at;
-    const bool in_pinned = cudaPointerGetAttributes(&at, mel_host) == cudaSuccess && at.type == cudaMemoryTypeHost;
-    const bool out_pinned = cudaPointerGetAttributes(&at, audio_host) == cudaSuccess && at.type == cudaMemoryTypeHost;
-    cudaGetLastError();  // clear "invalid value" some drivers raise for pageable pointers
-    const float *src = mel_host;
-    if (!in_pinned) { memcpy(e->pin_in, mel_host, nin); src = e->pin_in; }
-    if (!e->pin_status) MG_CUDA_TRY(cudaMallocHost(&e->pin_status, sizeof(int)));
-    MG_CUDA_TRY(cudaEventRecord(e->ev0, e->stream));
-    // upload, kernels and download are enqueued per batch slice (launch_generator_tc); one synchronisation at the end
-    rc = run_generator(e->mel, e->audio, batch, e->ws, e->stream, nullptr, src, out_pinned ? audio_host : (void *)e->pin_out,
-                       precision, pcm16);
-    if (rc) return rc;
-    MG_CUDA_TRY(cudaEventRecord(e->ev1, e->stream));
-    *e->pin_status = 0;
-    MG_CUDA_TRY(cudaMemcpyAsync(e->pin_status, status_ptr(e->ws, B, T), sizeof(int), cudaMemcpyDeviceToHost, e->stream));
-    MG_CUDA_TRY(cudaStreamSynchronize(e->stream));
-    if (!out_pinned) memcpy(audio_host, e->pin_out, nout);
-    if (*e->pin_status)
-        return set_error(MG_ERR_CUDA, "mg_gen_engine_forward: tensor-core pipeline wait timed out (code %d)", *e->pin_status);
-    MG_CUDA_TRY(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
-    return MG_OK;
-}
-
 int mg_gen_engine_forward(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T) {
-    int rc = engine_check("mg_gen_engine_forward", e, mel_host, audio_host);
-    if (!rc) rc = check_shape("mg_gen_engine_forward", B, T);
-    return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::uniform(B, T, e->packed));
+    return forward({"mg_gen_engine_forward", kHost, nullptr, 1, nullptr, mel_host, audio_host, B, T, nullptr,
+                    MG_GEN_PRECISION_FP32, nullptr, 0, nullptr, e});
 }
 
 int mg_gen_engine_forward_ragged(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max, const int *lengths) {
-    int rc = check_lengths("mg_gen_engine_forward_ragged", B, T_max, lengths);
-    if (!rc) rc = engine_check("mg_gen_engine_forward_ragged", e, mel_host, audio_host);
-    return rc ? rc : engine_forward(e, mel_host, audio_host, RunTable::ragged(lengths, B, T_max, e->packed));
+    return forward({"mg_gen_engine_forward_ragged", kHost | kNeedLengths, nullptr, 1, nullptr, mel_host, audio_host, B, T_max,
+                    lengths, MG_GEN_PRECISION_FP32, nullptr, 0, nullptr, e});
 }
 
 int mg_gen_engine_forward_precision(mg_gen_engine *e, const float *mel_host, float *audio_host, int B, int T_max,
                                     const int *lengths, int precision) {
-    const char *fn = "mg_gen_engine_forward_precision";
-    int rc = check_precision(fn, precision);
-    if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
-    if (!rc) rc = engine_check(fn, e, mel_host, audio_host);
-    if (rc) return rc;
-    return engine_forward(e, mel_host, audio_host, lengths ? RunTable::ragged(lengths, B, T_max, e->packed)
-                                                         : RunTable::uniform(B, T_max, e->packed),
-                          precision);
+    return forward({"mg_gen_engine_forward_precision", kHost, nullptr, 1, nullptr, mel_host, audio_host, B, T_max, lengths,
+                    precision, nullptr, 0, nullptr, e});
 }
 
 int mg_gen_engine_forward_pcm16(mg_gen_engine *e, const float *mel_host, int16_t *audio_host, int B, int T_max, const int *lengths,
                                 int precision) {
-    const char *fn = "mg_gen_engine_forward_pcm16";
-    int rc = check_precision(fn, precision);
-    if (!rc) rc = check_default_chain(fn);
-    if (!rc) rc = lengths ? check_lengths(fn, B, T_max, lengths) : check_shape(fn, B, T_max);
-    if (!rc) rc = engine_check(fn, e, mel_host, audio_host);
-    if (rc) return rc;
-    return engine_forward(e, mel_host, audio_host, lengths ? RunTable::ragged(lengths, B, T_max, e->packed)
-                                                         : RunTable::uniform(B, T_max, e->packed),
-                          precision, true);
+    return forward({"mg_gen_engine_forward_pcm16", kHost | kDefaultChainOnly | kPcm16, nullptr, 1, nullptr, mel_host, audio_host,
+                    B, T_max, lengths, precision, nullptr, 0, nullptr, e});
 }
 
 int mg_gen_engine_last_kernel_ms(mg_gen_engine *e, float *ms) {

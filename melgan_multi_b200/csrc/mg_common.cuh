@@ -205,6 +205,10 @@ int generator_tc_fused_up();  // bit 0: stage 2, bit 1: stage 3 run their stride
 int generator_tc_tail();      // bit i: stage i's ConvT runs at the TAIL of ResBlock i-1's kernel
 void generator_tc_set_tail(int mask);
 bool generator_tc_default_chain();  // no tail fusion, stage 3's ConvT (only) at the front of the last kernel
+// the refusals every generator entry point with a precision shares: an unknown precision, and a chain other than the
+// default one ("<fn>: <role> only, but ...", role e.g. "bf16 runs on the default chain")
+int check_precision(const char *fn, int precision);
+int check_default_chain(const char *fn, const char *role);
 const char *generator_tc_kernel_name(int i);
 const char *generator_tc_kernel_config(int i, int T);
 const char *resblock_config_name(int stage, int L);

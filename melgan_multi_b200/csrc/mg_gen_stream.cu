@@ -238,15 +238,6 @@ struct mg_gen_stream {
 namespace mg {
 namespace {
 
-int check_chain(const char *fn) {
-    if (!generator_tc_default_chain())
-        return set_error(MG_ERR_INVALID_ARGUMENT,
-                         "%s: streaming runs on the default chain only, but mg_gen_set_pipeline / MG_GEN_TAIL / MG_GEN_FUSE_UP selected "
-                         "another (tail mask %d, front mask %d); mg_gen_set_pipeline(-1) restores the default",
-                         fn, generator_tc_tail(), generator_tc_fused_up());
-    return MG_OK;
-}
-
 // Argument checks of a step (no CUDA call), then the plan.  On success p holds the launches, the new counters and the
 // slots' voices.  voice: n ids in [0, n_voices) (NULL: all 0); an open slot keeps its voice unless this step resets it.
 int plan_step(const char *fn, const mg_gen_stream *s, int n_voices, const int *voice, const int *frames, const int *flags, int n,
@@ -365,10 +356,8 @@ int mg_gen_stream_create(mg_gen_stream **out, int max_sessions, int max_push_fra
                          MG_GEN_RAGGED_MAX_B);
     if (max_push_frames < 1 || max_push_frames > (1 << 16))
         return set_error(MG_ERR_INVALID_ARGUMENT, "%s: max_push_frames = %d is outside [1, 65536]", fn, max_push_frames);
-    if (precision != MG_GEN_PRECISION_FP32 && precision != MG_GEN_PRECISION_BF16)
-        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: unknown precision %d (MG_GEN_PRECISION_FP32 = 0, MG_GEN_PRECISION_BF16 = 1)", fn,
-                         precision);
-    int rc = check_chain(fn);
+    int rc = check_precision(fn, precision);
+    if (!rc) rc = check_default_chain(fn, "streaming runs on the default chain");
     if (rc) return rc;
     const size_t need = mg_gen_stream_state_bytes(max_sessions, max_push_frames);
     if (state_bytes < need) return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "%s: state %zu < %zu bytes", fn, state_bytes, need);
@@ -403,7 +392,7 @@ int step_voices(const char *fn, mg_gen_stream *s, const void *const *packed, int
         if (!packed[v]) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] is NULL", fn, v);
         if ((uintptr_t)packed[v] % 16) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: packed[%d] must be 16-byte aligned", fn, v);
     }
-    int rc = check_chain(fn);
+    int rc = check_default_chain(fn, "streaming runs on the default chain");
     if (rc) return rc;
     bool any = false;
     for (int i = 0; frames && i < n && i < s->S; ++i) any |= frames[i] > 0;

@@ -220,40 +220,32 @@ def _ptr_array(ptrs):
     return (ctypes.c_void_p * len(ptrs))(*ptrs)
 
 
-def _lengths(lengths, B, T_max):
-    """Per-item mel lengths of a ragged batch as a C int array: a list, a tuple or a CPU integer tensor of B values in
-    [1, T_max].  A CUDA tensor is refused: reading it would synchronise the stream."""
-    if hasattr(lengths, "device") and hasattr(lengths, "is_floating_point"):
-        if lengths.device.type != "cpu":
-            raise EngineError("lengths must be a list, a tuple or a CPU tensor (reading a CUDA tensor would synchronise)")
-        if lengths.is_floating_point() or lengths.dim() != 1:
-            raise EngineError("lengths must be a 1-D integer tensor")
-        lengths = lengths.tolist()
-    lengths = [int(v) for v in lengths]
-    if len(lengths) != B:
-        raise EngineError("lengths has %d entries for a batch of %d" % (len(lengths), B))
-    bad = [v for v in lengths if not 1 <= v <= T_max]
+def _host_ints(values, B, name, lo, hi, range_error):
+    """B per-item values in [lo, hi) as a C int array: a list, a tuple or a CPU integer tensor.  A CUDA tensor is refused:
+    reading it would synchronise the stream.  name and range_error word the errors."""
+    if hasattr(values, "device") and hasattr(values, "is_floating_point"):
+        if values.device.type != "cpu":
+            raise EngineError("%s must be a list, a tuple or a CPU tensor (reading a CUDA tensor would synchronise)" % name)
+        if values.is_floating_point() or values.dim() != 1:
+            raise EngineError("%s must be a 1-D integer tensor" % name)
+        values = values.tolist()
+    values = [int(v) for v in values]
+    if len(values) != B:
+        raise EngineError("%s has %d entries for a batch of %d" % (name, len(values), B))
+    bad = [v for v in values if not lo <= v < hi]
     if bad:
-        raise EngineError("lengths must lie in [1, T_max = %d] (got %d)" % (T_max, bad[0]))
-    return (ctypes.c_int * B)(*lengths)
+        raise EngineError("%s (got %d)" % (range_error, bad[0]))
+    return (ctypes.c_int * B)(*values)
+
+
+def _lengths(lengths, B, T_max):
+    """Per-item mel lengths of a ragged batch, each in [1, T_max] (_host_ints)."""
+    return _host_ints(lengths, B, "lengths", 1, T_max + 1, "lengths must lie in [1, T_max = %d]" % T_max)
 
 
 def _voice_ids(voice, B, n_voices):
-    """Per-item voice ids of a multi-voice batch as a C int array: a list, a tuple or a CPU integer tensor of B values in
-    [0, n_voices).  A CUDA tensor is refused: reading it would synchronise the stream."""
-    if hasattr(voice, "device") and hasattr(voice, "is_floating_point"):
-        if voice.device.type != "cpu":
-            raise EngineError("voice must be a list, a tuple or a CPU tensor (reading a CUDA tensor would synchronise)")
-        if voice.is_floating_point() or voice.dim() != 1:
-            raise EngineError("voice must be a 1-D integer tensor")
-        voice = voice.tolist()
-    voice = [int(v) for v in voice]
-    if len(voice) != B:
-        raise EngineError("voice has %d entries for a batch of %d" % (len(voice), B))
-    bad = [v for v in voice if not 0 <= v < n_voices]
-    if bad:
-        raise EngineError("voice ids must lie in [0, n_voices = %d) (got %d)" % (n_voices, bad[0]))
-    return (ctypes.c_int * B)(*voice)
+    """Per-item voice ids of a multi-voice batch, each in [0, n_voices) (_host_ints)."""
+    return _host_ints(voice, B, "voice", 0, n_voices, "voice ids must lie in [0, n_voices = %d)" % n_voices)
 
 
 PRECISIONS = {"fp32": 0, "bf16": 1}  # MG_GEN_PRECISION_FP32 / _BF16, include/melgan_b200.h
@@ -536,67 +528,14 @@ class GeneratorDevice(_PackedBlob):
         product: inference only, contract at mg_gen_forward_precision in include/melgan_b200.h).  dtype torch.float32 (the
         default) or torch.int16: 16-bit PCM written by the last kernel, pcm16 of the float audio bit for bit (contract at
         mg_gen_forward_pcm16); out= must then be int16."""
-        torch = self.torch
-        code = _precision(precision)
-        pcm = _pcm16(torch.float32 if dtype is None else dtype)
-        if mel.dim() != 3 or mel.shape[1] != 80:
-            raise EngineError("mel must be [B, 80, T], got %s" % (tuple(mel.shape),))
-        if mel.device != self.device or mel.dtype != torch.float32:
-            raise EngineError("mel must be an fp32 tensor on %s" % (self.device,))
-        mel = mel.contiguous()
-        B, _, T = mel.shape
-        out = _audio_out(torch, out, (B, 1, 256 * T), pcm, self.device)
-        sc = self._scratch.current()
-        sc.check()  # the previous forward's status word on this stream, if its copy has landed
-        ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
-        with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream().cuda_stream
-            if pcm:
-                check(lib().mg_gen_forward_pcm16(_ptr_array([self.packed.data_ptr()]), 1, None, mel.data_ptr(), out.data_ptr(),
-                                                 B, T, None, code, ws.data_ptr(), ws.numel() * 4, stream))
-            elif code == 0:
-                check(lib().mg_gen_forward(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T,
-                                           ws.data_ptr(), ws.numel() * 4, stream))
-            else:
-                check(lib().mg_gen_forward_precision(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, None, code,
-                                                     ws.data_ptr(), ws.numel() * 4, stream))
-            off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4  # the status word sits after the activation buffers
-            sc.arm(ws.view(torch.int32)[off:off + 1])
-        return out
+        return self._forward(mel, None, None, None, out, precision, dtype)
 
     def forward_ragged(self, mel, lengths, out=None, precision="fp32", dtype=None):
         """Ragged batch (inference): mel [B, 80, T_max] with item i's frames [0, lengths[i]) valid (the rest is never read)
         -> audio [B, 1, 256 T_max]; item i's first 256 lengths[i] samples equal its own forward (at the same precision) bit
         for bit, the rest are 0.  lengths: a list, a tuple or a CPU integer tensor.  dtype as for forward.  Asynchronous,
         like forward."""
-        torch = self.torch
-        code = _precision(precision)
-        pcm = _pcm16(torch.float32 if dtype is None else dtype)
-        if mel.dim() != 3 or mel.shape[1] != 80:
-            raise EngineError("mel must be [B, 80, T_max], got %s" % (tuple(mel.shape),))
-        if mel.device != self.device or mel.dtype != torch.float32:
-            raise EngineError("mel must be an fp32 tensor on %s" % (self.device,))
-        mel = mel.contiguous()
-        B, _, T = mel.shape
-        lens = _lengths(lengths, B, T)
-        out = _audio_out(torch, out, (B, 1, 256 * T), pcm, self.device)
-        sc = self._scratch.current()
-        sc.check()
-        ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
-        with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream().cuda_stream
-            if pcm:
-                check(lib().mg_gen_forward_pcm16(_ptr_array([self.packed.data_ptr()]), 1, None, mel.data_ptr(), out.data_ptr(),
-                                                 B, T, lens, code, ws.data_ptr(), ws.numel() * 4, stream))
-            elif code == 0:
-                check(lib().mg_gen_forward_ragged(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens,
-                                                  ws.data_ptr(), ws.numel() * 4, stream))
-            else:
-                check(lib().mg_gen_forward_precision(self.packed.data_ptr(), mel.data_ptr(), out.data_ptr(), B, T, lens, code,
-                                                     ws.data_ptr(), ws.numel() * 4, stream))
-            off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4
-            sc.arm(ws.view(torch.int32)[off:off + 1])
-        return out
+        return self._forward(mel, lengths, None, None, out, precision, dtype)
 
     def forward_voices(self, voices, mel, voice, lengths=None, out=None, precision="fp32", dtype=None):
         """Many voices in one forward (inference): item i of mel [B, 80, T_max] runs on the weights of voices[voice[i]] (a
@@ -605,33 +544,44 @@ class GeneratorDevice(_PackedBlob):
         [0, len(voices)), and lengths as in forward_ragged (None: every item T_max frames), each a list, a tuple or a CPU
         integer tensor.  Items sorted by voice run fastest (contract at mg_gen_forward_voices, include/melgan_b200.h).
         dtype as for forward.  Uses this module's scratch of the current stream.  Asynchronous, like forward."""
+        return self._forward(mel, lengths, list(voices), voice, out, precision, dtype)
+
+    def _forward(self, mel, lengths, voices, voice, out, precision, dtype):
+        """forward, forward_ragged and forward_voices: lengths None (every item T_max frames) or B lengths; voices None
+        (every item on this module's weights) or a list of GeneratorDevice with B voice ids."""
         torch = self.torch
         code = _precision(precision)
         pcm = _pcm16(torch.float32 if dtype is None else dtype)
         if mel.dim() != 3 or mel.shape[1] != 80:
-            raise EngineError("mel must be [B, 80, T_max], got %s" % (tuple(mel.shape),))
+            T = "T" if lengths is None and voices is None else "T_max"
+            raise EngineError("mel must be [B, 80, %s], got %s" % (T, tuple(mel.shape)))
         if mel.device != self.device or mel.dtype != torch.float32:
             raise EngineError("mel must be an fp32 tensor on %s" % (self.device,))
-        voices = list(voices)
-        if not voices:
-            raise EngineError("forward_voices needs at least one voice")
-        for v in voices:
-            if not isinstance(v, GeneratorDevice) or v.device != self.device:
-                raise EngineError("every voice must be a GeneratorDevice on %s" % (self.device,))
+        if voices is not None:
+            if not voices:
+                raise EngineError("forward_voices needs at least one voice")
+            for v in voices:
+                if not isinstance(v, GeneratorDevice) or v.device != self.device:
+                    raise EngineError("every voice must be a GeneratorDevice on %s" % (self.device,))
         mel = mel.contiguous()
         B, _, T = mel.shape
         lens = None if lengths is None else _lengths(lengths, B, T)
-        ids = _voice_ids(voice, B, len(voices))
+        ids = None if voices is None else _voice_ids(voice, B, len(voices))
         out = _audio_out(torch, out, (B, 1, 256 * T), pcm, self.device)
         sc = self._scratch.current()
-        sc.check()
-        ws = sc.buffer("ws", lib().mg_gen_workspace_bytes(B, T))
+        sc.check()  # the previous forward's status word on this stream, if its copy has landed
+        nbytes = lib().mg_gen_workspace_bytes(B, T)
+        ws = sc.buffer("ws", nbytes)
         with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream().cuda_stream
-            blobs = _ptr_array([v.packed.data_ptr() for v in voices])  # (each read orders this stream after its pack)
-            fn = lib().mg_gen_forward_pcm16 if pcm else lib().mg_gen_forward_voices
-            check(fn(blobs, len(voices), ids, mel.data_ptr(), out.data_ptr(), B, T, lens, code, ws.data_ptr(), ws.numel() * 4, stream))
-            off = (lib().mg_gen_workspace_bytes(B, T) - 256) // 4
+            args = (mel.data_ptr(), out.data_ptr(), B, T, lens, code, ws.data_ptr(), ws.numel() * 4,
+                    torch.cuda.current_stream().cuda_stream)
+            if pcm or voices is not None:
+                blobs = [v.packed.data_ptr() for v in voices or [self]]  # (each read orders this stream after its pack)
+                fn = lib().mg_gen_forward_pcm16 if pcm else lib().mg_gen_forward_voices
+                check(fn(_ptr_array(blobs), len(blobs), ids, *args))
+            else:
+                check(lib().mg_gen_forward_precision(self.packed.data_ptr(), *args))
+            off = (nbytes - 256) // 4  # the status word sits after the activation buffers
             sc.arm(ws.view(torch.int32)[off:off + 1])
         return out
 
@@ -1249,20 +1199,7 @@ class GeneratorHost:
     def forward(self, mel, out=None, precision="fp32", dtype=np.float32):
         """mel [B, 80, T] -> audio [B, 1, 256 T]; precision as for GeneratorDevice.forward.  dtype np.float32 (the default)
         or np.int16: 16-bit PCM, pcm16 of the float audio bit for bit (mg_gen_engine_forward_pcm16)."""
-        code = _precision(precision)
-        pcm = _pcm16_np(dtype)
-        mel = np.ascontiguousarray(mel, dtype=np.float32)
-        B, C, T = mel.shape
-        if C != 80:
-            raise EngineError("mel must be [B, 80, T]")
-        out = self._out(out, (B, 1, 256 * T), pcm)
-        if pcm:
-            check(lib().mg_gen_engine_forward_pcm16(self._h, mel.ctypes.data, out.ctypes.data, B, T, None, code))
-        elif code == 0:
-            check(lib().mg_gen_engine_forward(self._h, mel.ctypes.data, out.ctypes.data, B, T))
-        else:
-            check(lib().mg_gen_engine_forward_precision(self._h, mel.ctypes.data, out.ctypes.data, B, T, None, code))
-        return out
+        return self._forward(mel, None, out, precision, dtype)
 
     @staticmethod
     def _out(out, shape, pcm):
@@ -1277,20 +1214,19 @@ class GeneratorHost:
     def forward_ragged(self, mel, lengths, out=None, precision="fp32", dtype=np.float32):
         """Ragged batch from host memory (mg_gen_engine_forward_ragged): mel [B, 80, T_max], lengths and precision as for
         GeneratorDevice.forward_ragged, dtype as for forward -> audio [B, 1, 256 T_max]."""
+        return self._forward(mel, lengths, out, precision, dtype)
+
+    def _forward(self, mel, lengths, out, precision, dtype):
         code = _precision(precision)
         pcm = _pcm16_np(dtype)
         mel = np.ascontiguousarray(mel, dtype=np.float32)
         if mel.ndim != 3 or mel.shape[1] != 80:
-            raise EngineError("mel must be [B, 80, T_max]")
+            raise EngineError("mel must be [B, 80, %s]" % ("T" if lengths is None else "T_max"))
         B, _, T = mel.shape
-        lens = _lengths(lengths, B, T)
+        lens = None if lengths is None else _lengths(lengths, B, T)
         out = self._out(out, (B, 1, 256 * T), pcm)
-        if pcm:
-            check(lib().mg_gen_engine_forward_pcm16(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens, code))
-        elif code == 0:
-            check(lib().mg_gen_engine_forward_ragged(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens))
-        else:
-            check(lib().mg_gen_engine_forward_precision(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens, code))
+        fn = lib().mg_gen_engine_forward_pcm16 if pcm else lib().mg_gen_engine_forward_precision
+        check(fn(self._h, mel.ctypes.data, out.ctypes.data, B, T, lens, code))
         return out
 
     def forward_ptr(self, mel_ptr, out_ptr, B, T):

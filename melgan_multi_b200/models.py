@@ -245,10 +245,7 @@ class Generator(_Repack, nn.Module):
         if not x.is_cuda:
             raise _engine.EngineError("melgan_multi_b200.Generator.generate needs a CUDA tensor (no CPU fallback)")
         with torch.no_grad():
-            dev = self._ensure_packed()
-            if lengths is None:
-                return dev.forward(x.detach().float(), precision=precision, dtype=dtype)
-            return dev.forward_ragged(x.detach().float(), lengths, precision=precision, dtype=dtype)
+            return self._ensure_packed()._forward(x.detach().float(), lengths, None, None, None, precision, dtype)
 
     def stream(self, max_sessions=1, max_push_frames=32, precision="fp32", dtype=torch.float32):
         """A streaming vocoder over this generator's weights (inference only): up to max_sessions live mel streams, each
