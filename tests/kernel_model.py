@@ -133,8 +133,8 @@ def res_index(C, layer, co, ci, tap, h):
 
 def front_index(C, s, ci, co, k, h):
     """Byte offset of half h of W[ci][co][k] of the front ConvT of the fused stage-s kernel (ResBlock-style chunks)."""
-    KC = tc_kc(C)
-    return lib_offset()(1, s, 0, 0, 0, 0) + 2 * ((k * (2 * C // KC) + ci // KC) * 2 * KC * C + in_chunk(C, co, ci % KC, h))
+    assert C == 256 >> s, (C, s)
+    return upf_index(s, ci, co, k, h)
 
 
 # (Cin, Cout, R = outputs per input position, K); layer index in the blob: pre 0, up s -> 1 + s
@@ -175,6 +175,90 @@ def weight_grid(layer):
     return np.meshgrid(*(np.arange(n) for n in dims), indexing="ij")
 
 
+# the fp32 part of the blob: every layer's folded weights in layer order, then every bias (csrc/mg_layout.h weight_offset,
+# bias_offset); Conv1d w[co][ci][tap] at [ci][tap][co], ConvTranspose1d W[ci][co][k] at [ci][co][k % S][k // S] (S = K / 2)
+GEN_LAYERS = synth.GENERATOR_LAYERS  # (name, kind, Cin, Cout, K); layer l of the blob is GEN_LAYERS[l]
+
+
+def gen_fp32_weight_offset(l):
+    """Float offset of layer l's fp32 weights."""
+    return sum(cin * cout * k for _n, _kind, cin, cout, k in GEN_LAYERS[:l])
+
+
+def gen_bias_offset(l):
+    """Float offset of layer l's bias."""
+    return gen_fp32_weight_offset(len(GEN_LAYERS)) + sum(cout for _n, _kind, _ci, cout, _k in GEN_LAYERS[:l])
+
+
+GEN_FP32_BYTES = 4 * gen_bias_offset(len(GEN_LAYERS))
+GEN_TC_START = cdiv(GEN_FP32_BYTES, 256) * 256
+
+
+def gen_fp32_index(l, a, b, tap):
+    """Byte offset of the fp32 copy of layer l's weight at [a][b][tap] of its torch layout (a = co, b = ci for a Conv1d;
+    a = ci, b = co for a ConvTranspose1d); numpy arrays welcome."""
+    _n, kind, cin, cout, K = GEN_LAYERS[l]
+    o = gen_fp32_weight_offset(l)
+    if kind == "conv":
+        return 4 * (o + (b * K + tap) * cout + a)
+    S = K // 2
+    return 4 * (o + ((a * cout + b) * S + tap % S) * 2 + tap // S)
+
+
+def upf_base(s):
+    """The fused stride-2 ConvT copies (stages 2, 3) follow conv_pre's block: 2C x C x 4 taps x (hi, lo) each."""
+    return up_base(4) + 80 * 512 * 7 * 4 + (32 * 64 * 64 if s == 3 else 0)
+
+
+def upf_index(s, ci, co, k, h):
+    """Byte offset of half h of ups[s]'s W[ci][co][k] in its fused-kernel copy (ResBlock-style chunks, 4 taps over 2C
+    input channels); numpy arrays welcome.  front_index without the library."""
+    C = 256 >> s
+    KC = tc_kc(C)
+    return upf_base(s) + 2 * ((k * (2 * C // KC) + ci // KC) * 2 * KC * C + in_chunk(C, co, ci % KC, h))
+
+
+GEN_BLOB_BYTES = upf_base(3) + 32 * 32 * 32
+
+
+def gen_grid(l):
+    """Index arrays (a, b, tap) over layer l's whole weight tensor in its torch layout (v's layout: a is the norm row)."""
+    _n, kind, cin, cout, K = GEN_LAYERS[l]
+    dims = (cout, cin, K) if kind == "conv" else (cin, cout, K)
+    return np.meshgrid(*(np.arange(n) for n in dims), indexing="ij")
+
+
+def gen_split_copies(l):
+    """{copy name: offset function (a, b, tap, h) -> byte offset} of layer l's split-bf16 copies, in torch-layout
+    indices: conv_pre's ring slots, a ConvT's ring slots (and the fused copy of stages 2 and 3), a ResBlock conv's chunks;
+    conv_post has none."""
+    if l == 0:
+        return {"tc": lambda a, b, t, h: gen_weight_offset(0, a, b, t, h)}
+    if l <= 4:
+        out = {"tc": lambda a, b, t, h: gen_weight_offset(l, a, b, t, h)}
+        if l >= 3:
+            out["upf"] = lambda a, b, t, h: upf_index(l - 1, a, b, t, h)
+        return out
+    if l <= 28:
+        C = GEN_LAYERS[l][3]
+        return {"tc": lambda a, b, t, h: res_index(C, l, a, b, t, h)}
+    return {}
+
+
+def gen_regions():
+    """[(name, start, end, padding)] of the generator's blob in address order: the fp32 weights and biases, the padding to
+    the 256-byte aligned tensor-core region, the 24 ResBlock convs, the four ConvTs, conv_pre, the two fused ConvTs."""
+    L = len(GEN_LAYERS)
+    out = [("fp32 " + GEN_LAYERS[l][0], 4 * gen_fp32_weight_offset(l), 4 * gen_fp32_weight_offset(l + 1), False) for l in range(L)]
+    out += [("bias " + GEN_LAYERS[l][0], 4 * gen_bias_offset(l), 4 * gen_bias_offset(l + 1), False) for l in range(L)]
+    out.append(("padding", GEN_FP32_BYTES, GEN_TC_START, True))
+    out += [("tc " + GEN_LAYERS[l][0], res_base(l), res_base(l + 1), False) for l in range(5, 29)]
+    out += [("tc ups.%d" % s, up_base(s), up_base(s) + up_tc_bytes(s), False) for s in range(4)]
+    out.append(("tc conv_pre", up_base(4), upf_base(2), False))
+    out += [("upf ups.2", upf_base(2), upf_base(3), False), ("upf ups.3", upf_base(3), GEN_BLOB_BYTES, False)]
+    return out
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # 4. the blob of one discriminator (restated from csrc/mg_layout.h) and its launch geometry
 # ------------------------------------------------------------------------------------------------------------------
@@ -207,6 +291,38 @@ BLOB_BYTES = TCT_START + TC_BYTES + 4096
 
 def gtc_start(l):
     return GTC_START + sum(GROUPS[i] for i in range(1, l)) * GTC_GROUP
+
+
+D_FP32_BYTES = 4 * _fp32_floats()
+ZERO_START = TCT_START + TC_BYTES  # 1024 zero floats: the conv_post1 dgrad launch's "bias"
+
+
+def disc_fp32_index(l, co, ci, tap):
+    """Byte offset of the fp32 copy of layer l's w[co][ci][tap] (every layer but conv_post1): conv_pre [tap][co 16],
+    grouped [group][ci 4][tap 41][co within group], conv_post2 [ci][tap]; numpy arrays welcome."""
+    _n, cin, cout, k, _s, groups, _p = LAYERS[l]
+    o = disc_weight_offset(l)
+    if l == 0:
+        return 4 * (o + tap * cout + co)
+    if l <= 4:
+        cog = cout // groups
+        return 4 * (o + ((co // cog * (cin // groups) + ci) * k + tap) * cog + co % cog)
+    assert l == 6, l
+    return 4 * (o + ci * k + tap)
+
+
+def disc_regions():
+    """[(name, start, end, padding)] of one discriminator's blob in address order: the fp32 weights (none for conv_post1)
+    and biases, the padding to the 256-byte aligned tensor-core part, conv_post1's copy, the Toeplitz copies of
+    grouped_convs.0-2 and .3, conv_post1's transposed copy, the zero row."""
+    out = [("fp32 " + LAYERS[l][0], 4 * disc_weight_offset(l), 4 * disc_weight_offset(l + 1), False) for l in range(7) if l != 5]
+    out += [("bias " + LAYERS[l][0], 4 * disc_bias_offset(l), 4 * disc_bias_offset(l + 1), False) for l in range(7)]
+    out.append(("padding", D_FP32_BYTES, TC_START, True))
+    out.append(("tc conv_post1", TC_START, GTC_START, False))
+    out += [("toeplitz " + LAYERS[l][0], gtc_start(l), gtc_start(l + 1), False) for l in (1, 2, 3)]
+    out += [("toeplitz " + LAYERS[4][0], G4TC_START, TCT_START, False), ("tcT conv_post1", TCT_START, ZERO_START, False),
+            ("zero row", ZERO_START, BLOB_BYTES, False)]
+    return out
 
 
 def toeplitz_slots(l):
@@ -462,6 +578,19 @@ DILATIONS = (1, 3, 9)
 def folded64(state, name, device="cuda"):
     w = synth.fold_weight_norm(state[name + ".weight_g"], state[name + ".weight_v"])
     return (torch.from_numpy(w).to(device, torch.float64), torch.from_numpy(state[name + ".bias"]).to(device, torch.float64))
+
+
+def fold64(g, v):
+    """synth.fold_weight_norm without its final rounding to fp32: w = g v / ||v|| in float64, norm over every axis but 0."""
+    v64 = v.astype(np.float64)
+    norm = np.sqrt((v64 ** 2).sum(axis=tuple(range(1, v.ndim)), keepdims=True))
+    return g.astype(np.float64).reshape(norm.shape) * v64 / norm
+
+
+def fold_bound(w64, inner):
+    """|w32 - w64| allowed to the pack kernels' fp32 fold of a norm row of `inner` elements (test_pack_blob_gpu's module
+    docstring): (ceil(inner / 128) + 15) 2^-25 |w64|, plus one subnormal ulp."""
+    return (cdiv(inner, 128) + 15) * 2.0 ** -25 * np.abs(w64) + 2.0 ** -149
 
 
 class Gen64:
