@@ -150,8 +150,12 @@ __global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ 
     float2 *A = buf + fr * 1024;
     float *mg = mag + fr * 516;
     mel_frame_bins(st, audio + (size_t)b * L, L, t, live, lt, A, A + 512, mg, nullptr);
-    if (live && lt < st->n_mels)
-        mel[((size_t)b * st->n_mels + lt) * T + t] = logf(fmaxf(mel_band_sum(st, mg, lt), 1e-5f));  // meldataset.py:19-25: log(clip(x, 1e-5) * 1)
+    if (live && lt < st->n_mels) {
+        // meldataset.py:19-25: log(clip(x, 1e-5) * 1).  Not fmaxf, which returns 1e-5 for a NaN s: np.clip and torch.clamp
+        // keep NaN, and a NaN (or Inf) sample must not reach a mel loss as log(1e-5) silence.  Equal to fmaxf otherwise.
+        const float s = mel_band_sum(st, mg, lt);
+        mel[((size_t)b * st->n_mels + lt) * T + t] = logf(s < 1e-5f ? 1e-5f : s);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

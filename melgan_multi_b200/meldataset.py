@@ -41,7 +41,10 @@ def mel_spectrogram(y, n_fft, num_mels, sampling_rate, hop_size, win_size, fmin,
                     norm=1):
     """y: CUDA float tensor [L] or [B, L] in [-1, 1] -> log-mel [num_mels, T] or [B, num_mels, T] (T = L / hop_size for whole
     hops).  ``check_range`` reproduces the reference's two asserts (one host sync); ``norm``: 1 = Slaney area normalisation
-    (the reference's call), 0 = none, 2 = L1."""
+    (the reference's call), 0 = none, 2 = L1.  Non-finite audio (with check_range=False) propagates as in the reference's
+    ``np.log(np.clip(x, 1e-5, None))``: every frame that reads a NaN or Inf sample is NaN in the bands its spectrum
+    makes NaN (an Inf sample can also give +Inf), never log(1e-5); the other frames and items are unchanged.  The
+    gradient is NaN exactly where torch autograd's float64 gradient is."""
     if not torch.is_tensor(y) or not y.is_cuda:
         raise _engine.EngineError("melgan_multi_b200.meldataset.mel_spectrogram needs a CUDA tensor (no CPU fallback; the "
                                   "reference's host path is librosa)")
