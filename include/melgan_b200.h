@@ -393,6 +393,49 @@ int mg_mel_spectrogram_backward(const void *tables, const float *audio, const fl
                                 void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Multi-resolution STFT loss (Parallel WaveGAN's MultiResolutionSTFTLoss) of predicted audio x against target audio y,
+ * both [B][L] device fp32, and its gradient with respect to x.  For each of n_res resolutions (n_fft[r], hop[r], and the
+ * window length given to the table build):
+ *   X = torch.stft(x, n_fft, hop, win_length, periodic Hann(win_length), center=True, pad_mode="reflect"), one-sided,
+ *   T = 1 + L / hop frames (mg_stft_loss_frames); x_mag = sqrt(clamp(|X|^2, min=1e-7)), y_mag likewise;
+ *   sc = ||y_mag - x_mag||_F / ||y_mag||_F and mag = mean |log y_mag - log x_mag| over the whole [B][T][n_fft/2 + 1].
+ * The losses are the means of sc and mag over the resolutions.  Supported: n_fft a power of two in [128, 2048],
+ * 1 <= win_length <= n_fft, hop >= 1, n_fft / 2 < L <= 2^30 (reflect padding by n_fft / 2), 1 to 8 resolutions.
+ *   mg_stft_loss_tables_build fills a HOST buffer of mg_stft_loss_tables_bytes(n_fft) bytes (0 for an unsupported n_fft)
+ *     for one resolution: the window zero-padded to n_fft with (n_fft - win_length) / 2 zeros on the left, then the
+ *     twiddles e^{-2 pi i k / n_fft}, k < n_fft / 2, each computed in double and rounded once.  The caller copies it to
+ *     device memory, 16-byte aligned, once per device.
+ *   mg_stft_loss_workspace_bytes: the forward workspace (each resolution's per-frame partial sums, and the norms the
+ *     backward reads) and the backward workspace (the largest resolution's per-frame gradients, B T n_fft floats).
+ *   mg_stft_loss_forward writes the two losses to the device scalars sc_loss and mag_loss.  The sums are reduced in a
+ *     fixed order (no atomics): the same inputs give the same bits on every run.
+ *   mg_stft_loss_backward writes grad_x = grad_sc d sc / dx + grad_mag d mag / dx [B][L], every element (it may be
+ *     uninitialised), for device scalars grad_sc and grad_mag.  forward_workspace is the workspace of the forward call on
+ *     the same x and y, which it reads; workspace is its own.  Torch autograd's conventions: the clamp passes gradient
+ *     where |X|^2 >= 1e-7, a zero ||y_mag - x_mag|| gives the sc term gradient 0, sign(0) = 0, gradient on reflected
+ *     positions is folded back onto the samples they copy.  The magnitudes are recomputed with the forward's arithmetic.
+ *     Deterministic, no floating-point atomics.
+ * Both are asynchronous on `stream`, with no host synchronisation (capturable in a CUDA graph); concurrent calls need
+ * their own workspaces.  NaN and Inf samples are not clamped away: they make the losses and the gradient NaN or Inf
+ * where float64 autograd of the definition does.  Refused with MG_ERR_INVALID_ARGUMENT before any CUDA call, with a
+ * message naming the argument: n_res outside [1, 8], a NULL array or pointer, misaligned tables or workspaces (16 bytes)
+ * or float pointers (4 bytes), an unsupported n_fft, win_length outside [1, n_fft], hop < 1, L <= n_fft / 2,
+ * L > 2^30, B < 1, a
+ * grid past 2^31 - 1 CTAs (B T per resolution, B ceil(L / 256) for the gradient's gather); a short workspace with
+ * MG_ERR_WORKSPACE_TOO_SMALL.
+ */
+size_t mg_stft_loss_tables_bytes(int n_fft);
+int mg_stft_loss_tables_build(int n_fft, int win_length, void *tables_host);
+int mg_stft_loss_frames(int n_fft, int hop, int L); /* 1 + L / hop, or 0 when the analysis or L is unsupported */
+int mg_stft_loss_workspace_bytes(int n_res, const int *n_fft, const int *hop, int B, int L, size_t *forward_bytes,
+                                 size_t *backward_bytes);
+int mg_stft_loss_forward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y,
+                         int B, int L, float *sc_loss, float *mag_loss, void *workspace, size_t workspace_bytes, void *stream);
+int mg_stft_loss_backward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y,
+                          int B, int L, const float *grad_sc, const float *grad_mag, const void *forward_workspace, float *grad_x,
+                          void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Host-buffer engine.   The call a non-PyTorch host makes: owns its device buffers, takes and
  * returns HOST memory, and performs the host<->device copies itself (this is the path
  * bench.py times as "e2e").  One engine per host thread / CUDA stream.

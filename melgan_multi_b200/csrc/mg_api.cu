@@ -68,6 +68,70 @@ static int run_one_kernel(const char *fn, cudaStream_t stream, F launch) {
 
 using namespace mg;
 
+/* ------------------------------- multi-resolution STFT loss ------------------------------ */
+
+size_t mg_stft_loss_tables_bytes(int n_fft) { return stft_tables_bytes(n_fft); }
+
+int mg_stft_loss_tables_build(int n_fft, int win_length, void *tables_host) { return stft_tables_build(n_fft, win_length, tables_host); }
+
+int mg_stft_loss_frames(int n_fft, int hop, int L) { return stft_frames(n_fft, hop, L); }
+
+int mg_stft_loss_workspace_bytes(int n_res, const int *n_fft, const int *hop, int B, int L, size_t *forward_bytes,
+                                 size_t *backward_bytes) {
+    const char *fn = "mg_stft_loss_workspace_bytes";
+    if (!forward_bytes || !backward_bytes)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %s is NULL", fn, !forward_bytes ? "forward_bytes" : "backward_bytes");
+    *forward_bytes = *backward_bytes = 0;
+    int T[8];
+    const int rc = stft_check(fn, n_res, nullptr, n_fft, hop, B, L, T);
+    if (rc) return rc;
+    stft_workspace(n_res, n_fft, B, T, forward_bytes, backward_bytes);
+    return MG_OK;
+}
+
+static int stft_check_pointer(const char *fn, const char *name, const void *p, unsigned align) {
+    if (!p) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %s is NULL", fn, name);
+    if ((uintptr_t)p % align) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %s must be %u-byte aligned", fn, name, align);
+    return MG_OK;
+}
+
+int mg_stft_loss_forward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y,
+                         int B, int L, float *sc_loss, float *mag_loss, void *workspace, size_t workspace_bytes, void *stream) {
+    const char *fn = "mg_stft_loss_forward";
+    int rc, T[8];
+    if (!tables && n_res >= 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: tables is NULL", fn);
+    if ((rc = stft_check(fn, n_res, tables, n_fft, hop, B, L, T))) return rc;
+    if ((rc = stft_check_pointer(fn, "x", x, 4)) || (rc = stft_check_pointer(fn, "y", y, 4)) ||
+        (rc = stft_check_pointer(fn, "sc_loss", sc_loss, 4)) || (rc = stft_check_pointer(fn, "mag_loss", mag_loss, 4)) ||
+        (rc = stft_check_pointer(fn, "workspace", workspace, 16)))
+        return rc;
+    size_t need, unused;
+    stft_workspace(n_res, n_fft, B, T, &need, &unused);
+    if (workspace_bytes < need)
+        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
+    return launch_stft_loss_forward(n_res, tables, n_fft, hop, x, y, B, L, T, sc_loss, mag_loss, workspace, (cudaStream_t)stream);
+}
+
+int mg_stft_loss_backward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y,
+                          int B, int L, const float *grad_sc, const float *grad_mag, const void *forward_workspace, float *grad_x,
+                          void *workspace, size_t workspace_bytes, void *stream) {
+    const char *fn = "mg_stft_loss_backward";
+    int rc, T[8];
+    if (!tables && n_res >= 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: tables is NULL", fn);
+    if ((rc = stft_check(fn, n_res, tables, n_fft, hop, B, L, T))) return rc;
+    if ((rc = stft_check_pointer(fn, "x", x, 4)) || (rc = stft_check_pointer(fn, "y", y, 4)) ||
+        (rc = stft_check_pointer(fn, "grad_sc", grad_sc, 4)) || (rc = stft_check_pointer(fn, "grad_mag", grad_mag, 4)) ||
+        (rc = stft_check_pointer(fn, "forward_workspace", forward_workspace, 16)) ||
+        (rc = stft_check_pointer(fn, "grad_x", grad_x, 4)) || (rc = stft_check_pointer(fn, "workspace", workspace, 16)))
+        return rc;
+    size_t unused, need;
+    stft_workspace(n_res, n_fft, B, T, &unused, &need);
+    if (workspace_bytes < need)
+        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
+    return launch_stft_loss_backward(n_res, tables, n_fft, hop, x, y, B, L, T, grad_sc, grad_mag, forward_workspace, grad_x, workspace,
+                                     (cudaStream_t)stream);
+}
+
 /* ------------------------------- host-buffer engine ------------------------------------- */
 
 struct mg_gen_engine {

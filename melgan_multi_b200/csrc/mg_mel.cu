@@ -17,6 +17,7 @@
 #include <math.h>
 
 #include "mg_common.cuh"
+#include "mg_fft.cuh"
 
 namespace mg {
 
@@ -81,8 +82,6 @@ int mel_tables_build(int sr, int n_mels, float fmin, float fmax, int norm, MelTa
     return MG_OK;
 }
 
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-
 // Frame t of item xb (128 threads, lt = 0..127, of a 256-thread CTA that calls this together: it holds __syncthreads):
 // windowed 512-point complex Stockham FFT in A / Bf, split into the 513 bins of the real transform; mg[k] = |X[k]|, and
 // X[k] itself when Xk is given.  The forward and the backward both run it, so the backward differentiates the very
@@ -98,28 +97,10 @@ __device__ __forceinline__ void mel_frame_bins(const MelTables *st, const float 
     }
     __syncthreads();
     // 512-point Stockham autosort FFT, radix 2: 9 passes, 256 butterflies each (2 per thread)
-    float2 *in = A, *out = Bf;
-#pragma unroll 1
-    for (int ns = 1; ns < 512; ns <<= 1) {
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            const int j = lt + 128 * r;
-            const int k = j & (ns - 1);
-            const float2 v0 = in[j], v1 = cmul(in[j + 256], st->tw[k * (512 / ns)]);  // e^{-2 pi i k / (2 ns)}
-            const int j0 = ((j - k) << 1) + k;
-            out[j0] = make_float2(v0.x + v1.x, v0.y + v1.y);
-            out[j0 + ns] = make_float2(v0.x - v1.x, v0.y - v1.y);
-        }
-        __syncthreads();
-        float2 *tmp = in; in = out; out = tmp;
-    }
+    float2 *in = stockham<512, 128, false>(A, Bf, st->tw, lt);
     // Z = in: bins of the real transform, X[k] = E[k] + e^{-2 pi i k / 1024} O[k], E = (Z[k] + conj Z[512-k]) / 2, O = (Z[k] - conj Z[512-k]) / 2i
     for (int k = lt; k <= 512; k += 128) {
-        const float2 zk = in[k & 511], zc = in[(512 - k) & 511];
-        const float2 E = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y - zc.y));
-        const float2 O = make_float2(0.5f * (zk.y + zc.y), -0.5f * (zk.x - zc.x));
-        const float2 w = k < 512 ? st->tw[k] : make_float2(-1.f, 0.f);
-        const float2 X = make_float2(E.x + w.x * O.x - w.y * O.y, E.y + w.x * O.y + w.y * O.x);
+        const float2 X = real_split(in[k & 511], in[(512 - k) & 511], k < 512 ? st->tw[k] : make_float2(-1.f, 0.f));
         mg[k] = sqrtf(X.x * X.x + X.y * X.y);  // power = 1 (meldataset.py:50)
         if (Xk) Xk[k] = X;
     }
@@ -169,16 +150,8 @@ __global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ 
 //   512-point inverse Stockham FFT (conjugate twiddles, unnormalised)  ->  times the window  ->  dframe[b][t][1024].
 // mel_backward_ola_kernel: grad_audio[b][i] = sum over the <= 4 frames covering padded sample i + 384, ascending t.
 //
-// Adjoint of the split, with a_k = (1 - i W^k) / 2, b_k = (1 + i W^k) / 2 (W^k = tw[k], W^512 = -1), X[k] = a_k Z[k & 511] +
-// b_k conj Z[(512 - k) & 511]:  dZ[j] = P(j) + Q((512 - j) & 511), P(k) = conj(a_k) G[k], Q(k) = b_k conj G[k]; dZ[0] also
-// takes P(512) + Q(512), the Nyquist bin's share.
+// The split's adjoint (split_adjoint_pass) and the inverse pass (stockham<512, 128, true>) are in mg_fft.cuh.
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float2 split_adjoint(const float2 G, const float2 w) {  // conj(a) G, w = W^k
-    return make_float2(0.5f * (G.x + w.y * G.x - w.x * G.y), 0.5f * (G.y + w.x * G.x + w.y * G.y));
-}
-__device__ __forceinline__ float2 split_adjoint_conj(const float2 G, const float2 w) {  // b conj(G)
-    return make_float2(0.5f * (G.x - w.y * G.x + w.x * G.y), 0.5f * (-G.y + w.x * G.x + w.y * G.y));
-}
 
 __global__ void __launch_bounds__(256) mel_backward_frame_kernel(const MelTables *__restrict__ tab, const float *__restrict__ audio,
                                                                  const float *__restrict__ grad_mel, float *__restrict__ dframe,
@@ -220,34 +193,10 @@ __global__ void __launch_bounds__(256) mel_backward_frame_kernel(const MelTables
         Xk[k] = make_float2(r * Xk[k].x, r * Xk[k].y);
     }
     __syncthreads();
-    float2 *in = A, *out = A + 512;
-    for (int j = lt; j < 512; j += 128) {
-        const int jc = (512 - j) & 511;
-        const float2 p = split_adjoint(Xk[j], st->tw[j]), q = split_adjoint_conj(Xk[jc], st->tw[jc]);
-        float2 d = make_float2(p.x + q.x, p.y + q.y);
-        if (j == 0) {  // the Nyquist bin reads Z[0] as well: P(512) + Q(512), W^512 = -1
-            const float2 p5 = split_adjoint(Xk[512], make_float2(-1.f, 0.f)), q5 = split_adjoint_conj(Xk[512], make_float2(-1.f, 0.f));
-            d = make_float2(d.x + (p5.x + q5.x), d.y + (p5.y + q5.y));
-        }
-        in[j] = d;
-    }
+    split_adjoint_pass<512, 128>(Xk, A, st->tw, lt);
     __syncthreads();
     // inverse transform: the forward's Stockham passes with conjugate twiddles, e^{+2 pi i k / (2 ns)}, no 1/512
-#pragma unroll 1
-    for (int ns = 1; ns < 512; ns <<= 1) {
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            const int j = lt + 128 * r;
-            const int k = j & (ns - 1);
-            const float2 tw = st->tw[k * (512 / ns)];
-            const float2 v0 = in[j], v1 = cmul(in[j + 256], make_float2(tw.x, -tw.y));
-            const int j0 = ((j - k) << 1) + k;
-            out[j0] = make_float2(v0.x + v1.x, v0.y + v1.y);
-            out[j0 + ns] = make_float2(v0.x - v1.x, v0.y - v1.y);
-        }
-        __syncthreads();
-        float2 *tmp = in; in = out; out = tmp;
-    }
+    float2 *in = stockham<512, 128, true>(A, A + 512, st->tw, lt);
     if (!live) return;
     // dz[n] = d/dRe z[n] + i d/dIm z[n], z[n] = w[2n] x[2n] + i w[2n+1] x[2n+1]
     float2 *df = reinterpret_cast<float2 *>(dframe + ((size_t)b * T + t) * kMelNfft);
