@@ -335,24 +335,34 @@ resblock_tc_kernel(const float *__restrict__ x, float *__restrict__ y_, int stag
     // fp32 lrelu(x[L-1]) in b1s (the tail ConvT's fix-up)
     auto write_x = [&](float (&A)[RPW][NA], const float *bsrc, bool keep_last) {
         const int L = len();
+        // KB k-panels at a time, both rows of a fragment: their bias pairs are read before their stores.  A bias read after
+        // a store to X may alias it, so one k-panel at a time ran each (load, lrelu, split, store) strictly after the
+        // previous one, at shared-memory latency.  All NCW / 8 pairs at once do not fit the register budget (ptxas spills
+        // in every configuration), nor do 4 in the stage-0 tile (NCP = 2), which is at its register cap
+        constexpr int KB = NCP > 1 ? 2 : NCW / 8 < 4 ? NCW / 8 : 4;
 #pragma unroll
         for (int r = 0; r < RPW; ++r)
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int p = (rb0 + r) * 64 + frag_row(t, h), tp = o + p;
-                const bool inr = interior || (tp >= 0 && tp < L);
-                uint8_t *xh = Xh + (c0 >> 3) * XPITCH + (p + SLACK) * 16 + q * 4, *xl = xh + XBYTES;
+            for (int k0 = 0; k0 < NCW / 8; k0 += KB) {
+                float2 bb[KB];
 #pragma unroll
-                for (int k = 0; k < NCW / 8; ++k) {
-                    const int col = c0 + 8 * k + 2 * q;
-                    const float2 bb = *reinterpret_cast<const float2 *>(bsrc + col);
-                    const float f0 = inr ? lrelu(A[r][4 * k + 2 * h] + bb.x) : 0.f;
-                    const float f1 = inr ? lrelu(A[r][4 * k + 2 * h + 1] + bb.y) : 0.f;
-                    uint32_t hi, lo;
-                    split2_bf16(f0, f1, hi, lo);
-                    *reinterpret_cast<uint32_t *>(xh + k * XPITCH) = hi;
-                    if constexpr (!ONE) *reinterpret_cast<uint32_t *>(xl + k * XPITCH) = lo;
-                    if (keep_last && tp == L - 1) *reinterpret_cast<float2 *>(b1s + col) = make_float2(f0, f1);
+                for (int j = 0; j < KB; ++j) bb[j] = *reinterpret_cast<const float2 *>(bsrc + c0 + 8 * (k0 + j) + 2 * q);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int p = (rb0 + r) * 64 + frag_row(t, h), tp = o + p;
+                    const bool inr = interior || (tp >= 0 && tp < L);
+                    uint8_t *xh = Xh + (c0 >> 3) * XPITCH + (p + SLACK) * 16 + q * 4, *xl = xh + XBYTES;
+#pragma unroll
+                    for (int j = 0; j < KB; ++j) {
+                        const int k = k0 + j, col = c0 + 8 * k + 2 * q;
+                        const float f0 = inr ? lrelu(A[r][4 * k + 2 * h] + bb[j].x) : 0.f;
+                        const float f1 = inr ? lrelu(A[r][4 * k + 2 * h + 1] + bb[j].y) : 0.f;
+                        uint32_t hi, lo;
+                        split2_bf16(f0, f1, hi, lo);
+                        *reinterpret_cast<uint32_t *>(xh + k * XPITCH) = hi;
+                        if constexpr (!ONE) *reinterpret_cast<uint32_t *>(xl + k * XPITCH) = lo;
+                        if (keep_last && tp == L - 1) *reinterpret_cast<float2 *>(b1s + col) = make_float2(f0, f1);
+                    }
                 }
             }
     };
