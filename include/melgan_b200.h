@@ -436,6 +436,50 @@ int mg_stft_loss_backward(int n_res, const void *const *tables, const int *n_fft
                           void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Multi-resolution log-mel L1 loss of predicted audio x against target audio y, both [B][L] device fp32, and its
+ * gradient with respect to x (HiFi-GAN's 45 * l1(mel(y_hat), mel(y)) without the 45, summed over several analyses).
+ * For each of n_res resolutions r (n_fft[r] = N, hop[r] = H, and the window length W, sampling rate, n_mels M, fmin and
+ * fmax given to the table build), p = (N - H) / 2:
+ *   x~ = x with p zeros on each side; frames T = 1 + (L + 2p - N) / H (mg_mel_loss_frames; T < 1 is refused);
+ *   w = periodic Hann of length W, zero-padded to N with (N - W) / 2 zeros on the left (librosa's pad_center);
+ *   X_t[k] = sum_n w[n] x~[t H + n] e^{-2 pi i k n / N}, k = 0..N/2;  S_t[m] = sum_k F[m, k] |X_t[k]|, F the librosa
+ *   Slaney filter bank (htk=False, Slaney area normalisation, bin frequencies k sr / N);  mel = ln(clip(S, min=1e-5));
+ *   l_r = mean over (b, m, t) of |mel_x - mel_y|.
+ * The loss is (1 / n_res) sum_r l_r, a device fp32 scalar.  At one resolution (1024, 256, 1024, 80) it is F.l1_loss of
+ * mg_mel_spectrogram's two outputs.  Supported: N a power of two in [128, 2048], 1 <= W <= N, 1 <= H <= N,
+ * 1 <= M <= 512 (empty filters allowed: their band is ln(1e-5) and gets no gradient), 0 <= fmin < fmax <= sr / 2,
+ * 1 to 8 resolutions, T >= 1, L <= 2^30.
+ *   mg_mel_loss_tables_build fills a HOST buffer of mg_mel_loss_tables_bytes(n_fft) bytes (0 for an unsupported n_fft):
+ *     the STFT loss's window and twiddles for (n_fft, win_length), then n_mels and the sparse filter bank.  The caller
+ *     copies it to device memory, 16-byte aligned, once per device.
+ *   mg_mel_loss_workspace_bytes: the forward workspace (one partial sum per item and frame of each resolution) and the
+ *     backward workspace (the largest resolution's per-frame gradients, B T n_fft floats).
+ *   mg_mel_loss_forward writes the loss to the device scalar `loss`.  Per-frame fp32 partials are summed in float64 in a
+ *     fixed order (no atomics): the same inputs give the same bits on every run.
+ *   mg_mel_loss_backward writes grad_x = grad d loss / dx [B][L], every element (it may be uninitialised), for the
+ *     device scalar grad.  It reads no forward workspace: the spectra and bands are recomputed with the forward's
+ *     arithmetic.  Torch autograd's conventions: d|a - b| / da = sign(a - b) with sign(0) = sign(NaN) = 0, the clip
+ *     passes the gradient where S >= 1e-5, a bin with |X| = 0 contributes 0, the rfft's adjoint runs over bins 0..N/2
+ *     as the forward has them, gradients on padding are dropped.  Deterministic, no floating-point atomics.
+ * Both are asynchronous on `stream`, with no host synchronisation (capturable in a CUDA graph); concurrent calls need
+ * their own workspaces.  NaN and Inf samples are not clamped away: they make the loss and the gradient NaN or Inf where
+ * float64 autograd of the definition does.  Refused with MG_ERR_INVALID_ARGUMENT before any CUDA call, with a message
+ * naming the argument: n_res outside [1, 8], a NULL array or pointer, misaligned tables or workspaces (16 bytes) or
+ * float pointers (4 bytes), an unsupported n_fft, win_length, n_mels, fmin or fmax, hop outside [1, n_fft], L outside
+ * [1, 2^30], fewer samples than one frame, B < 1, a grid past 2^31 - 1 CTAs (B T per resolution, B ceil(L / 256) for the
+ * gradient's gather); a short workspace with MG_ERR_WORKSPACE_TOO_SMALL.
+ */
+size_t mg_mel_loss_tables_bytes(int n_fft);
+int mg_mel_loss_tables_build(int n_fft, int win_length, int sampling_rate, int n_mels, float fmin, float fmax, void *tables_host);
+int mg_mel_loss_frames(int n_fft, int hop, int L); /* 1 + (L + 2p - n_fft) / hop, or 0 when the analysis or L is unsupported */
+int mg_mel_loss_workspace_bytes(int n_res, const int *n_fft, const int *hop, int B, int L, size_t *forward_bytes,
+                                size_t *backward_bytes);
+int mg_mel_loss_forward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y, int B,
+                        int L, float *loss, void *workspace, size_t workspace_bytes, void *stream);
+int mg_mel_loss_backward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y, int B,
+                         int L, const float *grad, float *grad_x, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Host-buffer engine.   The call a non-PyTorch host makes: owns its device buffers, takes and
  * returns HOST memory, and performs the host<->device copies itself (this is the path
  * bench.py times as "e2e").  One engine per host thread / CUDA stream.

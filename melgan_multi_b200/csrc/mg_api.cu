@@ -132,6 +132,62 @@ int mg_stft_loss_backward(int n_res, const void *const *tables, const int *n_fft
                                      (cudaStream_t)stream);
 }
 
+/* ------------------------------- multi-resolution mel loss ------------------------------- */
+
+size_t mg_mel_loss_tables_bytes(int n_fft) { return mel_loss_tables_bytes(n_fft); }
+
+int mg_mel_loss_tables_build(int n_fft, int win_length, int sampling_rate, int n_mels, float fmin, float fmax, void *tables_host) {
+    return mel_loss_tables_build(n_fft, win_length, sampling_rate, n_mels, fmin, fmax, tables_host);
+}
+
+int mg_mel_loss_frames(int n_fft, int hop, int L) { return mel_loss_frames(n_fft, hop, L); }
+
+int mg_mel_loss_workspace_bytes(int n_res, const int *n_fft, const int *hop, int B, int L, size_t *forward_bytes,
+                                size_t *backward_bytes) {
+    const char *fn = "mg_mel_loss_workspace_bytes";
+    if (!forward_bytes || !backward_bytes)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %s is NULL", fn, !forward_bytes ? "forward_bytes" : "backward_bytes");
+    *forward_bytes = *backward_bytes = 0;
+    int T[8];
+    const int rc = mel_loss_check(fn, n_res, nullptr, n_fft, hop, B, L, T);
+    if (rc) return rc;
+    mel_loss_workspace(n_res, n_fft, B, T, forward_bytes, backward_bytes);
+    return MG_OK;
+}
+
+int mg_mel_loss_forward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y, int B,
+                        int L, float *loss, void *workspace, size_t workspace_bytes, void *stream) {
+    const char *fn = "mg_mel_loss_forward";
+    int rc, T[8];
+    if (!tables && n_res >= 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: tables is NULL", fn);
+    if ((rc = mel_loss_check(fn, n_res, tables, n_fft, hop, B, L, T))) return rc;
+    if ((rc = stft_check_pointer(fn, "x", x, 4)) || (rc = stft_check_pointer(fn, "y", y, 4)) ||
+        (rc = stft_check_pointer(fn, "loss", loss, 4)) || (rc = stft_check_pointer(fn, "workspace", workspace, 16)))
+        return rc;
+    size_t need, unused;
+    mel_loss_workspace(n_res, n_fft, B, T, &need, &unused);
+    if (workspace_bytes < need)
+        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
+    return launch_mel_loss_forward(n_res, tables, n_fft, hop, x, y, B, L, T, loss, workspace, (cudaStream_t)stream);
+}
+
+int mg_mel_loss_backward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y, int B,
+                         int L, const float *grad, float *grad_x, void *workspace, size_t workspace_bytes, void *stream) {
+    const char *fn = "mg_mel_loss_backward";
+    int rc, T[8];
+    if (!tables && n_res >= 1) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: tables is NULL", fn);
+    if ((rc = mel_loss_check(fn, n_res, tables, n_fft, hop, B, L, T))) return rc;
+    if ((rc = stft_check_pointer(fn, "x", x, 4)) || (rc = stft_check_pointer(fn, "y", y, 4)) ||
+        (rc = stft_check_pointer(fn, "grad", grad, 4)) || (rc = stft_check_pointer(fn, "grad_x", grad_x, 4)) ||
+        (rc = stft_check_pointer(fn, "workspace", workspace, 16)))
+        return rc;
+    size_t unused, need;
+    mel_loss_workspace(n_res, n_fft, B, T, &unused, &need);
+    if (workspace_bytes < need)
+        return set_error(MG_ERR_WORKSPACE_TOO_SMALL, "%s: workspace of %zu bytes, %zu needed", fn, workspace_bytes, need);
+    return launch_mel_loss_backward(n_res, tables, n_fft, hop, x, y, B, L, T, grad, grad_x, workspace, (cudaStream_t)stream);
+}
+
 /* ------------------------------- host-buffer engine ------------------------------------- */
 
 struct mg_gen_engine {

@@ -263,6 +263,8 @@ int launch_mel_backward(const void *tables, const float *audio, const float *gra
                         void *workspace, size_t workspace_bytes, cudaStream_t s);
 size_t stft_tables_bytes(int n_fft);
 int stft_tables_build(int n_fft, int win_length, void *tables_host);
+// the window and twiddles of one resolution (the STFT-loss table layout, win[n_fft] then tw[n_fft / 2]), arguments checked
+void stft_tables_fill(int n_fft, int win_length, float *win);
 int stft_frames(int n_fft, int hop, int L);
 int stft_check(const char *fn, int n_res, const void *const *tables, const int *n_fft, const int *hop, int B, int L, int *T);
 void stft_workspace(int n_res, const int *n_fft, int B, const int *T, size_t *fwd, size_t *bwd);
@@ -271,6 +273,15 @@ int launch_stft_loss_forward(int n_res, const void *const *tables, const int *n_
 int launch_stft_loss_backward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y,
                               int B, int L, const int *T, const float *grad_sc, const float *grad_mag, const void *fwd_workspace,
                               float *grad_x, void *workspace, cudaStream_t s);
+size_t mel_loss_tables_bytes(int n_fft);
+int mel_loss_tables_build(int n_fft, int win_length, int sr, int n_mels, float fmin, float fmax, void *tables_host);
+int mel_loss_frames(int n_fft, int hop, int L);
+int mel_loss_check(const char *fn, int n_res, const void *const *tables, const int *n_fft, const int *hop, int B, int L, int *T);
+void mel_loss_workspace(int n_res, const int *n_fft, int B, const int *T, size_t *fwd, size_t *bwd);
+int launch_mel_loss_forward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y,
+                            int B, int L, const int *T, float *loss, void *workspace, cudaStream_t s);
+int launch_mel_loss_backward(int n_res, const void *const *tables, const int *n_fft, const int *hop, const float *x, const float *y,
+                             int B, int L, const int *T, const float *grad, float *grad_x, void *workspace, cudaStream_t s);
 int launch_msd_forward(const void *packed, const float *y, int Bt, int L, float *const *fmaps, int *status, cudaStream_t s);
 // batch: lengths and stride of the kernel's input (ConvT) / of the ResBlock itself (the output length for codes 12..14)
 // precision: MG_GEN_PRECISION_FP32 (3-pass split bf16) or MG_GEN_PRECISION_BF16 (one pass; only the default chain's kernels)

@@ -17,7 +17,7 @@
 #include <math.h>
 
 #include "mg_common.cuh"
-#include "mg_fft.cuh"
+#include "mg_mel_bank.cuh"
 
 namespace mg {
 
@@ -42,16 +42,12 @@ static double mel_to_hz(double m) {
     return m >= min_log_mel ? min_log_hz * exp(logstep * (m - min_log_mel)) : f_sp * m;
 }
 
-// librosa.filters.mel(sr, 1024, n_mels, fmin, fmax, htk=False, norm): norm 0 = None, 1 = Slaney area normalisation (what
+// librosa.filters.mel(sr, n_fft, n_mels, fmin, fmax, htk=False, norm): norm 0 = None, 1 = Slaney area normalisation (what
 // `norm=1` means in the librosa 0.6/0.7 API the reference was written against), 2 = L1 (what the integer 1 means since 0.8)
-int mel_tables_build(int sr, int n_mels, float fmin, float fmax, int norm, MelTables *t) {
-    if (sr < 1 || n_mels < 1 || n_mels > kMelMaxMels || !(fmin >= 0.f) || !(fmax > fmin) || fmax > sr / 2.0f + 1e-3f || norm < 0 || norm > 2)
-        return set_error(MG_ERR_INVALID_ARGUMENT, "mg_mel_tables_build: sr=%d n_mels=%d fmin=%g fmax=%g norm=%d", sr, n_mels, fmin, fmax, norm);
-    const double pi = 3.14159265358979323846;
-    for (int n = 0; n < kMelNfft; ++n) t->win[n] = (float)(0.5 - 0.5 * cos(2 * pi * n / kMelNfft));
-    for (int k = 0; k < kMelNfft / 2; ++k) t->tw[k] = make_float2((float)cos(2 * pi * k / kMelNfft), (float)-sin(2 * pi * k / kMelNfft));
-    t->n_mels = n_mels;
-    double edge[kMelMaxMels + 2];
+int mel_filters_build(const char *fn, int n_fft, int sr, int n_mels, float fmin, float fmax, int norm, int *kstart, int *kcount,
+                      int *woff, float *weights) {
+    const int bins = n_fft / 2 + 1;
+    double edge[kMelLossMaxMels + 2];
     const double m0 = hz_to_mel(fmin), m1 = hz_to_mel(fmax);
     for (int i = 0; i < n_mels + 2; ++i) edge[i] = mel_to_hz(m0 + (m1 - m0) * i / (n_mels + 1));
     int off = 0;
@@ -60,61 +56,39 @@ int mel_tables_build(int sr, int n_mels, float fmin, float fmax, int norm, MelTa
         const double scale = norm == 1 ? 2.0 / (hi - lo) : 1.0;
         int ks = -1, kc = 0;
         double l1 = 0;
-        for (int k = 0; k < kMelBinsFft; ++k) {
-            const double f = (double)k * (sr / 2.0) / (kMelNfft / 2);
+        for (int k = 0; k < bins; ++k) {
+            const double f = (double)k * (sr / 2.0) / (n_fft / 2);
             const double up = (f - lo) / (mid - lo), dn = (hi - f) / (hi - mid);
             const double w = up < dn ? (up > 0 ? up : 0.0) : (dn > 0 ? dn : 0.0);
             if (w > 0) {
                 if (ks < 0) ks = k;
-                if (off + (k - ks) >= 2 * kMelBinsFft) return set_error(MG_ERR_INVALID_ARGUMENT, "mg_mel_tables_build: filter bank too dense");
-                t->weights[off + (k - ks)] = (float)(w * scale);
+                if (off + (k - ks) >= 2 * bins) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: filter bank too dense", fn);
+                weights[off + (k - ks)] = (float)(w * scale);
                 kc = k - ks + 1;
                 l1 += w;
             }
         }
         if (norm == 2 && l1 > 0)
-            for (int i = 0; i < kc; ++i) t->weights[off + i] = (float)(t->weights[off + i] / l1);
-        t->kstart[m] = ks < 0 ? 0 : ks;
-        t->kcount[m] = kc;
-        t->woff[m] = off;
+            for (int i = 0; i < kc; ++i) weights[off + i] = (float)(weights[off + i] / l1);
+        kstart[m] = ks < 0 ? 0 : ks;
+        kcount[m] = kc;
+        woff[m] = off;
         off += kc;
     }
     return MG_OK;
 }
 
-// Frame t of item xb (128 threads, lt = 0..127, of a 256-thread CTA that calls this together: it holds __syncthreads):
-// windowed 512-point complex Stockham FFT in A / Bf, split into the 513 bins of the real transform; mg[k] = |X[k]|, and
-// X[k] itself when Xk is given.  The forward and the backward both run it, so the backward differentiates the very
-// magnitudes the forward summed.
-__device__ __forceinline__ void mel_frame_bins(const MelTables *st, const float *xb, int L, int t, bool live, int lt, float2 *A,
-                                               float2 *Bf, float *mg, float2 *Xk) {
-    // windowed frame, even samples -> real part, odd -> imaginary; sample index in the UNPADDED signal: t*hop - 384 + n
-    for (int n = lt; n < 512; n += 128) {
-        const int i0 = t * kMelHop - kMelPad + 2 * n;
-        const float x0 = (live && i0 >= 0 && i0 < L) ? __ldg(xb + i0) : 0.f;
-        const float x1 = (live && i0 + 1 >= 0 && i0 + 1 < L) ? __ldg(xb + i0 + 1) : 0.f;
-        A[n] = make_float2(st->win[2 * n] * x0, st->win[2 * n + 1] * x1);
-    }
-    __syncthreads();
-    // 512-point Stockham autosort FFT, radix 2: 9 passes, 256 butterflies each (2 per thread)
-    float2 *in = stockham<512, 128, false>(A, Bf, st->tw, lt);
-    // Z = in: bins of the real transform, X[k] = E[k] + e^{-2 pi i k / 1024} O[k], E = (Z[k] + conj Z[512-k]) / 2, O = (Z[k] - conj Z[512-k]) / 2i
-    for (int k = lt; k <= 512; k += 128) {
-        const float2 X = real_split(in[k & 511], in[(512 - k) & 511], k < 512 ? st->tw[k] : make_float2(-1.f, 0.f));
-        mg[k] = sqrtf(X.x * X.x + X.y * X.y);  // power = 1 (meldataset.py:50)
-        if (Xk) Xk[k] = X;
-    }
-    __syncthreads();
+int mel_tables_build(int sr, int n_mels, float fmin, float fmax, int norm, MelTables *t) {
+    if (sr < 1 || n_mels < 1 || n_mels > kMelMaxMels || !(fmin >= 0.f) || !(fmax > fmin) || fmax > sr / 2.0f + 1e-3f || norm < 0 || norm > 2)
+        return set_error(MG_ERR_INVALID_ARGUMENT, "mg_mel_tables_build: sr=%d n_mels=%d fmin=%g fmax=%g norm=%d", sr, n_mels, fmin, fmax, norm);
+    const double pi = 3.14159265358979323846;
+    for (int n = 0; n < kMelNfft; ++n) t->win[n] = (float)(0.5 - 0.5 * cos(2 * pi * n / kMelNfft));
+    for (int k = 0; k < kMelNfft / 2; ++k) t->tw[k] = make_float2((float)cos(2 * pi * k / kMelNfft), (float)-sin(2 * pi * k / kMelNfft));
+    t->n_mels = n_mels;
+    return mel_filters_build("mg_mel_tables_build", kMelNfft, sr, n_mels, fmin, fmax, norm, t->kstart, t->kcount, t->woff, t->weights);
 }
 
-// mel band m before the log: the fma dot product of its sparse filter run with the magnitudes
-__device__ __forceinline__ float mel_band_sum(const MelTables *st, const float *mg, int m) {
-    const int ks = st->kstart[m], kc = st->kcount[m];
-    const float *w = st->weights + st->woff[m];
-    float s = 0.f;
-    for (int i = 0; i < kc; ++i) s = fmaf(w[i], mg[ks + i], s);
-    return s;
-}
+__device__ __forceinline__ MelBank mel_bank(const MelTables *st) { return MelBank{st->kstart, st->kcount, st->woff, st->weights}; }
 
 __global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ tab, const float *__restrict__ audio,
                                                   float *__restrict__ mel, int L, int T) {
@@ -130,13 +104,9 @@ __global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ 
     const bool live = t < T;
     float2 *A = buf + fr * 1024;
     float *mg = mag + fr * 516;
-    mel_frame_bins(st, audio + (size_t)b * L, L, t, live, lt, A, A + 512, mg, nullptr);
-    if (live && lt < st->n_mels) {
-        // meldataset.py:19-25: log(clip(x, 1e-5) * 1).  Not fmaxf, which returns 1e-5 for a NaN s: np.clip and torch.clamp
-        // keep NaN, and a NaN (or Inf) sample must not reach a mel loss as log(1e-5) silence.  Equal to fmaxf otherwise.
-        const float s = mel_band_sum(st, mg, lt);
-        mel[((size_t)b * st->n_mels + lt) * T + t] = logf(s < 1e-5f ? 1e-5f : s);
-    }
+    // the forward and the backward both run mel_frame_bins, so the backward differentiates the very magnitudes the forward summed
+    mel_frame_bins<kMelNfft>(st->win, st->tw, audio + (size_t)b * L, L, t * kMelHop - kMelPad, live, lt, A, A + 512, mg, nullptr);
+    if (live && lt < st->n_mels) mel[((size_t)b * st->n_mels + lt) * T + t] = mel_log(mel_band_sum(mel_bank(st), mg, lt));
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -144,9 +114,8 @@ __global__ void __launch_bounds__(256) mel_kernel(const MelTables *__restrict__ 
 // passes where s >= 1e-5, |0| has gradient 0, the rfft adjoint over bins 0..512 as the forward has them, padding dropped).
 //
 // mel_backward_frame_kernel, same CTA geometry as mel_kernel, per frame:
-//   recompute X and s with the forward's arithmetic  ->  gs_m = g_m / s_m (0 below the clip)  ->  dmag = M^T gs (filters
-//   of one parity never share a bin -- each triangle ends where the next-but-one starts -- so two passes, even then odd,
-//   accumulate without atomics)  ->  G[k] = dmag_k X_k / |X_k|  ->  adjoint of the even/odd split into dZ[0..511]  ->
+//   recompute X and s with the forward's arithmetic  ->  gs_m = g_m / s_m (0 below the clip)  ->  dmag = M^T gs and
+//   G[k] = dmag_k X_k / |X_k| (mel_band_adjoint, mg_mel_bank.cuh)  ->  adjoint of the even/odd split into dZ[0..511]  ->
 //   512-point inverse Stockham FFT (conjugate twiddles, unnormalised)  ->  times the window  ->  dframe[b][t][1024].
 // mel_backward_ola_kernel: grad_audio[b][i] = sum over the <= 4 frames covering padded sample i + 384, ascending t.
 //
@@ -170,28 +139,17 @@ __global__ void __launch_bounds__(256) mel_backward_frame_kernel(const MelTables
     const bool live = t < T;
     float2 *A = buf + fr * 1024, *Xk = Xall + fr * 516;
     float *mg = mag + fr * 516, *dm = dmag + fr * 516;
-    mel_frame_bins(st, audio + (size_t)b * L, L, t, live, lt, A, A + 512, mg, Xk);
+    mel_frame_bins<kMelNfft>(st->win, st->tw, audio + (size_t)b * L, L, t * kMelHop - kMelPad, live, lt, A, A + 512, mg, Xk);
     const int n_mels = st->n_mels;
+    const MelBank bk = mel_bank(st);
     float gs = 0.f;
     if (live && lt < n_mels) {
-        const float s = mel_band_sum(st, mg, lt);
+        const float s = mel_band_sum(bk, mg, lt);
         gs = s >= 1e-5f ? __ldg(grad_mel + ((size_t)b * n_mels + lt) * T + t) / s : 0.f;  // log' = 1 / s; clamp(min=)' = [s >= min]
     }
     for (int k = lt; k <= 512; k += 128) dm[k] = 0.f;
     __syncthreads();
-#pragma unroll 1
-    for (int parity = 0; parity < 2; ++parity) {
-        if (lt < n_mels && (lt & 1) == parity) {
-            const int ks = st->kstart[lt], kc = st->kcount[lt];
-            const float *w = st->weights + st->woff[lt];
-            for (int i = 0; i < kc; ++i) dm[ks + i] = fmaf(w[i], gs, dm[ks + i]);
-        }
-        __syncthreads();
-    }
-    for (int k = lt; k <= 512; k += 128) {  // abs' = X / |X|, and 0 at X = 0
-        const float m = mg[k], r = m > 0.f ? dm[k] / m : 0.f;
-        Xk[k] = make_float2(r * Xk[k].x, r * Xk[k].y);
-    }
+    mel_band_adjoint<kMelNfft, 128>(bk, n_mels, lt, [&](int) { return gs; }, dm, mg, Xk);  // band lt is this thread's
     __syncthreads();
     split_adjoint_pass<512, 128>(Xk, A, st->tw, lt);
     __syncthreads();

@@ -27,6 +27,7 @@
 
 #include "mg_common.cuh"
 #include "mg_fft.cuh"
+#include "mg_frame_loss.cuh"
 
 namespace mg {
 
@@ -48,8 +49,12 @@ int stft_tables_build(int n_fft, int win_length, void *tables_host) {
         return set_error(MG_ERR_INVALID_ARGUMENT, "%s: n_fft=%d is not a power of two in [%d, %d]", fn, n_fft, kStftMinN, kStftMaxN);
     if (win_length < 1 || win_length > n_fft)
         return set_error(MG_ERR_INVALID_ARGUMENT, "%s: win_length=%d is outside [1, n_fft=%d]", fn, win_length, n_fft);
+    stft_tables_fill(n_fft, win_length, reinterpret_cast<float *>(tables_host));
+    return MG_OK;
+}
+
+void stft_tables_fill(int n_fft, int win_length, float *win) {
     const double pi = 3.14159265358979323846;
-    float *win = reinterpret_cast<float *>(tables_host);
     float2 *tw = reinterpret_cast<float2 *>(win + n_fft);
     const int left = (n_fft - win_length) / 2;
     for (int n = 0; n < n_fft; ++n) {
@@ -58,7 +63,6 @@ int stft_tables_build(int n_fft, int win_length, void *tables_host) {
         win[n] = (j >= 0 && j < win_length) ? (win_length == 1 ? 1.f : (float)(0.5 - 0.5 * cos(2 * pi * j / win_length))) : 0.f;
     }
     for (int k = 0; k < n_fft / 2; ++k) tw[k] = make_float2((float)cos(2 * pi * k / n_fft), (float)-sin(2 * pi * k / n_fft));
-    return MG_OK;
 }
 
 int stft_frames(int n_fft, int hop, int L) {
@@ -91,19 +95,6 @@ __device__ __forceinline__ float2 stft_bin(const float2 *Z, const float2 *__rest
 
 __device__ __forceinline__ float stft_clamp(float m2) { return m2 < kStftFloor ? kStftFloor : m2; }
 
-// fixed-order sum of v over the CTA's 8 warps; the total is valid in thread 0
-__device__ __forceinline__ float stft_block_sum(float v, float *red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    float s = 0.f;
-    if (threadIdx.x == 0)
-        for (int w = 0; w < 8; ++w) s += red[w];
-    __syncthreads();
-    return s;
-}
-
 template <int N>
 __global__ void __launch_bounds__(256) stft_loss_fwd_kernel(const float *__restrict__ tab, const float *__restrict__ x,
                                                             const float *__restrict__ y, float *__restrict__ part, int L, int hop,
@@ -131,9 +122,9 @@ __global__ void __launch_bounds__(256) stft_loss_fwd_kernel(const float *__restr
         s_y = fmaf(ym, ym, s_y);
         s_log += fabsf(logf(ym) - logf(xm));
     }
-    s_diff = stft_block_sum(s_diff, red);
-    s_y = stft_block_sum(s_y, red);
-    s_log = stft_block_sum(s_log, red);
+    s_diff = block_sum256(s_diff, red);
+    s_y = block_sum256(s_y, red);
+    s_log = block_sum256(s_log, red);
     if (tid == 0) {
         part[f] = s_diff;  // 3 B T can pass 2^31: index in 64 bits
         part[(size_t)BT + f] = s_y;
@@ -148,30 +139,15 @@ struct StftFinishArgs {
     int n_res;
 };
 
-// float64 sum of p[0 .. n) over the CTA's 1024 threads in a fixed order; the total is valid in thread 0
-__device__ __forceinline__ double stft_sum64(const float *__restrict__ p, int n, double *red) {
-    double acc = 0.0;
-    for (int i = threadIdx.x; i < n; i += 1024) acc += (double)__ldg(p + i);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    double s = 0.0;
-    if (threadIdx.x == 0)
-        for (int w = 0; w < 32; ++w) s += red[w];
-    __syncthreads();
-    return s;
-}
-
 __global__ void __launch_bounds__(1024) stft_loss_finish_kernel(StftFinishArgs a, float *__restrict__ sc, float *__restrict__ mag,
                                                                 float *__restrict__ stats) {
     __shared__ double red[32];
     double sc_acc = 0.0, mag_acc = 0.0;
     for (int r = 0; r < a.n_res; ++r) {
         const int bt = a.bt[r];
-        const double s_diff = stft_sum64(a.part[r], bt, red);
-        const double s_y = stft_sum64(a.part[r] + bt, bt, red);
-        const double s_log = stft_sum64(a.part[r] + (size_t)2 * bt, bt, red);
+        const double s_diff = sum64_1024(a.part[r], bt, red);
+        const double s_y = sum64_1024(a.part[r] + bt, bt, red);
+        const double s_log = sum64_1024(a.part[r] + (size_t)2 * bt, bt, red);
         if (threadIdx.x == 0) {
             const double num = sqrt(s_diff), den = sqrt(s_y);
             stats[2 * r] = (float)num;
@@ -226,14 +202,6 @@ __global__ void __launch_bounds__(256) stft_loss_bwd_frame_kernel(const float *_
     for (int n = tid; n < M; n += 256) df[n] = make_float2(__ldg(win + 2 * n) * dz[n].x, __ldg(win + 2 * n + 1) * dz[n].y);
 }
 
-// sum of the frame gradients at padded position p over the frames t covering it, [t h, t h + N), ascending t
-__device__ __forceinline__ float stft_gather(const float *__restrict__ db, int p, int N, int hop, int T) {
-    const int t1 = min(p / hop, T - 1), t0 = p >= N ? (p - N) / hop + 1 : 0;
-    float acc = 0.f;
-    for (int t = t0; t <= t1; ++t) acc += __ldg(db + (size_t)t * N + (p - t * hop));
-    return acc;
-}
-
 __global__ void __launch_bounds__(256) stft_loss_bwd_gather_kernel(const float *__restrict__ dframe, float *__restrict__ grad_x, int L,
                                                                    int N, int hop, int T, int accumulate) {
     const int chunks = (L + 255) >> 8;
@@ -241,9 +209,9 @@ __global__ void __launch_bounds__(256) stft_loss_bwd_gather_kernel(const float *
     if (i >= L) return;
     const float *db = dframe + (size_t)b * T * N;
     const int h = N / 2;
-    float acc = stft_gather(db, i + h, N, hop, T);
-    if (i >= 1 && i <= h) acc += stft_gather(db, h - i, N, hop, T);
-    if (i >= L - 1 - h && i <= L - 2) acc += stft_gather(db, h + (L - 1) + (L - 1 - i), N, hop, T);
+    float acc = frame_gather(db, i + h, N, hop, T);
+    if (i >= 1 && i <= h) acc += frame_gather(db, h - i, N, hop, T);
+    if (i >= L - 1 - h && i <= L - 2) acc += frame_gather(db, h + (L - 1) + (L - 1 - i), N, hop, T);
     float *out = grad_x + (size_t)b * L + i;
     *out = accumulate ? *out + acc : acc;
 }

@@ -59,24 +59,27 @@ def build_tables(n_fft, win_length):
 
 
 class _Analysis:
-    """The resolutions of one module as the C calls take them, and each device's uploaded tables.  Tables are uploaded
-    with a copy from pageable host memory, which a CUDA graph capture forbids: tables() uploads them before any capture (the
-    module calls it from .to() / .cuda()), and a first call on a device inside a capture raises EngineError."""
+    """The resolutions of one loss module as the C calls take them, and each device's uploaded tables.  Tables are
+    uploaded with a copy from pageable host memory, which a CUDA graph capture forbids: tables() uploads them before any
+    capture (the module calls it from .to() / .cuda()), and a first call on a device inside a capture raises EngineError.
+    owner names the module in messages; workspace_call is its mg_*_workspace_bytes."""
 
-    def __init__(self, fft_sizes, hop_sizes, win_lengths):
+    def __init__(self, fft_sizes, hop_sizes, host, owner="MultiResolutionSTFTLoss", workspace_call=None):
         self.n = len(fft_sizes)
         self.n_fft = (ctypes.c_int * self.n)(*fft_sizes)
         self.hop = (ctypes.c_int * self.n)(*hop_sizes)
-        self.host = [build_tables(n, w) for n, w in zip(fft_sizes, win_lengths)]
+        self.host = host
+        self.owner = owner
+        self.workspace_call = workspace_call or _lib().mg_stft_loss_workspace_bytes
         self.device = {}
 
     def tables(self, device):
         d = self.device.get(device)
         if d is None:
             if torch.cuda.is_current_stream_capturing():
-                raise _engine.EngineError("MultiResolutionSTFTLoss: the tables for %s are not uploaded yet and a CUDA graph "
-                                          "capture forbids the copy; call the module once, or move it with .to(%s), before "
-                                          "capturing" % (device, device))
+                raise _engine.EngineError("%s: the tables for %s are not uploaded yet and a CUDA graph capture forbids the "
+                                          "copy; call the module once, or move it with .to(%s), before capturing"
+                                          % (self.owner, device, device))
             tabs = [torch.from_numpy(h).to(device) for h in self.host]
             d = (tabs, (ctypes.c_void_p * self.n)(*[t.data_ptr() for t in tabs]))
             self.device[device] = d
@@ -84,8 +87,20 @@ class _Analysis:
 
     def workspace_bytes(self, B, L):
         f, b = ctypes.c_size_t(), ctypes.c_size_t()
-        _engine.check(_lib().mg_stft_loss_workspace_bytes(self.n, self.n_fft, self.hop, B, L, ctypes.byref(f), ctypes.byref(b)))
+        _engine.check(self.workspace_call(self.n, self.n_fft, self.hop, B, L, ctypes.byref(f), ctypes.byref(b)))
         return f.value, b.value
+
+
+class _TablesModule(torch.nn.Module):
+    """A loss module whose .to(device) / .cuda() upload its _Analysis's tables there, so a first call inside a CUDA
+    graph capture finds them."""
+
+    def _apply(self, fn, *args, **kwargs):
+        out = super()._apply(fn, *args, **kwargs)
+        dev = fn(torch.empty(0)).device
+        if dev.type == "cuda":
+            self._an.tables(torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device()))
+        return out
 
 
 def _workspace(nbytes, device):
@@ -135,7 +150,7 @@ class _STFTLoss(torch.autograd.Function):
         return grad, None, None
 
 
-class MultiResolutionSTFTLoss(torch.nn.Module):
+class MultiResolutionSTFTLoss(_TablesModule):
     """Parallel WaveGAN's multi-resolution STFT loss: ``forward(x, y) -> (sc_loss, mag_loss)`` for predicted audio x and
     target audio y, fp32 CUDA tensors [B, L] of one shape.  The module has no parameters; it keeps each device's tables.
 
@@ -163,15 +178,7 @@ class MultiResolutionSTFTLoss(torch.nn.Module):
             if not 1 <= w <= n:
                 raise _engine.EngineError("MultiResolutionSTFTLoss: win_length %d outside [1, fft_size %d]" % (w, n))
         self.fft_sizes, self.hop_sizes, self.win_lengths = fft_sizes, hop_sizes, win_lengths
-        self._an = _Analysis(fft_sizes, hop_sizes, win_lengths)
-
-    def _apply(self, fn, *args, **kwargs):
-        # .to(device) / .cuda() upload the tables there, so a first call inside a CUDA graph capture finds them
-        out = super()._apply(fn, *args, **kwargs)
-        dev = fn(torch.empty(0)).device
-        if dev.type == "cuda":
-            self._an.tables(torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device()))
-        return out
+        self._an = _Analysis(fft_sizes, hop_sizes, [build_tables(n, w) for n, w in zip(fft_sizes, win_lengths)])
 
     def forward(self, x, y):
         for name, t in (("x", x), ("y", y)):
