@@ -480,6 +480,42 @@ int mg_mel_loss_backward(int n_res, const void *const *tables, const int *n_fft,
                          int L, const float *grad, float *grad_x, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Denoiser (WaveGlow's Denoiser): subtract a vocoder's bias spectrum from its audio.  audio [B][L_max] device fp32; item i
+ * owns its first L_i = lengths[i] samples (lengths NULL: every item L_max) and uses bias row voice[i] (voice NULL: row 0)
+ * of bias [n_voices][n_fft/2 + 1] device fp32.  With N = n_fft, H = hop, W = win_length and, in float64 terms,
+ *   S  = torch.stft(a_i[:L_i], N, H, W, periodic Hann(W), center=True, pad_mode="reflect"), 1 + L_i / H frames;
+ *   M' = max(|S| - strength bias[voice[i]], 0)  (written `x < 0 ? 0 : x`: NaN stays NaN);
+ *   P  = S / |S| where |S| > 0, else 1;
+ *   out_i[:L_i] = torch.istft(M' P, N, H, W, periodic Hann(W), center=True, length=L_i), out_i[L_i:] = 0.
+ * tables: the STFT loss's table for (n_fft, win_length) (mg_stft_loss_tables_build), on the device, 16-byte aligned.
+ * Supported: N a power of two in [128, 2048], 1 <= H <= W <= N (torch.istft's limit), N/2 < L_i <= L_max <= 2^30, any (N, H, W, L_i) whose
+ * window-square envelope stays >= 1e-11 at every output sample some frame reaches (torch.istft's NOLA condition, checked
+ * on the host in float64 for each distinct length), B <= MG_GEN_RAGGED_MAX_B when lengths or voice is given.
+ *   mg_denoise_workspace_bytes: the frame workspace, sum_i (1 + L_i / H) N floats (each frame resynthesised and windowed).
+ *   mg_denoise_bias writes bias [n_rows][N/2 + 1] = |X[k]| of frame 0 of each row of audio [n_rows][L] (the same frame,
+ *     FFT and bins as the forward): WaveGlow's bias spectrum of a generator's audio.  1 <= n_rows <= 65535.
+ *   mg_denoise_forward writes out [B][L_max], every element; mg_denoise_forward_pcm16 writes int16 out, pcm16 of the
+ *     float output (mg_gen_forward_pcm16's rounding, by the same kernel).  Each output sample sums its frames and the
+ *     window-square envelope in ascending frame order: no atomics, the same inputs give the same bits on every run, and
+ *     each item's samples are those of its own B = 1 call.  win_length must be the one the tables were built with.
+ * Asynchronous on `stream`, no host synchronisation (capturable in a CUDA graph); concurrent calls need their own
+ * workspaces.  NaN and Inf samples are not clamped away: a non-finite sample makes its frames non-finite, hence the output
+ * samples those frames reach.  Refused with MG_ERR_INVALID_ARGUMENT before any CUDA call, with a message naming the
+ * argument: an unsupported n_fft, hop < 1, win_length outside [1, n_fft], hop > win_length, B < 1, L_max > 2^30, a length outside
+ * (n_fft/2, L_max], a ragged or voiced batch of more than MG_GEN_RAGGED_MAX_B items, n_voices < 1, a voice outside
+ * [0, n_voices), a non-finite strength, a NULL or misaligned pointer (tables and workspace 16 bytes, float 4, int16 2), a
+ * grid past 2^31 - 1 CTAs, the NOLA condition; a short workspace with MG_ERR_WORKSPACE_TOO_SMALL.
+ */
+int mg_denoise_workspace_bytes(int n_fft, int hop, int B, int L_max, const int *lengths, size_t *bytes);
+int mg_denoise_bias(const void *tables, int n_fft, const float *audio, int n_rows, int L, float *bias, void *stream);
+int mg_denoise_forward(const void *tables, int n_fft, int hop, int win_length, const float *audio, int B, int L_max, const int *lengths,
+                       const float *bias, int n_voices, const int *voice, float strength, float *out, void *workspace,
+                       size_t workspace_bytes, void *stream);
+int mg_denoise_forward_pcm16(const void *tables, int n_fft, int hop, int win_length, const float *audio, int B, int L_max,
+                             const int *lengths, const float *bias, int n_voices, const int *voice, float strength, int16_t *out,
+                             void *workspace, size_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Host-buffer engine.   The call a non-PyTorch host makes: owns its device buffers, takes and
  * returns HOST memory, and performs the host<->device copies itself (this is the path
  * bench.py times as "e2e").  One engine per host thread / CUDA stream.

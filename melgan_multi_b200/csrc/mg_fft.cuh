@@ -1,7 +1,7 @@
 // Radix-2 Stockham FFT pieces shared by the mel front end (mg_mel.cu) and the multi-resolution STFT loss
-// (mg_stft_loss.cu).  A real frame of N = 2M samples is transformed as the M-point complex sequence
-// z[n] = x[2n] + i x[2n+1]; real_split turns its transform Z into the bins X[0..M] of the real transform, and
-// split_adjoint_pass is the adjoint of that split.  Twiddle tables hold tw[k] = e^{-2 pi i k / N} for k < M.
+// (mg_stft_loss.cu), the mel loss (mg_mel_loss.cu) and the denoiser (mg_denoise.cu).  A real frame of N = 2M samples is
+// transformed as the M-point complex sequence z[n] = x[2n] + i x[2n+1]; real_split turns its transform Z into the bins
+// X[0..M] of the real transform, real_unsplit is its inverse and split_adjoint_pass its adjoint.  Twiddle tables hold tw[k] = e^{-2 pi i k / N} for k < M.
 // Every function is called by all NT threads of a group together (they hold __syncthreads).
 #pragma once
 
@@ -46,6 +46,17 @@ __device__ __forceinline__ float2 real_split(const float2 zk, const float2 zc, c
     const float2 E = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y - zc.y));
     const float2 O = make_float2(0.5f * (zk.y + zc.y), -0.5f * (zk.x - zc.x));
     return make_float2(E.x + w.x * O.x - w.y * O.y, E.y + w.x * O.y + w.y * O.x);
+}
+
+// Inverse of the split: Z[k] = E + i O with E = (X[k] + conj X[M-k]) / 2, O = (X[k] - conj X[M-k]) conj(W^k) / 2, from
+// xk = X[k], xc = X[M - k] and w = W^k, k = 0..M-1; the M-point inverse pass of Z gives M (x[2n] + i x[2n+1]).  At k = 0
+// (xc = X[M]) the imaginary parts of X[0] and X[M] are dropped, as irfft drops them.
+__device__ __forceinline__ float2 real_unsplit(float2 xk, float2 xc, const float2 w, bool k0) {
+    if (k0) xk.y = xc.y = 0.f;
+    const float2 E = make_float2(0.5f * (xk.x + xc.x), 0.5f * (xk.y - xc.y));
+    const float2 D = make_float2(0.5f * (xk.x - xc.x), 0.5f * (xk.y + xc.y));  // (X[k] - conj X[M-k]) / 2
+    const float2 O = make_float2(D.x * w.x + D.y * w.y, D.y * w.x - D.x * w.y);  // D conj(w)
+    return make_float2(E.x - O.y, E.y + O.x);
 }
 
 // Adjoint of the split, with a_k = (1 - i W^k) / 2, b_k = (1 + i W^k) / 2, X[k] = a_k Z[k mod M] + b_k conj Z[(M - k) mod M]:

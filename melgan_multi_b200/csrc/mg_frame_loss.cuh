@@ -1,5 +1,6 @@
 // Fixed-order reductions and the frame-gradient gather shared by the multi-resolution STFT loss (mg_stft_loss.cu) and
-// the multi-resolution mel loss (mg_mel_loss.cu).  No atomics: every sum has the same bits on every run.
+// the multi-resolution mel loss (mg_mel_loss.cu), and the denoiser's overlap-add (mg_denoise.cu).  No atomics: every
+// sum has the same bits on every run.
 #pragma once
 
 namespace mg {
@@ -38,6 +39,22 @@ __device__ __forceinline__ float frame_gather(const float *__restrict__ db, int 
     float acc = 0.f;
     for (int t = t0; t <= t1; ++t) acc += __ldg(db + (size_t)t * N + (p - t * hop));
     return acc;
+}
+
+// frame_gather's sum and, in the same loop and order, the window-square envelope sum win[p - t h]^2 (the overlap-add
+// of an inverse STFT); false when no frame covers p
+__device__ __forceinline__ bool frame_gather_env(const float *__restrict__ db, const float *__restrict__ win, int p, int N, int hop,
+                                                 int T, float &acc, float &env) {
+    const int t1 = min(p / hop, T - 1), t0 = p >= N ? (p - N) / hop + 1 : 0;
+    acc = 0.f;
+    env = 0.f;
+    for (int t = t0; t <= t1; ++t) {
+        const int n = p - t * hop;
+        const float w = __ldg(win + n);
+        acc += __ldg(db + (size_t)t * N + n);
+        env = fmaf(w, w, env);
+    }
+    return t0 <= t1;
 }
 
 }  // namespace mg
