@@ -515,6 +515,68 @@ int mg_denoise_forward_pcm16(const void *tables, int n_fft, int hop, int win_len
                              const int *lengths, const float *bias, int n_voices, const int *voice, float strength, int16_t *out,
                              void *workspace, size_t workspace_bytes, void *stream);
 
+/* Streaming denoiser: mg_denoise_forward applied to live audio.  A handle serves up to max_sessions (<= MG_GEN_RAGGED_MAX_B)
+ * slots at one analysis (n_fft N, hop H, win_length W) and one strength.  Each mg_denoise_stream_step gives slot i (i < n)
+ * in_samples[i] in [0, max_push_samples] new fp32 samples and flags[i] (flags NULL: all 0), with mg_gen_stream_step's
+ * meaning: MG_GEN_STREAM_RESET drops the slot's unfinished utterance first, MG_GEN_STREAM_END ends it after these samples.
+ * It writes the slot's newly final denoised samples to out[i][0 .. out_samples[i]).
+ * The finality rule.  With R the samples an open utterance has received: frame t reads samples [t H - N/2, t H + N/2)
+ * reflected at 0 (frame 0 reads 0 .. N/2), so frames 0 .. q, q = floor((R - N/2) / H), are computable once R > N/2.
+ * Output sample j sums frames up to floor((j + N/2) / H) <= q, so exactly
+ *     E(R) = 0 if R <= N/2, else clamp((q + 1) H - N/2, 0, R)
+ * samples have been emitted over the utterance's steps; R - E(R) lies in [N - H, N - 1] in steady state (768 .. 1023
+ * samples at N = 1024, H = 256).  The rule follows the frames the kernel sums, not the window's support: a later frame's
+ * term is added even where the window is 0, so a NaN or Inf reaches exactly the samples it reaches in mg_denoise_forward.
+ * After the END step, at length L, all L samples have been emitted (frames up to floor(L / H) reflect at L; samples no
+ * frame reaches when H > N/2 are 0) and the slot is free.  The concatenation of an utterance's outputs is bit-identical to
+ * mg_denoise_forward of its L samples (same tables, bias row, strength) for any push schedule, 0- and 1-sample pushes
+ * included; mg_denoise_stream_step_pcm16 writes int16 out, pcm16 of what the float step writes (the format is chosen per
+ * step and may alternate on one handle).
+ * Arguments:
+ *   tables: the STFT loss's table for (n_fft, win_length) on the device; bias [n_voices][N/2 + 1] device fp32
+ *   voice: HOST array of n ids in [0, n_voices) (NULL: all 0).  A slot's bias row binds on the step that opens its
+ *          utterance and is released at END or RESET; a changed id on an open slot without RESET is refused, as in
+ *          mg_gen_stream_step_voices.
+ *   audio_in [n][in_stride] device fp32: slot i's new samples are audio_in[i][0 .. in_samples[i]) (in_samples[i] <=
+ *          in_stride); may be NULL when every in_samples[i] is 0.  mg_gen_stream_step's audio [n][mg_gen_stream_max_out(P)]
+ *          with its out_samples is a valid (audio_in, in_stride, in_samples) as it is.
+ *   in_samples, flags, out_samples: HOST arrays; out_samples is filled before the call returns.  The step derives every
+ *          count and launch from sample counts alone, enqueues its work on `stream` and never synchronises or reads the
+ *          device.
+ *   out [n][mg_denoise_stream_max_out(N, H, max_push_samples)] device fp32 (int16 for _pcm16): only out[i][0 ..
+ *          out_samples[i]) is written.  max_out = max_push_samples + N - 1, reached by an END push of max_push_samples
+ *          when R - E(R) = N - 1.
+ *   state: caller-owned device memory of mg_denoise_stream_state_bytes(N, H, max_sessions, max_push_samples) bytes,
+ *          256-byte aligned, for the lifetime of the handle and not shared with another handle: each session's tail of
+ *          at most N samples, its window and a ring of the frames its pending samples need.  No step lets a byte an
+ *          earlier step has not written reach an output, so its initial contents do not matter.
+ * Supported: N a power of two in [128, 2048], 1 <= H <= W <= N, max_push_samples in [1, 2^20], utterances of
+ * N/2 < L <= 2^30 samples.  create refuses the length-independent part of torch.istft's NOLA condition (a residue mod H
+ * whose window-square sum is below 1e-11), the END step the rest, at the utterance's length.  Refused with
+ * MG_ERR_INVALID_ARGUMENT before any CUDA call, with a message naming the argument, and leaving the counters unchanged:
+ * a bad analysis, max_sessions or max_push_samples, a non-finite strength, n outside [0, max_sessions], n_voices < 1, an
+ * id out of range or changed on an open slot, in_samples outside [0, max_push_samples] or past in_stride, unknown flag
+ * bits, END on a slot with no samples or at L <= N/2, an utterance past 2^30 samples, the NOLA condition, a NULL or
+ * misaligned pointer (state 256 bytes, tables 16, float 4, int16 2); a short state with MG_ERR_WORKSPACE_TOO_SMALL.  One
+ * thread drives a handle at a time; its steps must be enqueued on one stream (or otherwise ordered).
+ * mg_denoise_stream_dry_step advances the counters exactly as a step would, with no device and no pointer, and reports
+ * out_samples and the frames the step would compute (new_frames, may be NULL); a handle advanced this way refuses later
+ * real steps. */
+typedef struct mg_denoise_stream mg_denoise_stream; /* host-side counters only */
+size_t mg_denoise_stream_state_bytes(int n_fft, int hop, int max_sessions, int max_push_samples);
+int mg_denoise_stream_max_out(int n_fft, int hop, int max_push_samples);
+int mg_denoise_stream_create(mg_denoise_stream **out, int n_fft, int hop, int win_length, int max_sessions, int max_push_samples,
+                             float strength, void *state, size_t state_bytes);
+void mg_denoise_stream_destroy(mg_denoise_stream *s);
+int mg_denoise_stream_step(mg_denoise_stream *s, const void *tables, const float *bias, int n_voices, const int *voice,
+                           const float *audio_in, long long in_stride, const int *in_samples, const int *flags, int n, float *out,
+                           int *out_samples, void *stream);
+int mg_denoise_stream_step_pcm16(mg_denoise_stream *s, const void *tables, const float *bias, int n_voices, const int *voice,
+                                 const float *audio_in, long long in_stride, const int *in_samples, const int *flags, int n, int16_t *out,
+                                 int *out_samples, void *stream);
+int mg_denoise_stream_dry_step(mg_denoise_stream *s, int n_voices, const int *voice, const int *in_samples, const int *flags, int n,
+                               int *out_samples, int *new_frames);
+
 /* ---------------------------------------------------------------------------------------
  * Host-buffer engine.   The call a non-PyTorch host makes: owns its device buffers, takes and
  * returns HOST memory, and performs the host<->device copies itself (this is the path

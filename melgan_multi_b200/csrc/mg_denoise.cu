@@ -9,7 +9,7 @@
 //   f N in the workspace.  The frame is read reflecting at the item's own length, through the forward FFT and split of
 //   mg_stft_frame.cuh; each bin becomes Y; real_unsplit and the inverse Stockham pass give the real frame, which is
 //   scaled by 1 / M (M = N / 2: the pass returns M times the samples; exact, M is a power of two) and multiplied by the
-//   window.
+//   window.  The frame's code is MG_DENOISE_FRAME (mg_denoise.cuh), which the streaming denoiser's frame kernel expands too.
 // denoise_ola_kernel<S>: one thread per output sample: the frames covering its padded position and the window-square
 //   envelope, both summed in ascending frame order (frame_gather_env), then their quotient stored as audio_sample<S>
 //   (S float or int16_t); 0 from L_i to L_max, and 0 where no frame reaches (torch.istft's zero fill past the last frame
@@ -21,17 +21,12 @@
 #include <vector>
 
 #include "mg_common.cuh"
+#include "mg_denoise.cuh"
 #include "mg_fft.cuh"
 #include "mg_frame_loss.cuh"
 #include "mg_stft_frame.cuh"
 
 namespace mg {
-
-constexpr int kDnMinN = 128, kDnMaxN = 2048;
-constexpr int kDnMaxL = 1 << 30;   // keeps every sample, padded position and 2 (L - 1) inside int
-constexpr double kDnNola = 1e-11;  // torch.istft's least window-square envelope
-
-static bool dn_n_ok(int n) { return n >= kDnMinN && n <= kDnMaxN && (n & (n - 1)) == 0; }
 
 template <int N>
 __global__ void __launch_bounds__(128) denoise_bias_kernel(const float *__restrict__ tab, const float *__restrict__ audio, int L,
@@ -51,31 +46,12 @@ template <int N>
 __global__ void __launch_bounds__(128) denoise_frame_kernel(const float *__restrict__ tab, const float *__restrict__ audio, int hop,
                                                             float strength, float *__restrict__ frames,
                                                             const __grid_constant__ RunTable run) {
-    constexpr int M = N / 2;
-    __shared__ __align__(16) float2 buf[2 * M];
-    __shared__ __align__(16) float2 Y[M + 1];
+    __shared__ __align__(16) float2 buf[N];
+    __shared__ __align__(16) float2 Y[N / 2 + 1];
     const int lt = threadIdx.x, f = blockIdx.x;
     const RunPos at = run.find(f);  // the grid is first[n] frames, with no gaps: every frame belongs to an item
     const float *__restrict__ b = run.blob_at(f);
-    const float *win = tab;
-    const float2 *tw = reinterpret_cast<const float2 *>(tab + N);
-    const float2 *Z = stft_frame<N>(win, tw, audio + (size_t)at.item * run.stride, at.len, at.unit * hop, lt, buf, buf + M);
-    for (int k = lt; k <= M; k += 128) {
-        const float2 X = stft_bin<N>(Z, tw, k);
-        const float m = sqrtf(X.x * X.x + X.y * X.y), d = m - strength * __ldg(b + k);
-        const float mc = d < 0.f ? 0.f : d;  // NaN stays NaN
-        const float r = mc / m;
-        Y[k] = m > 0.f ? make_float2(r * X.x, r * X.y) : make_float2(mc, 0.f);  // |X| = 0: phase 0
-    }
-    __syncthreads();
-    float2 *A = Z == buf ? buf + M : buf;  // the buffer Z is not in (Z is read no more)
-    for (int k = lt; k < M; k += 128) A[k] = real_unsplit(Y[k], Y[M - k], k ? __ldg(tw + k) : make_float2(1.f, 0.f), k == 0);
-    __syncthreads();
-    const float2 *z = stockham<M, 128, true>(A, A == buf ? buf + M : buf, tw, lt);
-    constexpr float inv = 1.f / M;
-    float2 *out = reinterpret_cast<float2 *>(frames + (size_t)f * N);
-    for (int n = lt; n < M; n += 128)
-        out[n] = make_float2(__ldg(win + 2 * n) * (z[n].x * inv), __ldg(win + 2 * n + 1) * (z[n].y * inv));
+    MG_DENOISE_FRAME(N, tab, audio + (size_t)at.item * run.stride, at.len, at.unit * hop, strength, b, frames + (size_t)f * N, lt, buf, Y)
 }
 
 template <class S>
@@ -102,7 +78,17 @@ __global__ void __launch_bounds__(256) denoise_ola_kernel(const float *__restric
 
 // ---- host side -------------------------------------------------------------------------------------------------------
 
-static int dn_frames(int hop, int L) { return 1 + L / hop; }
+void dn_window_sq(int n_fft, int hop, int win_length, std::vector<double> &w2, std::vector<double> &full) {
+    const double pi = 3.14159265358979323846;
+    const int left = (n_fft - win_length) / 2;
+    w2.assign(n_fft, 0.0);
+    for (int j = 0; j < win_length; ++j) {
+        const double w = win_length == 1 ? 1.0 : 0.5 - 0.5 * cos(2 * pi * j / win_length);
+        w2[left + j] = w * w;
+    }
+    full.assign(std::min(hop, n_fft), 0.0);
+    for (int n = 0; n < n_fft; ++n) full[n % hop] += w2[n];
+}
 
 // float64 window-square envelope of torch.istft at padded position p of a T-frame signal, w2 = the squared window
 static double dn_env_at(const std::vector<double> &w2, int N, int hop, int T, long long p) {
@@ -115,7 +101,7 @@ static double dn_env_at(const std::vector<double> &w2, int N, int hop, int T, lo
 // the first output sample (of an L-sample item) whose envelope is below 1e-11, or -1: torch.istft's NOLA check, over the
 // output positions some frame reaches.  Interior positions (every frame position n = p mod hop present) read the
 // per-residue sums `full`, so the cost is O(N^2 / hop + N), not O(L).
-static long long dn_nola_fail(const std::vector<double> &w2, const std::vector<double> &full, int N, int hop, int L) {
+long long dn_nola_fail(const std::vector<double> &w2, const std::vector<double> &full, int N, int hop, int L) {
     const int T = dn_frames(hop, L);
     const long long start = N / 2, end = std::min<long long>((long long)N / 2 + L, (long long)N + (long long)hop * (T - 1));
     const long long i0 = std::max<long long>(start, N - 1), i1 = std::min<long long>(end, (long long)hop * T);  // interior
@@ -137,7 +123,7 @@ static long long dn_nola_fail(const std::vector<double> &w2, const std::vector<d
     return -1;
 }
 
-static int dn_check_pointer(const char *fn, const char *name, const void *p, unsigned align) {
+int dn_check_pointer(const char *fn, const char *name, const void *p, unsigned align) {
     if (!p) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %s is NULL", fn, name);
     if ((uintptr_t)p % align) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: %s must be %u-byte aligned", fn, name, align);
     return MG_OK;
@@ -187,15 +173,8 @@ static int denoise_forward(const char *fn, const void *tables, int n_fft, int ho
                 return set_error(MG_ERR_INVALID_ARGUMENT, "%s: voice[%d]=%d is outside [0, n_voices=%d)", fn, i, voice[i], n_voices);
     if (!isfinite(strength)) return set_error(MG_ERR_INVALID_ARGUMENT, "%s: strength=%g is not finite", fn, (double)strength);
     // torch.istft's NOLA refusal, in float64, once per distinct length
-    std::vector<double> w2(n_fft, 0.0), full;
-    const double pi = 3.14159265358979323846;
-    const int left = (n_fft - win_length) / 2;
-    for (int j = 0; j < win_length; ++j) {
-        const double w = win_length == 1 ? 1.0 : 0.5 - 0.5 * cos(2 * pi * j / win_length);
-        w2[left + j] = w * w;
-    }
-    full.assign(std::min(hop, n_fft), 0.0);
-    for (int n = 0; n < n_fft; ++n) full[n % hop] += w2[n];
+    std::vector<double> w2, full;
+    dn_window_sq(n_fft, hop, win_length, w2, full);
     std::vector<int> seen;
     for (int i = 0; i < B; ++i) {
         const int L = lengths ? lengths[i] : L_max;

@@ -41,20 +41,38 @@ __device__ __forceinline__ float frame_gather(const float *__restrict__ db, int 
     return acc;
 }
 
+// where frame t of a frame_gather_env sum lives: frames stored one after another (the batch denoiser), or in a ring of
+// K slots, frame t in slot t mod K (the streaming denoiser's per-session frames)
+struct FramesLinear {
+    const float *__restrict__ db;
+    int N;
+    __device__ __forceinline__ const float *operator()(int t) const { return db + (size_t)t * N; }
+};
+struct FramesRing {
+    const float *__restrict__ db;
+    int N, K;
+    __device__ __forceinline__ const float *operator()(int t) const { return db + (size_t)(t % K) * N; }
+};
+
 // frame_gather's sum and, in the same loop and order, the window-square envelope sum win[p - t h]^2 (the overlap-add
-// of an inverse STFT); false when no frame covers p
-__device__ __forceinline__ bool frame_gather_env(const float *__restrict__ db, const float *__restrict__ win, int p, int N, int hop,
-                                                 int T, float &acc, float &env) {
+// of an inverse STFT); false when no frame covers p.  frame(t): frame t's N floats
+template <class Frames>
+__device__ __forceinline__ bool frame_gather_env(Frames frame, const float *__restrict__ win, int p, int N, int hop, int T, float &acc,
+                                                 float &env) {
     const int t1 = min(p / hop, T - 1), t0 = p >= N ? (p - N) / hop + 1 : 0;
     acc = 0.f;
     env = 0.f;
     for (int t = t0; t <= t1; ++t) {
         const int n = p - t * hop;
         const float w = __ldg(win + n);
-        acc += __ldg(db + (size_t)t * N + n);
+        acc += __ldg(frame(t) + n);
         env = fmaf(w, w, env);
     }
     return t0 <= t1;
+}
+__device__ __forceinline__ bool frame_gather_env(const float *__restrict__ db, const float *__restrict__ win, int p, int N, int hop,
+                                                 int T, float &acc, float &env) {
+    return frame_gather_env(FramesLinear{db, N}, win, p, N, hop, T, acc, env);
 }
 
 }  // namespace mg

@@ -6,7 +6,8 @@ a standard-normal one (``mode="normal"``), ``[1, 80, 88]``, one row per voice.  
 ``S = torch.stft(a, n_fft, hop, win_length, hann, center=True, pad_mode="reflect")``, subtracts ``strength * bias``
 from ``|S|``, clamps at 0, keeps the phase of S (phase 0 where ``|S| = 0``) and returns
 ``torch.istft(..., length=L)``: every step on the package's own kernels, for uniform, ragged and multi-voice batches,
-in fp32 or 16-bit PCM.  Inference only.  CUDA only, like the rest of the package: there is no CPU fallback.
+in fp32 or 16-bit PCM.  ``Denoiser.stream`` applies the same denoiser to live audio, each session's samples
+emitted once final and bit-identical to ``forward`` of the whole utterance.  Inference only.  CUDA only, like the rest of the package: there is no CPU fallback.
 """
 import ctypes
 import math
@@ -39,6 +40,24 @@ def _lib():
         f.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                       ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p,
                       ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+    L.mg_denoise_stream_state_bytes.restype = ctypes.c_size_t
+    L.mg_denoise_stream_state_bytes.argtypes = [ctypes.c_int] * 4
+    L.mg_denoise_stream_max_out.restype = ctypes.c_int
+    L.mg_denoise_stream_max_out.argtypes = [ctypes.c_int] * 3
+    L.mg_denoise_stream_create.restype = ctypes.c_int
+    L.mg_denoise_stream_create.argtypes = [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                           ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t]
+    L.mg_denoise_stream_destroy.restype = None
+    L.mg_denoise_stream_destroy.argtypes = [ctypes.c_void_p]
+    for name in ("mg_denoise_stream_step", "mg_denoise_stream_step_pcm16"):
+        f = getattr(L, name)
+        f.restype = ctypes.c_int
+        f.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                      ctypes.c_longlong, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                      ctypes.c_void_p]
+    L.mg_denoise_stream_dry_step.restype = ctypes.c_int
+    L.mg_denoise_stream_dry_step.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                             ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
     _LIB = L
     return L
 
@@ -167,3 +186,127 @@ class Denoiser(_TablesModule):
             _engine.check(call(tabs[0], n, h, self.win_length, x.data_ptr(), B, L, lens, self.bias_spec.data_ptr(), V, ids, strength,
                                out.data_ptr(), ws.data_ptr(), nbytes.value, torch.cuda.current_stream().cuda_stream))
         return out.reshape(shape)
+
+    def stream(self, max_sessions=1, max_push_samples=256 * 32 + 1542, strength=0.1, dtype=torch.float32, state=None):
+        """A DenoiserStream of this denoiser: up to max_sessions live sessions, at most max_push_samples new samples per
+        session and step (the default takes GeneratorStream's output at its default max_push_frames=32), one strength for
+        the handle's lifetime.  dtype: the default output format, torch.float32 or torch.int16."""
+        return DenoiserStream(self, max_sessions, max_push_samples, strength, dtype, state)
+
+
+class DenoiserStream:
+    """Denoising of up to ``max_sessions`` live audio streams (mg_denoise_stream_*, contract in include/melgan_b200.h).
+    Each step takes each session's newly received samples and returns the denoised samples that became final: E(R) of
+    them once R samples have been received (E(R) = 0 for R <= n_fft / 2, else clamp((q + 1) hop - n_fft / 2, 0, R),
+    q = (R - n_fft / 2) // hop), all L after the step that ends the utterance; their concatenation equals
+    ``Denoiser.forward`` of the whole utterance bit for bit (same bias row and strength), in fp32 and int16.
+
+    The bias and tables are read from the denoiser at every step, so refresh() between steps takes effect; the handle's
+    state lives on the device the denoiser was on when the stream was opened, and a step after the denoiser was moved
+    with .to() to another device is refused.  Chaining after a GeneratorStream needs no copy::
+
+        a, c = gs.step_packed(mel, frames, flags, voice=v)
+        y, m = ds.step_packed(a, c, flags, voice=v)
+
+    One thread drives a handle at a time, and its steps must be enqueued on one CUDA stream (or otherwise ordered)."""
+
+    def __init__(self, denoiser, max_sessions, max_push_samples, strength, dtype, state):
+        self._dn = denoiser
+        self.dtype = dtype
+        _engine._pcm16(dtype)
+        self.device = denoiser.bias_spec.device
+        if self.device.type != "cuda":
+            raise _engine.EngineError("Denoiser.stream: the denoiser is on %s; it needs CUDA (no CPU fallback)" % (self.device,))
+        self.strength = float(strength)
+        if not math.isfinite(self.strength):
+            raise _engine.EngineError("Denoiser.stream: strength %r is not finite" % (self.strength,))
+        self.max_sessions, self.max_push_samples = int(max_sessions), int(max_push_samples)
+        n, h = denoiser.n_fft, denoiser.hop
+        L = _lib()
+        nbytes = L.mg_denoise_stream_state_bytes(n, h, self.max_sessions, self.max_push_samples)
+        if nbytes == 0:
+            raise _engine.EngineError("Denoiser.stream: max_sessions must lie in [1, 256] and max_push_samples in [1, 2^20]")
+        if state is None:
+            state = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        if state.device != self.device or state.numel() * state.element_size() < nbytes or not state.is_contiguous():
+            raise _engine.EngineError("Denoiser.stream: state must be a contiguous CUDA tensor of at least %d bytes on %s"
+                                      % (nbytes, self.device))
+        self.state = state
+        self.max_out = L.mg_denoise_stream_max_out(n, h, self.max_push_samples)
+        self._h = ctypes.c_void_p()
+        _engine.check(L.mg_denoise_stream_create(ctypes.byref(self._h), n, h, denoiser.win_length, self.max_sessions,
+                                                 self.max_push_samples, self.strength, state.data_ptr(),
+                                                 state.numel() * state.element_size()))
+        self._in = torch.zeros((self.max_sessions, self.max_push_samples), dtype=torch.float32, device=self.device)
+
+    def step_packed(self, audio, counts, flags=None, voice=None, out=None):
+        """The C step on a packed buffer: audio [n, stride] fp32 CUDA (slot i's new samples first, e.g. GeneratorStream's
+        output), counts: n sample counts, flags: None or n ints (STREAM_END / STREAM_RESET), voice: None (bias row 0) or n
+        bias rows.  Returns (out [n, max_out], per-slot sample counts as a list of ints).  out: None (a new tensor of the
+        handle's dtype) or a contiguous fp32 or int16 CUDA tensor [n, max_out], whose dtype picks this step's format."""
+        n = len(counts)
+        if not self._h:
+            raise _engine.EngineError("DenoiserStream: the stream is closed")
+        bias = self._dn.bias_spec
+        if bias.device != self.device:
+            raise _engine.EngineError("DenoiserStream: the denoiser was moved to %s, this stream's state is on %s (open a new "
+                                      "stream after .to())" % (bias.device, self.device))
+        if audio is not None and (not torch.is_tensor(audio) or audio.device != self.device or audio.dtype != torch.float32
+                                  or audio.dim() != 2 or audio.shape[0] < n or audio.stride(1) != 1):
+            raise _engine.EngineError("DenoiserStream: audio must be an fp32 [n, stride] tensor on %s with unit-stride rows"
+                                      % (self.device,))
+        ids = None if voice is None else _engine._voice_ids(voice, n, bias.shape[0])
+        if out is None:
+            out = torch.empty((n, self.max_out), dtype=self.dtype, device=self.device)
+        if out.dtype not in (torch.float32, torch.int16) or out.device != self.device or out.dim() != 2 or out.shape[0] < n \
+                or out.shape[1] != self.max_out or not out.is_contiguous():
+            raise _engine.EngineError("DenoiserStream: out must be a contiguous fp32 or int16 [%d, %d] tensor on %s"
+                                      % (n, self.max_out, self.device))
+        cnt_in = (ctypes.c_int * max(n, 1))(*[int(v) for v in counts])
+        fl = (ctypes.c_int * max(n, 1))(*[int(v) for v in flags]) if flags is not None else None
+        cnt = (ctypes.c_int * max(n, 1))()
+        with torch.cuda.device(self.device):
+            tabs = self._dn._an.tables(self.device)
+            L = _lib()
+            fn = L.mg_denoise_stream_step_pcm16 if out.dtype == torch.int16 else L.mg_denoise_stream_step
+            _engine.check(fn(self._h, tabs[0], bias.data_ptr(), bias.shape[0], ids, audio.data_ptr() if audio is not None else None,
+                             audio.stride(0) if audio is not None else 0, cnt_in, fl, n, out.data_ptr(), cnt,
+                             torch.cuda.current_stream().cuda_stream))
+        return out, [cnt[i] for i in range(n)]
+
+    def step(self, chunks, end=None, reset=None, voice=None):
+        """chunks: one entry per slot 0 .. n-1, each a [1, m] or [m] fp32 CUDA tensor (m <= max_push_samples) or None;
+        end / reset / voice as for GeneratorStream.step.  Returns n [1, m_i] CUDA tensors of newly final denoised audio in
+        the handle's dtype.  Asynchronous on the current stream: the lengths are known on return."""
+        n = len(chunks)
+        if n > self.max_sessions:
+            raise _engine.EngineError("DenoiserStream: %d chunks for %d sessions" % (n, self.max_sessions))
+        counts = []
+        for i, c in enumerate(chunks):
+            if c is None:
+                counts.append(0)
+                continue
+            if not torch.is_tensor(c) or not (c.dim() == 1 or (c.dim() == 2 and c.shape[0] == 1)) \
+                    or c.shape[-1] > self.max_push_samples:
+                raise _engine.EngineError("DenoiserStream: chunk %d must be [1, m] or [m] with m <= %d, got %s"
+                                          % (i, self.max_push_samples, tuple(c.shape) if torch.is_tensor(c) else type(c).__name__))
+            if c.device != self.device or c.dtype != torch.float32:
+                raise _engine.EngineError("DenoiserStream: chunks must be fp32 tensors on %s" % (self.device,))
+            counts.append(int(c.shape[-1]))
+            if counts[-1]:
+                self._in[i, :counts[-1]].copy_(c.reshape(-1))
+        flags = [(_engine.STREAM_END if end is not None and end[i] else 0) | (_engine.STREAM_RESET if reset is not None and reset[i]
+                                                                                else 0) for i in range(n)]
+        out, m = self.step_packed(self._in, counts, flags, voice=voice)
+        return [out[i:i + 1, :k] for i, k in enumerate(m)]
+
+    def close(self):
+        if self._h:
+            _lib().mg_denoise_stream_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
